@@ -475,6 +475,126 @@ void embedding_bag_bwd(const Tensor& dout, const Tensor& ids, Tensor& dtable) {
                          dtable.data_ptr<float>(), ids.size(0), ids.size(1), dtable.size(1), cur_stream());
 }
 
+// ------------------------------------------------------------------ row-sparse embedding bags (embedding.cu)
+inline void check_ids(const Tensor& t, const char* name) {
+  TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor");
+  TORCH_CHECK(t.scalar_type() == at::kLong, name, " must be int64");
+  TORCH_CHECK(t.is_contiguous(), name, " must be contiguous");
+}
+
+// ids [B, L] (offsets None) or [nnz] with offsets [B]; out [B, D]
+void embedding_bag_mean_fwd(const Tensor& table, const Tensor& ids, const c10::optional<Tensor>& offsets, Tensor& out) {
+  check_f32(table, "table");
+  check_f32(out, "out");
+  check_ids(ids, "ids");
+  TORCH_CHECK(table.dim() == 2);
+  const bool csr = offsets.has_value() && offsets->defined();
+  if (csr) check_ids(*offsets, "offsets");
+  TORCH_CHECK(csr ? ids.dim() == 1 : ids.dim() == 2, "ids must be [nnz] with offsets or [B, L] without");
+  const int64_t B = csr ? offsets->numel() : ids.size(0);
+  const int L = csr ? 0 : (int)ids.size(1);
+  const int D = (int)table.size(1);
+  TORCH_CHECK(out.size(0) == B && out.size(1) == D);
+  c10::cuda::CUDAGuard g(table.device());
+  edl::embedding_bag_mean_fwd(table.data_ptr<float>(), ids.data_ptr<int64_t>(), opt_ptr<int64_t>(offsets),
+                              out.data_ptr<float>(), B, ids.numel(), L, D, cur_stream());
+}
+
+void embedding_bag_mean_bwd_sparse(const Tensor& dout, const Tensor& ids, const c10::optional<Tensor>& offsets,
+                                   Tensor& indices, Tensor& values) {
+  check_f32(dout, "dout");
+  check_f32(values, "values");
+  check_ids(ids, "ids");
+  check_ids(indices, "indices");
+  const bool csr = offsets.has_value() && offsets->defined();
+  if (csr) check_ids(*offsets, "offsets");
+  const int64_t B = dout.size(0), nnz = ids.numel();
+  const int D = (int)dout.size(1);
+  TORCH_CHECK(csr ? offsets->numel() == B : ids.size(0) == B);
+  TORCH_CHECK(indices.numel() == nnz && values.numel() == nnz * D);
+  c10::cuda::CUDAGuard g(dout.device());
+  edl::embedding_bag_mean_bwd_sparse(dout.data_ptr<float>(), ids.data_ptr<int64_t>(), opt_ptr<int64_t>(offsets),
+                                     indices.data_ptr<int64_t>(), values.data_ptr<float>(), B, nnz,
+                                     csr ? 0 : (int)ids.size(1), D, cur_stream());
+}
+
+// S slots of fixed-length bags at once: ids [B, S, L], tables[s] [V_s, D] (one entry per slot, repeats allowed)
+void embedding_bags_mean_fwd(const std::vector<Tensor>& tables, const Tensor& ids, Tensor& out) {
+  check_ids(ids, "ids");
+  check_f32(out, "out");
+  TORCH_CHECK(ids.dim() == 3 && (int64_t)tables.size() == ids.size(1) && ids.size(1) <= edl::kMaxSparseTables);
+  const int64_t D = tables[0].size(1);
+  edl::SlotTables tabs{};
+  for (size_t s = 0; s < tables.size(); ++s) {
+    check_f32(tables[s], "table");
+    TORCH_CHECK(tables[s].dim() == 2 && tables[s].size(1) == D, "the tables of one call share their width");
+    tabs.w[s] = tables[s].data_ptr<float>();
+  }
+  TORCH_CHECK(out.numel() == ids.size(0) * ids.size(1) * D);
+  c10::cuda::CUDAGuard g(ids.device());
+  edl::embedding_bags_mean_fwd(ids.data_ptr<int64_t>(), out.data_ptr<float>(), ids.size(0), (int)ids.size(1),
+                               (int)ids.size(2), (int)D, tabs, cur_stream());
+}
+
+void embedding_bags_mean_bwd_sparse(const Tensor& dout, const Tensor& ids, Tensor& indices, Tensor& values) {
+  check_f32(dout, "dout");
+  check_ids(ids, "ids");
+  check_ids(indices, "indices");
+  check_f32(values, "values");
+  TORCH_CHECK(ids.dim() == 3 && dout.dim() == 3 && dout.size(0) == ids.size(0) && dout.size(1) == ids.size(1));
+  const int64_t D = dout.size(2);
+  TORCH_CHECK(indices.numel() == ids.numel() && values.numel() == ids.numel() * D);
+  c10::cuda::CUDAGuard g(ids.device());
+  edl::embedding_bags_mean_bwd_sparse(dout.data_ptr<float>(), ids.data_ptr<int64_t>(), indices.data_ptr<int64_t>(),
+                                      values.data_ptr<float>(), ids.size(0), (int)ids.size(1), (int)ids.size(2),
+                                      (int)D, cur_stream());
+}
+
+// Lazy Adam over the row-sparse gradients (indices[t] [n_t], values[t] [n_t, D]) of tables w[t] [rows_t, D] with
+// moments m[t], v[t]: the gradients are concatenated, keyed by (table, row), stably sorted (the plumbing) and
+// applied by one kernel per kMaxSparseTables tables.
+void sparse_adam(const std::vector<Tensor>& indices, const std::vector<Tensor>& values, std::vector<Tensor> w,
+                 std::vector<Tensor> m, std::vector<Tensor> v, const Tensor& lr, const Tensor& step, double beta1,
+                 double beta2, double eps) {
+  const size_t T = w.size();
+  TORCH_CHECK(T > 0 && T <= (size_t)edl::kMaxSparseTables && indices.size() == T && values.size() == T &&
+              m.size() == T && v.size() == T, "sparse_adam: 1..", edl::kMaxSparseTables, " tables per call");
+  check_f32(lr, "lr");
+  check_f32(step, "step");
+  const int64_t D = w[0].size(1);
+  edl::SparseTables tabs{};
+  tabs.count = (int)T;
+  int64_t n = 0;
+  for (size_t t = 0; t < T; ++t) {
+    check_f32(w[t], "w");
+    check_f32(m[t], "m");
+    check_f32(v[t], "v");
+    TORCH_CHECK(w[t].dim() == 2 && w[t].size(1) == D && m[t].sizes() == w[t].sizes() && v[t].sizes() == w[t].sizes(),
+                "sparse_adam: tables of one call share their width");
+    TORCH_CHECK(w[t].size(0) < (int64_t(1) << 40));
+    TORCH_CHECK(indices[t].scalar_type() == at::kLong && indices[t].dim() == 1 &&
+                values[t].numel() == indices[t].numel() * D);
+    tabs.w[t] = w[t].data_ptr<float>();
+    tabs.m[t] = m[t].data_ptr<float>();
+    tabs.v[t] = v[t].data_ptr<float>();
+    tabs.rows[t] = w[t].size(0);
+    tabs.start[t] = n;
+    n += indices[t].numel();
+  }
+  if (n == 0) return;
+  c10::cuda::CUDAGuard g(w[0].device());
+  const Tensor ids = at::cat(indices).contiguous();
+  std::vector<Tensor> flat;
+  for (const auto& x : values) flat.push_back(x.reshape({-1, D}));
+  const Tensor vals = at::cat(flat).to(at::kFloat).contiguous();
+  Tensor keys = at::empty_like(ids);
+  edl::sparse_adam_keys(ids.data_ptr<int64_t>(), keys.data_ptr<int64_t>(), n, tabs, cur_stream());
+  const auto sorted = at::sort(keys, /*stable=*/true, /*dim=*/0, /*descending=*/false);
+  const Tensor sorted_keys = std::get<0>(sorted).contiguous(), perm = std::get<1>(sorted).contiguous();
+  edl::sparse_adam(sorted_keys.data_ptr<int64_t>(), perm.data_ptr<int64_t>(), vals.data_ptr<float>(), n, (int)D, tabs,
+                   lr.data_ptr<float>(), step.data_ptr<float>(), (float)beta1, (float)beta2, (float)eps, cur_stream());
+}
+
 void normalize_u8(const Tensor& x, Tensor& y, std::vector<double> mean, std::vector<double> stdv,
                   const c10::optional<Tensor>& flip) {
   TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kByte && x.is_contiguous() && x.dim() == 4 && x.size(3) == 3);
@@ -581,6 +701,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("pair_weight_fold", &pair_weight_fold);
   m.def("fold_pair_stats", &fold_pair_stats);
   m.def("embedding_bag_bwd", &embedding_bag_bwd);
+  m.def("embedding_bag_mean_fwd", &embedding_bag_mean_fwd);
+  m.def("embedding_bag_mean_bwd_sparse", &embedding_bag_mean_bwd_sparse);
+  m.def("embedding_bags_mean_fwd", &embedding_bags_mean_fwd);
+  m.def("embedding_bags_mean_bwd_sparse", &embedding_bags_mean_bwd_sparse);
+  m.def("sparse_adam", &sparse_adam);
   m.def("normalize_u8", &normalize_u8);
   m.def("peer_ship", &peer_ship);
   m.def("logit_ship", &logit_ship);

@@ -144,6 +144,39 @@ void embedding_bag_bwd(const void* dout, bool bf16, const int64_t* ids, float* d
 void normalize_u8(const uint8_t* x, void* y, int64_t N, int H, int W, const float* mean,
                   const float* stdv, const uint8_t* flip, cudaStream_t s);
 
+// ---- embedding.cu: row-sparse embedding bags (fp32 tables) ----
+// offsets == nullptr: fixed-length bags [B, L]; else CSR bag starts [B] over ids [nnz] (nn.EmbeddingBag convention)
+void embedding_bag_mean_fwd(const float* table, const int64_t* ids, const int64_t* offsets, float* out, int64_t B,
+                            int64_t nnz, int L, int D, cudaStream_t s);
+// uncoalesced row-sparse gradient: indices [nnz], values [nnz, D]
+void embedding_bag_mean_bwd_sparse(const float* dout, const int64_t* ids, const int64_t* offsets, int64_t* indices,
+                                   float* values, int64_t B, int64_t nnz, int L, int D, cudaStream_t s);
+// the same for S slots of fixed-length bags at once: ids [B, S, L], slot s reads table w[s] (all of width D);
+// out [B, S, D]; backward: indices [S, B * L], values [S, B * L, D] (slot-major)
+constexpr int kMaxSparseTables = 64;
+struct SlotTables {
+  const float* w[kMaxSparseTables];
+};
+void embedding_bags_mean_fwd(const int64_t* ids, float* out, int64_t B, int S, int L, int D, const SlotTables& tabs,
+                             cudaStream_t s);
+void embedding_bags_mean_bwd_sparse(const float* dout, const int64_t* ids, int64_t* indices, float* values, int64_t B,
+                                    int S, int L, int D, cudaStream_t s);
+// lazy Adam over the rows of the row-sparse gradients of up to kMaxSparseTables fp32 tables [rows, D] of one width D
+struct SparseTables {
+  float* w[kMaxSparseTables];
+  float* m[kMaxSparseTables];
+  float* v[kMaxSparseTables];
+  int64_t rows[kMaxSparseTables];
+  int64_t start[kMaxSparseTables];   // first position of table t's rows in the concatenated gradient
+  int count;
+};
+// keys[i] = t << 40 | ids[i] for the concatenated gradient indices (-1: id outside its table)
+void sparse_adam_keys(const int64_t* ids, int64_t* keys, int64_t n, const SparseTables& tabs, cudaStream_t s);
+// sorted_keys / perm: stable sort of the keys; values: the concatenated gradient rows [n, D]
+void sparse_adam(const int64_t* sorted_keys, const int64_t* perm, const float* values, int64_t n, int D,
+                 const SparseTables& tabs, const float* lr, const float* step, float beta1, float beta2, float eps,
+                 cudaStream_t s);
+
 // ---- augment.cu: random-resized crop + flip + normalise from decoded uint8 RGB images of different sizes ----
 struct AugmentItem {   // one per output image; 32 bytes = 8 x int32 (the Python side fills an int32 [N, 8] tensor)
   int64_t offset;      // byte offset of the decoded image (interleaved RGB) inside the pool buffer

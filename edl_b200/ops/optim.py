@@ -186,6 +186,95 @@ class FlatAdam(_FlatOptimizerBase):
                 g.param.copy_(src)
 
 
+class SparseAdam:
+    """Lazy Adam for fp32 tables with row-sparse gradients (``ops.embedding_bag_mean_sparse``; Paddle's ``adam`` with
+    ``lazy_mode=True``).  Only the rows present in a gradient are updated, with FlatAdam's formula
+    ``w -= lr * mhat / (sqrt(vhat) + eps)``; other rows and their ``m`` / ``v`` are not touched.  The bias correction
+    counts ``step()`` calls on a device scalar, so steps never synchronise with the host.  On a GPU the gradients of
+    all tables of one width are keyed by (table, row) and stably sorted, and one kernel (csrc/embedding.cu) sums every
+    run of equal keys in a fixed order and updates that row: the result is deterministic, and every rank that applies
+    the same gathered gradient gets the same tables."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8):
+        self.params = list(params)
+        for p in self.params:
+            if p.dtype != torch.float32 or p.dim() != 2:
+                raise TypeError("SparseAdam: fp32 [V, D] tables only, got %s %s" % (p.dtype, tuple(p.shape)))
+        dev = self.params[0].device if self.params else torch.device("cpu")
+        self.betas, self.eps = (float(betas[0]), float(betas[1])), float(eps)
+        self.lr = float(lr)
+        self.lr_t = torch.full((1,), self.lr, dtype=torch.float32, device=dev)
+        self.step_t = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.state = [{"m": torch.zeros_like(p, dtype=torch.float32), "v": torch.zeros_like(p, dtype=torch.float32)}
+                      for p in self.params]
+
+    def set_lr(self, lr: float):
+        self.lr = float(lr)
+        self.lr_t.fill_(self.lr)
+
+    def zero_grad(self):
+        for p in self.params:
+            p.grad = None
+
+    @torch.no_grad()
+    def step(self):
+        self.step_t += 1
+        todo = []
+        for i, p in enumerate(self.params):
+            if p.grad is None:
+                continue
+            if not p.grad.is_sparse:
+                raise TypeError("SparseAdam: the gradient of a %s table is dense; build the model with "
+                                "sparse_grad=True" % (tuple(p.shape),))
+            todo.append(i)
+        if todo and self.params[0].is_cuda:
+            self._step_cuda(todo)
+        else:
+            for i in todo:
+                self._step_cpu(self.params[i], self.state[i])
+
+    def _step_cuda(self, todo):
+        """One key / sort / update sequence per group of up to 64 tables of one width (csrc/embedding.cu)."""
+        from . import native, count_launch
+
+        groups = {}
+        for i in todo:
+            groups.setdefault(self.params[i].shape[1], []).append(i)
+        for ids in groups.values():
+            for k in range(0, len(ids), 64):
+                chunk = ids[k:k + 64]
+                grads = [self.params[i].grad for i in chunk]
+                native().sparse_adam([g._indices()[0] for g in grads], [g._values() for g in grads],
+                                     [self.params[i].data for i in chunk], [self.state[i]["m"] for i in chunk],
+                                     [self.state[i]["v"] for i in chunk], self.lr_t, self.step_t, self.betas[0],
+                                     self.betas[1], self.eps)
+                count_launch(2)
+
+    def _step_cpu(self, p, st):
+        b1, b2 = self.betas
+        gc = p.grad.double().coalesce()           # repeated rows summed in fp64, like the kernel
+        rows, grad = gc.indices()[0], gc.values().float()
+        m = st["m"][rows].mul_(b1).add_(grad, alpha=1 - b1)
+        v = st["v"][rows].mul_(b2).addcmul_(grad, grad, value=1 - b2)
+        t = float(self.step_t.item())
+        mhat = m / (1 - b1 ** t)
+        vhat = v / (1 - b2 ** t)
+        p.data[rows] = p.data[rows] - self.lr * mhat / (vhat.sqrt() + self.eps)
+        st["m"][rows] = m
+        st["v"][rows] = v
+
+    def state_dict(self):
+        return {"lr": self.lr, "step": self.step_t,
+                "m": [st["m"] for st in self.state], "v": [st["v"] for st in self.state]}
+
+    def load_state_dict(self, sd):
+        self.set_lr(sd["lr"])
+        self.step_t.copy_(sd["step"])
+        for st, m, v in zip(self.state, sd["m"], sd["v"]):
+            st["m"].copy_(m)
+            st["v"].copy_(v)
+
+
 # ---------------------------------------------------------------------------------------------
 # LR schedules (host side; the result is written into the optimizer's device scalar)
 

@@ -22,7 +22,10 @@ Here:
   optimizer kernel multiplies into the gradients -- no extra pass over the gradients;
 * the ranks of a stage meet either through a ``torch.distributed`` group or -- in-place elastic mode on GPUs --
   through a ``Fabric`` (store + rank + world, parallel/symm.py): no process group, no NCCL communicator at all;
-* CPU / gloo groups (the fit_a_line plumbing config) fall back to ``dist.all_reduce``.
+* CPU / gloo groups (the fit_a_line plumbing config) fall back to ``dist.all_reduce``;
+* row-sparse embedding tables (parameters marked ``_edl_sparse``, ``dp.sparse_params``) stay out of the flat buffers:
+  ``finish()`` all-gathers the looked-up rows of their gradients over the library group, so every rank then applies
+  the same deterministic ``ops.SparseAdam`` update to the same rows.
 """
 from __future__ import annotations
 
@@ -34,7 +37,7 @@ from typing import Callable, Dict, List, Optional
 import torch
 import torch.distributed as dist
 
-from .flat import FlatParams
+from .flat import FlatParams, is_sparse_param
 
 
 def _host_id() -> str:
@@ -175,6 +178,9 @@ class ElasticDataParallel:
         self.hierarchical = os.environ.get("EDL_HIERARCHICAL_ALLREDUCE", hierarchical)
         self.overlap_wgrad = os.environ.get("EDL_OVERLAP_WGRAD", "1") == "1"
         self.enabled = True     # False: gradients stay local (DGC exchanges them itself)
+        self.sparse_params = [p for p in module.parameters() if p.requires_grad and is_sparse_param(p)]
+        self.last_sparse_bytes = 0      # bytes of row-sparse gradient this rank contributed to the last exchange
+        self._check_sparse_backend(fabric)
         self._bind_group(group, fabric)
         self.flat = FlatParams(module, grad_alloc=self._grad_alloc if self.pool is not None else None)
         self._plan()
@@ -182,6 +188,12 @@ class ElasticDataParallel:
         self.comm_launches = 0
 
     # ------------------------------------------------------------------ group / memory
+    def _check_sparse_backend(self, fabric):
+        if fabric is not None and self.sparse_params:
+            raise NotImplementedError(
+                "row-sparse embedding tables (sparse_grad=True) need a torch.distributed group: the in-place fabric "
+                "backend does not exchange sparse gradients")
+
     def _bind_group(self, group, fabric=None):
         self.group = group
         self.fabric = fabric
@@ -209,7 +221,7 @@ class ElasticDataParallel:
 
             need = 0
             for p in self.module.parameters():
-                if p.requires_grad:
+                if p.requires_grad and not is_sparse_param(p):
                     # gradients + (fused optimizer) the bf16 parameter shadow every rank stores into
                     need += (p.numel() + 256) * p.element_size() * (2 if p.element_size() == 2 else 1)
             need += 4 << 20
@@ -549,7 +561,72 @@ class ElasticDataParallel:
             for g in self.flat.groups.values():
                 bad = (~torch.isfinite(g.grad).all()).to(torch.int32).view(1)
                 self.found_inf.copy_(torch.maximum(self.found_inf, bad))
+        if self.sparse_params:
+            self._exchange_sparse()
         self._reset_pending()
+
+    # ------------------------------------------------------------------ row-sparse tables
+    @torch.no_grad()
+    def _exchange_sparse(self):
+        """All-gather the row-sparse gradients of ``sparse_params`` (uncoalesced COO: indices [nnz], values
+        [nnz, D]) so every rank ends up with every rank's rows, in rank order, scaled by 1/world with ``average``.
+        Ranks may hold different nnz: one all-gather of the counts, then one of the indices and one of the values of
+        all tables, each padded to the largest rank; the padding is sliced away before the gradient is rebuilt, so
+        it reaches no row.  Reading the counts is the step's one host synchronisation (on more than one rank)."""
+        from ..ops.embedding import sparse_rows
+
+        idxs, vals = [], []
+        for p in self.sparse_params:
+            g = p.grad
+            if g is None:
+                idxs.append(torch.empty(0, dtype=torch.int64, device=p.device))
+                vals.append(torch.empty(0, p.shape[1], dtype=torch.float32, device=p.device))
+            else:
+                if not g.is_sparse:
+                    raise TypeError("the gradient of a sparse table (%s) is dense" % (tuple(p.shape),))
+                idxs.append(g._indices()[0])
+                vals.append(g._values().float())
+        self.last_sparse_bytes = sum(i.numel() * 8 + v.numel() * 4 for i, v in zip(idxs, vals))
+        if self.world <= 1 or not self.enabled:
+            return
+        dev = self.device
+        P, W = len(self.sparse_params), self.world
+        counts = torch.tensor([i.numel() for i in idxs], dtype=torch.int64, device=dev)
+        all_counts = torch.empty(W * P, dtype=torch.int64, device=dev)
+        dist.all_gather_into_tensor(all_counts, counts, group=self.group)
+        cnt = all_counts.view(W, P).tolist()
+        dims = [p.shape[1] for p in self.sparse_params]
+        cap_i = max(sum(c) for c in cnt)
+        cap_v = max(sum(c[j] * dims[j] for j in range(P)) for c in cnt)
+        if cap_i == 0:
+            return
+        send_i = torch.zeros(cap_i, dtype=torch.int64, device=dev)
+        send_v = torch.zeros(cap_v, dtype=torch.float32, device=dev)
+        n_i = sum(i.numel() for i in idxs)
+        n_v = sum(v.numel() for v in vals)
+        if n_i:
+            send_i[:n_i].copy_(torch.cat(idxs))
+            send_v[:n_v].copy_(torch.cat([v.reshape(-1) for v in vals]))
+        recv_i = torch.empty(W * cap_i, dtype=torch.int64, device=dev)
+        recv_v = torch.empty(W * cap_v, dtype=torch.float32, device=dev)
+        dist.all_gather_into_tensor(recv_i, send_i, group=self.group)
+        dist.all_gather_into_tensor(recv_v, send_v, group=self.group)
+        scale = 1.0 / W if self.average else 1.0
+        pos_i = [r * cap_i for r in range(W)]
+        pos_v = [r * cap_v for r in range(W)]
+        for j, p in enumerate(self.sparse_params):
+            pi, pv = [], []
+            for r in range(W):
+                c = cnt[r][j]
+                pi.append(recv_i[pos_i[r]:pos_i[r] + c])
+                pv.append(recv_v[pos_v[r]:pos_v[r] + c * dims[j]])
+                pos_i[r] += c
+                pos_v[r] += c * dims[j]
+            ind = torch.cat(pi)
+            val = torch.cat(pv).view(-1, dims[j])
+            if scale != 1.0:
+                val.mul_(scale)
+            p.grad = sparse_rows(ind, val, p.shape)
 
     # ------------------------------------------------------------------ global-norm clipping (SURVEY K9)
     def _launch_clip(self):
@@ -696,8 +773,12 @@ class ElasticDataParallel:
             if self.sqnorm is not None:
                 self.sqnorm.zero_()
             self.last_algos = []
+            for p in self.sparse_params:
+                p.grad = None
             return
         self.flat.zero_grad()
+        for p in self.sparse_params:
+            p.grad = None
         if self.found_inf is not None:
             self.found_inf.zero_()
         if self.sqnorm is not None:
@@ -754,6 +835,7 @@ class ElasticDataParallel:
             raise RuntimeError("the optimizer state is sharded across the ranks of the old stage: call "
                                "consolidate_optimizer_state() (planned change, collective over the OLD stage) or "
                                "localize_optimizer_state() (a peer died) before rebuild()")
+        self._check_sparse_backend(fabric)
         for h in self._hook_handles:
             h.remove()
         old_pool = self.pool
@@ -801,6 +883,8 @@ class ElasticDataParallel:
                                group=self.group)
                 if g.master is not None:
                     g.param.copy_(g.master.to(g.param.dtype))
+        for p in self.sparse_params:
+            self.broadcast_tensor(p.data, root)
 
     @torch.no_grad()
     def broadcast_tensor(self, t: torch.Tensor, root: int = 0):

@@ -46,16 +46,24 @@ def _round_up(n: int, m: int) -> int:
     return (n + m - 1) // m * m
 
 
+def is_sparse_param(p: torch.Tensor) -> bool:
+    """A table whose gradient is row-sparse (``ops.embedding_bag_mean_sparse``; models mark it ``_edl_sparse``)."""
+    return bool(getattr(p, "_edl_sparse", False))
+
+
 class FlatParams:
     """Re-home ``module``'s trainable parameters into flat per-dtype buffers.
 
     ``grad_alloc(numel, dtype, device) -> Tensor`` lets the caller provide gradient storage (e.g.
     a slice of symmetric memory); ``pad_multiple`` pads each group so it can be split evenly across
-    ranks by the two-shot all-reduce."""
+    ranks by the two-shot all-reduce.
+
+    Parameters marked ``_edl_sparse`` (row-sparse embedding tables, see ``is_sparse_param``) keep their own storage and
+    sparse gradients: they are left out of the flat buffers."""
 
     def __init__(self, module: torch.nn.Module, grad_alloc: Optional[Callable] = None,
                  pad_multiple: int = 8 * 16 * 8, reverse: bool = True, direct_sinks: bool = True):
-        named = [(n, p) for n, p in module.named_parameters() if p.requires_grad]
+        named = [(n, p) for n, p in module.named_parameters() if p.requires_grad and not is_sparse_param(p)]
         if reverse:
             named = named[::-1]
         if not named:

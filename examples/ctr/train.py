@@ -8,7 +8,11 @@ Here the model trains on GPUs with the embedding tables replicated and their (de
 all-reduced by the fused NVSwitch kernels like any other parameter (26 x 40 MB fp32 = 1.04 GB per
 step at the reference's table size -- the "embedding all-reduce bandwidth sweep").
 
+With ``--sparse`` the tables are row-sparse instead (``sparse_grad=True``, the reference's ``is_sparse=True``): a
+step only exchanges and updates the rows its batch looked up (all-gathered, ``ops.SparseAdam``).
+
     python examples/ctr/train.py --steps 20                    # 1 GPU / CPU smoke
+    python examples/ctr/train.py --sparse --vocab 1000001      # row-sparse tables at the reference's size
     torchrun --nproc-per-node 8 examples/ctr/train.py --sweep  # all-reduce bus bandwidth vs message size
 """
 import argparse
@@ -78,6 +82,7 @@ def main():
     ap.add_argument("--lr", type=float, default=1e-4)
     ap.add_argument("--model", default="ctr_dnn", choices=["ctr_dnn", "deepfm"])
     ap.add_argument("--sweep", action="store_true")
+    ap.add_argument("--sparse", action="store_true", help="row-sparse embedding gradients + lazy Adam on the tables")
     ap.add_argument("--out", default="")
     ap.add_argument("--save", default="", help="rank 0 writes the trained model's state dict here (input of dumper.py)")
     args = ap.parse_args()
@@ -96,9 +101,11 @@ def main():
         result["sweep"] = sweep(dev, world, rank)
     else:
         torch.manual_seed(0)
-        model = (DeepFM if args.model == "deepfm" else CtrDnn)(sparse_feature_dim=args.vocab).to(dev)
+        model = (DeepFM if args.model == "deepfm" else CtrDnn)(sparse_feature_dim=args.vocab,
+                                                                sparse_grad=args.sparse).to(dev)
         dp = ElasticDataParallel(model, bucket_cap_mb=64)
         opt = ops.FlatAdam(dp.flat, lr=args.lr)
+        sparse_opt = ops.SparseAdam(dp.sparse_params, lr=args.lr) if args.sparse else None
         gen = torch.Generator(device=dev).manual_seed(100 + rank)
         scores, labels = [], []
         t0 = time.time()
@@ -110,6 +117,8 @@ def main():
             loss.backward()
             dp.finish()
             opt.step()
+            if sparse_opt is not None:
+                sparse_opt.step()
             scores.append(torch.softmax(logits.detach().float(), -1)[:, 1])
             labels.append(label)
             if step % 10 == 0 and rank == 0:
@@ -119,6 +128,8 @@ def main():
             torch.cuda.synchronize()
         result["examples_per_s"] = args.batch * world * args.steps / (time.time() - t0)
         result["grad_bytes_per_step"] = sum(g.grad.numel() * g.grad.element_size() for g in dp.flat.groups.values())
+        if args.sparse:
+            result["grad_bytes_per_step"] += dp.last_sparse_bytes     # indices + values this rank sent last step
         if rank == 0:
             print(json.dumps(result))
             if args.save:
