@@ -162,11 +162,21 @@ struct GemmFp8Args {
   const float* col_shift = nullptr;
   bool relu = false;
   int device = -1;
+  // gemm_fp8_blockscaled only: a_scales fp32 [ceil(K/128), M], b_scales fp32 [ceil(N/128), ceil(K/128)]
+  const float* a_scales = nullptr;
+  const float* b_scales = nullptr;
 };
 const char* gemm_fp8(const GemmFp8Args& args, cudaStream_t stream);
+// D[M,N] bf16 = relu?((sum_b (A_b * B_b^T) * a_scales[b, m] * b_scales[n / 128, b]) * col_scale[n] + col_shift[n])
+// over the 128-element K blocks b; col_scale carries only the folded BN scale here.
+const char* gemm_fp8_blockscaled(const GemmFp8Args& args, cudaStream_t stream);
 
 // bf16 -> e4m3 with a per-tensor scale (q = sat(x / scale)); amax_out (optional) receives max|x| for
 // calibration / delayed scaling.
 void quantize_e4m3(const void* x_bf16, void* q, int64_t n, const float* scale, float* amax_out, cudaStream_t s);
+
+// bf16 [M, K] (row pitch lda elements) -> e4m3 q [M, K] (contiguous) and fp32 sa [ceil(K/128), M]: per row and
+// 128-element K block, s = max|x| / 448 (1 when the block is all zero) and q = sat(x / s).  K % 8 == 0.
+const char* quantize_e4m3_blocks(const void* x_bf16, int64_t lda, void* q, float* sa, int M, int K, cudaStream_t s);
 
 }  // namespace edl

@@ -242,6 +242,69 @@ void quantize_e4m3(const Tensor& x, Tensor& q, const Tensor& scale, const c10::o
                      at::cuda::getCurrentCUDAStream().stream());
 }
 
+// q [M, K] e4m3 bytes (contiguous), sa fp32 [ceil(K/128), M] = per-row, per-128-element-block scales of x [M, K]
+void quantize_e4m3_blocks(const Tensor& x, Tensor& q, Tensor& sa) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.scalar_type() == at::kBFloat16, "x must be a 2-D bf16 CUDA tensor");
+  TORCH_CHECK(x.stride(1) == 1, "x needs a contiguous last dim");
+  const int64_t M = x.size(0), K = x.size(1), kb = (K + 127) / 128;
+  TORCH_CHECK(M > 0 && K > 0 && K % 8 == 0, "block quantiser needs K % 8 == 0, got K = ", K);
+  TORCH_CHECK(x.stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0,
+              "x rows must be 16-byte aligned");
+  TORCH_CHECK(q.is_cuda() && q.element_size() == 1 && q.is_contiguous() && q.dim() == 2 && q.size(0) == M &&
+              q.size(1) == K, "q must be a contiguous 1-byte [M, K] tensor");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(q.data_ptr()) % 8 == 0, "q must be 8-byte aligned");
+  TORCH_CHECK(sa.is_cuda() && sa.scalar_type() == at::kFloat && sa.is_contiguous() && sa.dim() == 2 &&
+              sa.size(0) == kb && sa.size(1) == M, "sa must be contiguous fp32 [ceil(K/128), M]");
+  TORCH_CHECK(x.device() == q.device() && x.device() == sa.device(), "tensors on different devices");
+  c10::cuda::CUDAGuard guard(x.device());
+  const char* err = edl::quantize_e4m3_blocks(x.data_ptr(), x.stride(0), q.data_ptr(), sa.data_ptr<float>(), (int)M,
+                                              (int)K, at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl quantize_e4m3_blocks failed: ", err);
+}
+
+// D bf16 [M,N] = relu?((sum_b (A8_b * B8_b^T) * sa[b, m] * sb[n / 128, b]) * col_scale + col_shift)
+void gemm_fp8_blockscaled(const Tensor& A, const Tensor& sa, const Tensor& B, const Tensor& sb, Tensor& D,
+                          const c10::optional<Tensor>& col_scale, const c10::optional<Tensor>& col_shift, bool relu) {
+  TORCH_CHECK(A.is_cuda() && B.is_cuda() && D.is_cuda() && A.dim() == 2 && B.dim() == 2 && D.dim() == 2);
+  TORCH_CHECK(A.element_size() == 1 && B.element_size() == 1, "A and B hold e4m3 bytes");
+  TORCH_CHECK(D.scalar_type() == at::kBFloat16, "D must be bf16");
+  TORCH_CHECK(A.stride(1) == 1 && B.stride(1) == 1 && D.stride(1) == 1, "operands need a contiguous last dim");
+  TORCH_CHECK(A.size(1) == B.size(1), "K mismatch: ", A.size(1), " vs ", B.size(1));
+  TORCH_CHECK(D.size(0) == A.size(0) && D.size(1) == B.size(0), "D must be [M, N]");
+  const int64_t M = A.size(0), N = B.size(0), K = A.size(1), kb = (K + 127) / 128;
+  TORCH_CHECK(K % 16 == 0 && A.stride(0) % 16 == 0 && B.stride(0) % 16 == 0 && D.stride(0) % 8 == 0,
+              "fp8 GEMM needs 16-byte aligned rows");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(A.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(B.data_ptr()) % 16 == 0 &&
+              reinterpret_cast<uintptr_t>(D.data_ptr()) % 16 == 0, "A, B and D must be 16-byte aligned");
+  TORCH_CHECK(sa.is_cuda() && sa.scalar_type() == at::kFloat && sa.is_contiguous() && sa.dim() == 2 &&
+              sa.size(0) == kb && sa.size(1) == M, "sa must be contiguous fp32 [ceil(K/128), M]");
+  TORCH_CHECK(sb.is_cuda() && sb.scalar_type() == at::kFloat && sb.is_contiguous() && sb.dim() == 2 &&
+              sb.size(0) == (N + 127) / 128 && sb.size(1) == kb, "sb must be contiguous fp32 [ceil(N/128), ceil(K/128)]");
+  for (const auto* t : {&col_scale, &col_shift})
+    if (t->has_value() && (*t)->defined())
+      TORCH_CHECK((*t)->is_cuda() && (*t)->scalar_type() == at::kFloat && (*t)->is_contiguous() && (*t)->numel() == N,
+                  "col_scale / col_shift must be contiguous fp32 [N]");
+  edl::GemmFp8Args g;
+  g.A = A.data_ptr();
+  g.B = B.data_ptr();
+  g.D = D.data_ptr();
+  g.M = M;
+  g.K = K;
+  g.N = N;
+  g.lda = A.stride(0);
+  g.ldb = B.stride(0);
+  g.ldd = D.stride(0);
+  g.col_scale = optp<float>(col_scale);
+  g.col_shift = optp<float>(col_shift);
+  g.relu = relu;
+  g.a_scales = sa.data_ptr<float>();
+  g.b_scales = sb.data_ptr<float>();
+  g.device = A.device().index();
+  c10::cuda::CUDAGuard guard(A.device());
+  const char* err = edl::gemm_fp8_blockscaled(g, at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl gemm_fp8_blockscaled failed: ", err);
+}
+
 bool conv3x3_supported(int64_t n, int64_t h, int64_t w, int64_t cin, int64_t cout, bool dgrad, int64_t groups) {
   return edl::conv3x3_supported((int)n, (int)h, (int)w, (int)cin, (int)cout, dgrad, (int)groups);
 }
@@ -371,6 +434,8 @@ void register_gemm_bindings(pybind11::module_& m) {
   m.def("persistent_gemm_enabled", &edl::persistent_gemm_enabled);
   m.def("gemm_fp8", &gemm_fp8);
   m.def("quantize_e4m3", &quantize_e4m3);
+  m.def("gemm_fp8_blockscaled", &gemm_fp8_blockscaled);
+  m.def("quantize_e4m3_blocks", &quantize_e4m3_blocks);
   m.def("conv3x3_supported", &conv3x3_supported);
   m.def("conv3x3_infer", &conv3x3_infer);
   m.def("gemm_bf16_ship", &gemm_bf16_ship);

@@ -4,10 +4,16 @@
 // warps 4..11 two consumer warpgroups that issue the MMAs of their 64 rows and then run the
 // epilogue (dequantisation scale * folded-BN scale, shift, ReLU, bf16, swizzled staging, TMA store).
 // A K block is 128 fp8 = one 128-byte swizzle span, so the shared-memory geometry and the operand
-// descriptors are those of the bf16 kernel.  Also hosts the bf16 -> e4m3 quantiser.
+// descriptors are those of the bf16 kernel.  Also hosts the bf16 -> e4m3 quantisers.
+//
+// Two scalings share the kernel: per-tensor (one activation scale, per-output-channel weight scales, all
+// folded into col_scale) and block-scaled (an fp32 scale per activation row and 128-element K block, one
+// per 128x128 weight block, applied per k-block in the main loop: see Fp8BlockParams).
 #include <cuda.h>
 #include <cuda_fp8.h>
+#include <cstdint>
 #include <cstdio>
+#include <type_traits>
 
 #include "gemm.h"
 #include "kernels.h"
@@ -28,6 +34,13 @@ struct Fp8Params {
   int relu;
 };
 
+// Block-scaled variant: sa fp32 [KB, M] (one scale per row and 128-element K block, K-block-major so that a
+// k-block's scales for a tile's rows are contiguous), sb fp32 [ceil(N/128), KB] (one per 128x128 weight block).
+struct Fp8BlockParams : Fp8Params {
+  const float* sa;
+  const float* sb;
+};
+
 template <int BLOCK_N, int STAGES>
 struct Smem {
   static constexpr int kABytes = kBlockM * kBlockKBytes;
@@ -39,10 +52,11 @@ struct Smem {
   static constexpr int kTotal = kTileBytes + 256 + 1024;
 };
 
-template <int BLOCK_N, int STAGES>
+template <int BLOCK_N, int STAGES, typename P>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_fp8_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                        const __grid_constant__ CUtensorMap tmD, const Fp8Params p) {
+                        const __grid_constant__ CUtensorMap tmD, const P p) {
+  constexpr bool kBlockScaled = std::is_same<P, Fp8BlockParams>::value;
   using L = Smem<BLOCK_N, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -90,22 +104,61 @@ gemm_fp8_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     const int row = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // first accumulator row of this thread (second: + 8)
     const int cq = (lane & 3) * 2;
     float acc[BLOCK_N / 2];
-    for (int i = 0; i < num_kb; ++i) {
-      const int s = i % STAGES;
-      ptx::mbar_wait(&full_bar[s], (i / STAGES) & 1);
-      const uint32_t sa = ptx::smem_u32(smem + s * L::kStageBytes);
-      const uint64_t da0 = ptx::make_smem_desc(sa + cw * 8192, 16, 1024);
-      const uint64_t db0 = ptx::make_smem_desc(sa + L::kABytes, 16, 1024);
-      ptx::wgmma_fence();
+    if constexpr (kBlockScaled) {
+      // Per k-block: the 4 MMAs go into tmp (scale-d = 0 on the first), then tmp is promoted into acc with
+      // this block's row scale * weight-block scale.  The scale loads are issued before the full-barrier wait
+      // and first read after the MMAs, so their latency hides behind both.  Rows past M read scale 0 (their
+      // stores are clipped); a tile's BLOCK_N <= 128 columns lie in one 128-row weight block.
+      float tmp[BLOCK_N / 2];
 #pragma unroll
-      for (int k = 0; k < kBlockKBytes / kMmaKBytes; ++k)     // start-address field counts 16-byte units
-        ptx::WgmmaE4m3<BLOCK_N>::mma(acc, da0 + (uint64_t)(k * (kMmaKBytes >> 4)), db0 + (uint64_t)(k * (kMmaKBytes >> 4)),
-                                     (i | k) != 0 ? 1u : 0u);
-      ptx::wgmma_commit();
-      ptx::wgmma_wait<1>();
-      if (i > 0 && (threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+      for (int j = 0; j < BLOCK_N / 2; ++j) acc[j] = 0.f;
+      const int r0 = m0 + row, r1 = m0 + row + 8;
+      const float* sb_tile = p.sb + (size_t)(n0 / 128) * num_kb;
+      for (int i = 0; i < num_kb; ++i) {
+        const int s = i % STAGES;
+        const float* sa_kb = p.sa + (size_t)i * p.M;
+        const float sbk = __ldg(sb_tile + i);
+        const float sa0 = r0 < p.M ? __ldg(sa_kb + r0) : 0.f;
+        const float sa1 = r1 < p.M ? __ldg(sa_kb + r1) : 0.f;
+        ptx::mbar_wait(&full_bar[s], (i / STAGES) & 1);
+        const uint32_t sa = ptx::smem_u32(smem + s * L::kStageBytes);
+        const uint64_t da0 = ptx::make_smem_desc(sa + cw * 8192, 16, 1024);
+        const uint64_t db0 = ptx::make_smem_desc(sa + L::kABytes, 16, 1024);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockKBytes / kMmaKBytes; ++k)
+          ptx::WgmmaE4m3<BLOCK_N>::mma(tmp, da0 + (uint64_t)(k * (kMmaKBytes >> 4)), db0 + (uint64_t)(k * (kMmaKBytes >> 4)),
+                                       k != 0 ? 1u : 0u);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        if ((threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty_bar[s]);
+        const float f0 = sa0 * sbk, f1 = sa1 * sbk;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          acc[4 * j] = fmaf(tmp[4 * j], f0, acc[4 * j]);
+          acc[4 * j + 1] = fmaf(tmp[4 * j + 1], f0, acc[4 * j + 1]);
+          acc[4 * j + 2] = fmaf(tmp[4 * j + 2], f1, acc[4 * j + 2]);
+          acc[4 * j + 3] = fmaf(tmp[4 * j + 3], f1, acc[4 * j + 3]);
+        }
+      }
+    } else {
+      for (int i = 0; i < num_kb; ++i) {
+        const int s = i % STAGES;
+        ptx::mbar_wait(&full_bar[s], (i / STAGES) & 1);
+        const uint32_t sa = ptx::smem_u32(smem + s * L::kStageBytes);
+        const uint64_t da0 = ptx::make_smem_desc(sa + cw * 8192, 16, 1024);
+        const uint64_t db0 = ptx::make_smem_desc(sa + L::kABytes, 16, 1024);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockKBytes / kMmaKBytes; ++k)     // start-address field counts 16-byte units
+          ptx::WgmmaE4m3<BLOCK_N>::mma(acc, da0 + (uint64_t)(k * (kMmaKBytes >> 4)), db0 + (uint64_t)(k * (kMmaKBytes >> 4)),
+                                       (i | k) != 0 ? 1u : 0u);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<1>();
+        if (i > 0 && (threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+      }
+      ptx::wgmma_wait<0>();
     }
-    ptx::wgmma_wait<0>();
     asm volatile("bar.sync 1, 256;" ::: "memory");       // the ring is drained: it becomes the staging tile
     uint8_t* sd = smem;
 #pragma unroll
@@ -134,7 +187,7 @@ gemm_fp8_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   }
 }
 
-template <int BLOCK_N, int STAGES>
+template <int BLOCK_N, int STAGES, typename P>
 const char* launch(const GemmFp8Args& g, cudaStream_t stream) {
   using L = Smem<BLOCK_N, STAGES>;
   alignas(64) CUtensorMap tmA, tmB, tmD;
@@ -156,7 +209,7 @@ const char* launch(const GemmFp8Args& g, cudaStream_t stream) {
     const uint32_t box[2] = {64, kBlockM};
     if (const char* e = encode_tmap(&tmD, g.D, 2, dims, st, box, 2)) return e;
   }
-  auto kern = gemm_fp8_wgmma_kernel<BLOCK_N, STAGES>;
+  auto kern = gemm_fp8_wgmma_kernel<BLOCK_N, STAGES, P>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal);
@@ -164,7 +217,17 @@ const char* launch(const GemmFp8Args& g, cudaStream_t stream) {
     apply_carveout((const void*)kern);
     attr_set = true;
   }
-  Fp8Params p{g.M, g.N, g.K, g.col_scale, g.col_shift, g.relu ? 1 : 0};
+  P p{};
+  p.M = g.M;
+  p.N = g.N;
+  p.K = g.K;
+  p.col_scale = g.col_scale;
+  p.col_shift = g.col_shift;
+  p.relu = g.relu ? 1 : 0;
+  if constexpr (std::is_same<P, Fp8BlockParams>::value) {
+    p.sa = g.a_scales;
+    p.sb = g.b_scales;
+  }
   const int tiles = ((g.M + kBlockM - 1) / kBlockM) * ((g.N + BLOCK_N - 1) / BLOCK_N);
   kern<<<tiles, kThreads, L::kTotal, stream>>>(tmA, tmB, tmD, p);
   cudaError_t e = cudaGetLastError();
@@ -201,16 +264,79 @@ quantize_e4m3_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ 
   }
 }
 
-}  // namespace
+// Row-block quantiser: one half-warp per (row m, 128-element K block b).  Each lane loads 8 bf16 (16 bytes),
+// the block's max|x| is reduced with shuffles across the 16 lanes that share it, s = amax / 448 (1 for an
+// all-zero block) goes to sa[b, m], and every lane stores its 8 bytes sat(x / s).  K % 8 == 0, so a lane's
+// 8 elements are either all inside the (possibly shorter) tail block or all past K.
+__global__ void __launch_bounds__(256)
+quantize_e4m3_blocks_kernel(const __nv_bfloat16* __restrict__ x, int64_t lda, uint8_t* __restrict__ q,
+                            float* __restrict__ sa, int M, int K) {
+  const int kbs = (K + kBlockKBytes - 1) / kBlockKBytes;
+  const int segs = M * kbs;
+  const int hl = threadIdx.x & 15;
+  const unsigned mask = 0xffffu << (threadIdx.x & 16);   // the 16 lanes of this half-warp
+  for (int seg = blockIdx.x * 16 + (threadIdx.x >> 4); seg < segs; seg += gridDim.x * 16) {
+    const int m = seg / kbs, b = seg - m * kbs;
+    const int k = b * kBlockKBytes + hl * 8;
+    const bool live = k < K;
+    float f[8];
+    if (live) {
+      unpack8(ld_vec(x + (int64_t)m * lda + k), f);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] = 0.f;
+    }
+    float amax = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(f[j]));
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(mask, amax, o));
+    const float s = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+    if (hl == 0) sa[(int64_t)b * M + m] = s;
+    if (live) {
+      uint8_t o[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        o[j] = (uint8_t)__nv_cvt_float_to_fp8(__fdiv_rn(f[j], s), __NV_SATFINITE, __NV_E4M3);
+      *reinterpret_cast<uint2*>(q + (int64_t)m * K + k) = *reinterpret_cast<const uint2*>(o);
+    }
+  }
+}
 
-const char* gemm_fp8(const GemmFp8Args& g, cudaStream_t stream) {
+const char* check_fp8_args(const GemmFp8Args& g) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return "empty GEMM";
   if (g.K % 16 != 0 || g.lda % 16 != 0 || g.ldb % 16 != 0 || g.ldd % 8 != 0) return "fp8 GEMM needs 16-byte aligned rows";
   if (g.device >= 0) {
     cudaError_t e = cudaSetDevice(g.device);
     if (e != cudaSuccess) return cudaGetErrorString(e);
   }
-  return g.N <= 64 ? launch<64, 4>(g, stream) : launch<128, 3>(g, stream);
+  return nullptr;
+}
+
+}  // namespace
+
+const char* gemm_fp8(const GemmFp8Args& g, cudaStream_t stream) {
+  if (const char* e = check_fp8_args(g)) return e;
+  return g.N <= 64 ? launch<64, 4, Fp8Params>(g, stream) : launch<128, 3, Fp8Params>(g, stream);
+}
+
+const char* gemm_fp8_blockscaled(const GemmFp8Args& g, cudaStream_t stream) {
+  if (g.a_scales == nullptr || g.b_scales == nullptr) return "block-scaled fp8 GEMM needs both scale tensors";
+  if (const char* e = check_fp8_args(g)) return e;
+  return g.N <= 64 ? launch<64, 4, Fp8BlockParams>(g, stream) : launch<128, 3, Fp8BlockParams>(g, stream);
+}
+
+const char* quantize_e4m3_blocks(const void* x, int64_t lda, void* q, float* sa, int M, int K, cudaStream_t s) {
+  if (M <= 0 || K <= 0) return "empty input";
+  if (K % 8 != 0 || lda % 8 != 0) return "block quantiser needs 16-byte aligned rows";
+  const int64_t segs = (int64_t)M * ((K + kBlockKBytes - 1) / kBlockKBytes);
+  if (segs > INT32_MAX / 2) return "block quantiser: too many blocks";
+  int64_t blocks = (segs + 15) / 16;
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
+  quantize_e4m3_blocks_kernel<<<(int)blocks, 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(x), lda,
+                                                          reinterpret_cast<uint8_t*>(q), sa, M, K);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
 void quantize_e4m3(const void* x, void* q, int64_t n, const float* scale, float* amax_out, cudaStream_t s) {

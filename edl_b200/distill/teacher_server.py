@@ -162,7 +162,10 @@ def main(argv=None):
     ap.add_argument("--thread", type=int, default=4)
     ap.add_argument("--max_batch", type=int, default=64)
     ap.add_argument("--mem_optim", action="store_true", help="accepted for CLI parity; no-op")
-    ap.add_argument("--fp8", action="store_true", help="e4m3 wgmma GEMMs for the 1x1 convolutions (calibrated on random data)")
+    ap.add_argument("--fp8", action="store_true", help="e4m3 wgmma GEMMs for the 1x1 convolutions")
+    ap.add_argument("--fp8_scaling", choices=("tensor", "block"), default="tensor",
+                    help="with --fp8: 'tensor' = one activation scale per layer, calibrated on random data; 'block' = "
+                         "per-row, per-128-channel activation scales computed as each layer runs (no calibration)")
     args = ap.parse_args(argv)
     logging.basicConfig(level=logging.INFO)
     dev = "cuda:%s" % args.gpu_ids.split(",")[0] if torch.cuda.is_available() else "cpu"
@@ -171,7 +174,9 @@ def main(argv=None):
     srv = TeacherServer(model, feed_names, fetch_names, feed_shapes, device=dev, dtype=dtype, port=args.port,
                         max_batch=args.max_batch, workers=max(4, args.thread))
     net = getattr(srv.model, "net", srv.model)
-    if args.fp8 and dev.startswith("cuda") and hasattr(net, "enable_fp8"):
+    if args.fp8 and dev.startswith("cuda") and hasattr(net, "enable_fp8") and args.fp8_scaling == "block":
+        logging.info("fp8 (block-scaled): converted %d layers", net.enable_fp8(scaling="block"))
+    elif args.fp8 and dev.startswith("cuda") and hasattr(net, "enable_fp8"):
         shape = feed_shapes[feed_names[0]]
         calib = torch.randn(8, *shape, device=dev).to(dtype).contiguous(memory_format=torch.channels_last)
         logging.info("fp8: converted %d layers", net.enable_fp8(calib))

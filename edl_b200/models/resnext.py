@@ -14,7 +14,7 @@ layer is  conv -> *scale + shift (+ residual) -> ReLU :
 """
 import math
 import os
-from typing import List
+from typing import List, Optional
 
 import torch
 import torch.nn as nn
@@ -98,6 +98,18 @@ class FoldedConv(nn.Module):
         self._ones, self._zeros = torch.ones_like(self.scale), torch.zeros_like(self.scale)
         return True
 
+    def enable_fp8_blocks(self):
+        """Block-scaled fp8: quantise the weights once per 128x128 block; the input is scaled per row and 128-channel
+        block when the layer runs, so there is nothing to calibrate and no host synchronisation."""
+        from ..ops.fp8 import quantize_weight_blocks
+
+        if not self.fp8_eligible():
+            return False
+        self.w8 = None                                      # leaves the per-tensor mode
+        self.w8_blocks, self.w_block_scales = quantize_weight_blocks(self.weight.view(self.cout, self.cin))
+        self._ones, self._zeros = torch.ones_like(self.scale), torch.zeros_like(self.scale)
+        return True
+
     def forward(self, x, residual=None):
         fast = (x.is_cuda and x.dtype == torch.bfloat16 and self.k == 1 and self.groups == 1
                 and self.cin % 8 == 0 and self.cout % 8 == 0)
@@ -110,6 +122,16 @@ class FoldedConv(nn.Module):
             x2 = x.permute(0, 2, 3, 1).reshape(-1, c)
             y = torch.empty((n, self.cout, h, w), device=x.device, dtype=x.dtype, memory_format=torch.channels_last)
             y2 = y.permute(0, 2, 3, 1).reshape(-1, self.cout)
+            if getattr(self, "w8_blocks", None) is not None:
+                from ..ops.fp8 import gemm_fp8_blockscaled, quantize_e4m3_blocks
+
+                x8, sa = quantize_e4m3_blocks(x2)
+                w8, sb = self.w8_blocks, self.w_block_scales
+                if residual is None:
+                    gemm_fp8_blockscaled(x8, sa, w8, sb, self.scale, self.shift, self.relu, out=y2)
+                    return y
+                gemm_fp8_blockscaled(x8, sa, w8, sb, self.scale, self.shift, False, out=y2)
+                return ops.scale_shift_act(y, self._ones, self._zeros, residual, self.relu)
             if getattr(self, "w8", None) is not None:
                 from ..ops.fp8 import gemm_fp8, quantize_e4m3
 
@@ -208,10 +230,21 @@ class ResNeXt(nn.Module):
         nn.init.uniform_(self.fc_weight, -1.0 / math.sqrt(cin), 1.0 / math.sqrt(cin))
 
     @torch.no_grad()
-    def enable_fp8(self, calib_batch: torch.Tensor, margin: float = 1.0) -> int:
-        """Calibrate activation ranges on ``calib_batch`` (one bf16 forward) and switch every eligible 1x1
-        convolution to the e4m3 wgmma GEMM.  Returns the number of converted layers."""
+    def enable_fp8(self, calib_batch: Optional[torch.Tensor] = None, margin: float = 1.0, scaling: str = "tensor") -> int:
+        """Switch every eligible 1x1 convolution to the e4m3 wgmma GEMM.  Returns the number of converted layers.
+
+        ``scaling="tensor"``: calibrate one activation scale per layer on ``calib_batch`` (one bf16 forward).
+        ``scaling="block"``: per-128-channel-block activation scales computed from each block's own max|x| when
+        the layer runs, per-128x128-block weight scales; needs no batch, runs no forward and never syncs."""
         convs = [m for m in self.modules() if isinstance(m, FoldedConv)]
+        if scaling == "block":
+            return sum(1 for c in convs if c.enable_fp8_blocks())
+        if scaling != "tensor":
+            raise ValueError("enable_fp8: scaling must be 'tensor' or 'block', got %r" % (scaling,))
+        if calib_batch is None:
+            raise ValueError("enable_fp8(scaling='tensor') needs a calibration batch")
+        for c in convs:
+            c.w8_blocks = None                              # leaves the block-scaled mode
         for c in convs:
             c.begin_calibration()
         self.forward_features(calib_batch)

@@ -39,6 +39,9 @@ def main():
     ap.add_argument("--temperature", type=float, default=1.0)
     ap.add_argument("--teacher_ckpt", default=None)
     ap.add_argument("--teacher_fp8", type=int, default=0)
+    ap.add_argument("--teacher_fp8_scaling", choices=("tensor", "block"), default="tensor",
+                    help="'tensor': one activation scale per layer from a random calibration batch; 'block': per-row, "
+                         "per-128-channel scales computed as each layer runs (no calibration)")
     ap.add_argument("--checkpoint", default="./distill_link_ckpt")
     ap.add_argument("--fetch_steps", type=int, default=10)
     args = ap.parse_args()
@@ -65,7 +68,9 @@ def main():
         if args.teacher_ckpt:
             tm.load_state_dict(torch.load(args.teacher_ckpt, map_location="cpu"))
         tm = to_inference_dtype(tm, torch.bfloat16, dev).eval()
-        if args.teacher_fp8:
+        if args.teacher_fp8 and args.teacher_fp8_scaling == "block":
+            tm.enable_fp8(scaling="block")
+        elif args.teacher_fp8:
             calib = torch.randn(B, 3, 224, 224, device=dev).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
             tm.enable_fp8(calib)
         worker = TeacherWorker(tm, link)
