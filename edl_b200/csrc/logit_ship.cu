@@ -68,9 +68,12 @@ peer_ship_kernel(const int4* __restrict__ src, int4* __restrict__ dst_peer, int6
 }
 
 // One block per row: ship the logits row to the peer slot, compute (max, lse) at temperature T.
+// `vec` (decided on the host): every row of source and slot starts on a 16-byte boundary, so the
+// copy moves 8 logits per 128-bit access; otherwise (C % 8 != 0, or an unaligned base) it goes
+// element by element.
 __global__ void __launch_bounds__(kRowThreads)
 logit_ship_kernel(const __nv_bfloat16* __restrict__ logits, __nv_bfloat16* __restrict__ slot_peer,
-                  float* __restrict__ stats_peer /* [B,2] */, int B, int C, float inv_temp,
+                  float* __restrict__ stats_peer /* [B,2] */, int B, int C, int vec, float inv_temp,
                   uint32_t* __restrict__ flag_peer, const uint32_t* __restrict__ seq_ptr, uint32_t seq_imm,
                   unsigned int* __restrict__ done) {
   __shared__ float sh[kRowThreads / 32];
@@ -78,7 +81,7 @@ logit_ship_kernel(const __nv_bfloat16* __restrict__ logits, __nv_bfloat16* __res
   const __nv_bfloat16* src = logits + (int64_t)row * C;
   __nv_bfloat16* dst = slot_peer + (int64_t)row * C;
   float mx = -INFINITY;
-  const int nvec = C / 8;
+  const int nvec = vec ? C / 8 : 0;
   for (int v = threadIdx.x; v < nvec; v += kRowThreads) {
     const bf16x8 x = ld_vec(src + v * 8);
     st_peer(reinterpret_cast<int4*>(dst) + v, *reinterpret_cast<const int4*>(&x));
@@ -209,10 +212,12 @@ void peer_ship(const void* src, void* dst_peer, int64_t nbytes, void* flag_peer,
 
 void logit_ship(const void* logits, void* slot_peer, float* stats_peer, int B, int C, float temperature,
                 void* flag_peer, const void* seq_ptr, uint32_t seq_imm, void* done_counter, cudaStream_t s) {
+  const bool vec = C % 8 == 0 && reinterpret_cast<uintptr_t>(logits) % 16 == 0 &&
+                   reinterpret_cast<uintptr_t>(slot_peer) % 16 == 0;
   logit_ship_kernel<<<B, kRowThreads, 0, s>>>(
       reinterpret_cast<const __nv_bfloat16*>(logits), reinterpret_cast<__nv_bfloat16*>(slot_peer), stats_peer, B,
-      C, 1.f / temperature, reinterpret_cast<uint32_t*>(flag_peer), reinterpret_cast<const uint32_t*>(seq_ptr),
-      seq_imm, reinterpret_cast<unsigned int*>(done_counter));
+      C, vec ? 1 : 0, 1.f / temperature, reinterpret_cast<uint32_t*>(flag_peer),
+      reinterpret_cast<const uint32_t*>(seq_ptr), seq_imm, reinterpret_cast<unsigned int*>(done_counter));
 }
 
 void soft_ce_recv(const void* logits, bool logits_bf16, const void* slot, const float* slot_stats, const void* flag,

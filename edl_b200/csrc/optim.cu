@@ -177,8 +177,8 @@ __global__ void clip_scale_kernel(const float* __restrict__ parts, int nparts, i
   s = warp_sum(s);
   if (threadIdx.x == 0) {
     const float norm = sqrtf(s);
-    // a non-finite norm leaves the scale at 1: the found_inf machinery (loss scaling) owns that case
-    *grad_scale = (norm == norm && norm > max_norm) ? max_norm / (norm + 1e-6f) : 1.f;
+    // a non-finite norm (inf or NaN) leaves the scale at 1: the found_inf machinery (loss scaling) owns that case
+    *grad_scale = (isfinite(norm) && norm > max_norm) ? max_norm / (norm + 1e-6f) : 1.f;
     if (norm_out != nullptr) *norm_out = norm;
   }
 }

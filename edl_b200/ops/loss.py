@@ -4,6 +4,8 @@
 distill losses (example/distill/nlp/model.py:54-66)."""
 from __future__ import annotations
 
+import math
+
 import torch
 import torch.nn.functional as F
 
@@ -26,6 +28,13 @@ def _ref_loss(logits, target, mode, s_temp, t_temp, label_smooth, kl, loss_scale
     return loss.mean() * loss_scale
 
 
+def _smoothed_onehot_plogp(c, label_smooth):
+    """``sum_j p_j log p_j`` of a one-hot over ``c`` classes smoothed by ``label_smooth``."""
+    off = label_smooth / c
+    on = 1.0 - label_smooth + off
+    return (on * math.log(on) if on > 0 else 0.0) + (c - 1) * off * math.log(off)
+
+
 class _SoftCEFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, target, mode, s_temp, t_temp, label_smooth, kl, loss_scale):
@@ -34,7 +43,12 @@ class _SoftCEFn(torch.autograd.Function):
         C = native()
         logits = logits.contiguous()
         n = logits.shape[0]
-        loss = torch.zeros((), device=logits.device, dtype=torch.float32)
+        # the kernel adds every row's share into `loss`.  KL against a smoothed one-hot: the target's sum p log p is
+        # the same constant for every row, so it is the starting value
+        start = 0.0
+        if mode == 2 and kl and label_smooth > 0:
+            start = _smoothed_onehot_plogp(logits.shape[1], label_smooth) * loss_scale
+        loss = torch.full((), start, device=logits.device, dtype=torch.float32)
         stats = torch.empty(n, 4, device=logits.device, dtype=torch.float32)
         tgt = target.contiguous()
         if mode == 2:

@@ -29,6 +29,7 @@ Here:
 """
 from __future__ import annotations
 
+import math
 import os
 import weakref
 from dataclasses import dataclass, field
@@ -304,7 +305,8 @@ class ElasticDataParallel:
         """Let the engine run ``opt`` (a ``FlatSGDMomentum`` on this engine's flat buffers) bucket by bucket: inside
         the reduction kernel on > 1 rank, right behind the bucket's last gradient on one.  ``fused=None`` follows
         ``EDL_FUSED_OPT`` (default on).  Not used with loss scaling, clipping (both need every gradient before any
-        update), the hierarchical or library reduction paths, or weight-decay masks on a single rank."""
+        update), or the hierarchical or library reduction paths.  Weight-decay masks are supported: each bucket's
+        launch takes the matching slice of the mask."""
         self.opt = opt
         if fused is None:
             fused = os.environ.get("EDL_FUSED_OPT", "1") == "1"
@@ -675,7 +677,8 @@ class ElasticDataParallel:
 
     def _clip_cpu(self):
         total = sum(float(g.grad.float().pow(2).sum()) for g in self.flat.groups.values()) ** 0.5
-        if total > self.clip_norm:
+        # like clip_scale_kernel: a non-finite norm is left to the found_inf machinery, the gradients stay as they are
+        if math.isfinite(total) and total > self.clip_norm:
             for g in self.flat.groups.values():
                 g.grad.mul_(self.clip_norm / (total + 1e-6))
         self.last_grad_norm = total
