@@ -44,15 +44,22 @@ void bn_stats(const Tensor& x, Tensor& sums) {
 void bn_apply(const Tensor& x, const c10::optional<Tensor>& res, Tensor& y, const Tensor& sums,
               const Tensor& gamma, const Tensor& beta, const c10::optional<Tensor>& running_mean,
               const c10::optional<Tensor>& running_var, Tensor& saved_mean, Tensor& saved_rstd,
-              double eps, double momentum, bool relu) {
+              double eps, double momentum, bool relu, const c10::optional<Tensor>& mask) {
   check_bf16(x, "x");
   check_bf16(y, "y");
   check_f32(gamma, "gamma");
   check_f32(beta, "beta");
   const int C = x.size(-1);
   const int64_t M = x.numel() / C;
+  if (mask.has_value() && mask->defined()) {
+    TORCH_CHECK(res.has_value() && res->defined() && relu, "bn_apply: mask bits belong to ReLU after a residual add");
+    TORCH_CHECK(edl::bn_mask_supported(M, C), "bn_apply: no mask bits for this shape (see bn_relu_mask_supported)");
+    TORCH_CHECK(mask->is_cuda() && mask->scalar_type() == at::kByte && mask->is_contiguous() &&
+                mask->numel() * 8 == M * C && reinterpret_cast<uintptr_t>(mask->data_ptr()) % 16 == 0,
+                "bn_apply: mask must be a contiguous, 16-byte aligned uint8 [M, C / 8]");
+  }
   c10::cuda::CUDAGuard g(x.device());
-  edl::bn_apply(x.data_ptr(), opt_ptr<void>(res), y.data_ptr(), sums.data_ptr<float>(),
+  edl::bn_apply(x.data_ptr(), opt_ptr<void>(res), y.data_ptr(), opt_ptr<void>(mask), sums.data_ptr<float>(),
                 gamma.data_ptr<float>(), beta.data_ptr<float>(), opt_ptr<float>(running_mean),
                 opt_ptr<float>(running_var), saved_mean.data_ptr<float>(),
                 saved_rstd.data_ptr<float>(), M, C, (float)eps, (float)momentum, relu,
@@ -72,6 +79,26 @@ void scale_shift_act(const Tensor& x, const c10::optional<Tensor>& res, Tensor& 
                        shift.data_ptr<float>(), M, C, relu, cur_stream());
 }
 
+// y of the BN backward kernels: the bf16 BN output, or its uint8 ReLU mask bits [M, C / 8] (bn_apply's mask)
+struct YOrMask {
+  const void* y = nullptr;
+  const void* mask = nullptr;
+};
+YOrMask y_or_mask(const c10::optional<Tensor>& y, int64_t M, int C) {
+  YOrMask r;
+  if (!y.has_value() || !y->defined()) return r;
+  TORCH_CHECK(y->is_cuda() && y->is_contiguous(), "y must be a contiguous CUDA tensor");
+  if (y->scalar_type() == at::kByte) {
+    TORCH_CHECK(edl::bn_mask_supported(M, C) && y->numel() * 8 == M * C &&
+                reinterpret_cast<uintptr_t>(y->data_ptr()) % 16 == 0, "mask bits: uint8 [M, C / 8] of a supported shape");
+    r.mask = y->data_ptr();
+  } else {
+    TORCH_CHECK(y->scalar_type() == at::kBFloat16 && y->numel() == M * C, "y must be bf16 [M, C]");
+    r.y = y->data_ptr();
+  }
+  return r;
+}
+
 void bn_bwd_reduce(const Tensor& dy, const Tensor& x, const c10::optional<Tensor>& y,
                    const Tensor& gamma, const Tensor& beta, const Tensor& saved_mean,
                    const Tensor& saved_rstd, Tensor& dsums, bool relu) {
@@ -79,8 +106,9 @@ void bn_bwd_reduce(const Tensor& dy, const Tensor& x, const c10::optional<Tensor
   check_bf16(x, "x");
   const int C = x.size(-1);
   const int64_t M = x.numel() / C;
+  const YOrMask ym = y_or_mask(y, M, C);
   c10::cuda::CUDAGuard g(x.device());
-  edl::bn_bwd_reduce(dy.data_ptr(), x.data_ptr(), opt_ptr<void>(y), gamma.data_ptr<float>(),
+  edl::bn_bwd_reduce(dy.data_ptr(), x.data_ptr(), ym.y, ym.mask, gamma.data_ptr<float>(),
                      beta.data_ptr<float>(), saved_mean.data_ptr<float>(),
                      saved_rstd.data_ptr<float>(), dsums.data_ptr<float>(), M, C, relu,
                      cur_stream());
@@ -97,8 +125,9 @@ void bn_bwd_apply(const Tensor& dy, const Tensor& x, const c10::optional<Tensor>
   check_bf16(dx, "dx");
   const int C = x.size(-1);
   const int64_t M = x.numel() / C;
+  const YOrMask ym = y_or_mask(y, M, C);
   c10::cuda::CUDAGuard g(x.device());
-  edl::bn_bwd_apply(dy.data_ptr(), x.data_ptr(), opt_ptr<void>(y), gamma.data_ptr<float>(),
+  edl::bn_bwd_apply(dy.data_ptr(), x.data_ptr(), ym.y, ym.mask, gamma.data_ptr<float>(),
                     beta.data_ptr<float>(), saved_mean.data_ptr<float>(),
                     saved_rstd.data_ptr<float>(),
                     dsums.data_ptr<float>(), dx.data_ptr(), opt_ptr<void>(dres),
@@ -667,7 +696,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bn_fwd_fused", &bn_fwd_fused);
   m.def("bn_bwd_fused", &bn_bwd_fused);
   m.def("bn_stats", &bn_stats);
-  m.def("bn_apply", &bn_apply);
+  m.def("bn_apply", &bn_apply, pybind11::arg("x"), pybind11::arg("res"), pybind11::arg("y"), pybind11::arg("sums"),
+        pybind11::arg("gamma"), pybind11::arg("beta"), pybind11::arg("running_mean"), pybind11::arg("running_var"),
+        pybind11::arg("saved_mean"), pybind11::arg("saved_rstd"), pybind11::arg("eps"), pybind11::arg("momentum"),
+        pybind11::arg("relu"), pybind11::arg("mask") = pybind11::none());
+  m.def("bn_relu_mask_supported", &edl::bn_relu_mask_supported,
+        "the streaming BN kernels run for [M, C] and can keep the residual ReLU mask as bits");
   m.def("scale_shift_act", &scale_shift_act);
   m.def("bn_bwd_reduce", &bn_bwd_reduce);
   m.def("bn_bwd_apply", &bn_bwd_apply);

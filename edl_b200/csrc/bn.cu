@@ -439,12 +439,16 @@ void bn_stats(const void* x, float* sums, int64_t M, int C, cudaStream_t stream)
   bn_stats_kernel<<<g.grid, g.block, smem, stream>>>(BF(x), sums, M, C);
 }
 
-void bn_apply(const void* x, const void* res, void* y, const float* sums, const float* gamma,
+bool bn_relu_mask_supported(int64_t M, int C) { return g_use_stream && bn_mask_supported(M, C); }
+
+// mask bits exist only for the streaming kernels: callers check bn_relu_mask_supported() before asking for them, and a
+// saved mask is read back by the streaming kernels whatever bn_set_stream_kernels() says by then
+void bn_apply(const void* x, const void* res, void* y, void* mask, const float* sums, const float* gamma,
               const float* beta, float* running_mean, float* running_var, float* saved_mean,
               float* saved_rstd, int64_t M, int C, float eps, float momentum, bool relu,
               cudaStream_t stream) {
-  if (g_use_stream && bn_stream_supported(M, C))
-    return bn_apply_stream(x, res, y, sums, gamma, beta, running_mean, running_var, saved_mean,
+  if (mask != nullptr || (g_use_stream && bn_stream_supported(M, C)))
+    return bn_apply_stream(x, res, y, mask, sums, gamma, beta, running_mean, running_var, saved_mean,
                            saved_rstd, M, C, eps, momentum, relu, stream);
   BnGrid g = bn_grid(M, C, kNumSMs * 8);
   bn_apply_kernel<<<g.grid, g.block, 0, stream>>>(BF(x), BF(res), BFW(y), sums, gamma, beta,
@@ -459,11 +463,11 @@ void scale_shift_act(const void* x, const void* res, void* y, const float* scale
                                                          C, relu ? 1 : 0);
 }
 
-void bn_bwd_reduce(const void* dy, const void* x, const void* y, const float* gamma,
+void bn_bwd_reduce(const void* dy, const void* x, const void* y, const void* mask, const float* gamma,
                    const float* beta, const float* saved_mean, const float* saved_rstd,
                    float* dsums, int64_t M, int C, bool relu, cudaStream_t stream) {
-  if (g_use_stream && bn_stream_supported(M, C))
-    return bn_bwd_reduce_stream(dy, x, y, gamma, beta, saved_mean, saved_rstd, dsums, M, C, relu,
+  if (mask != nullptr || (g_use_stream && bn_stream_supported(M, C)))
+    return bn_bwd_reduce_stream(dy, x, y, mask, gamma, beta, saved_mean, saved_rstd, dsums, M, C, relu,
                                 stream);
   BnGrid g = bn_grid(M, C, kNumSMs * 4);
   size_t smem = (size_t)kBnThreads * 16 * sizeof(float);
@@ -477,12 +481,12 @@ void bn_bwd_reduce(const void* dy, const void* x, const void* y, const float* ga
 #undef LAUNCH
 }
 
-void bn_bwd_apply(const void* dy, const void* x, const void* y, const float* gamma,
+void bn_bwd_apply(const void* dy, const void* x, const void* y, const void* mask, const float* gamma,
                   const float* beta, const float* saved_mean, const float* saved_rstd,
                   const float* dsums, void* dx, void* dres, float* dgamma, float* dbeta, int64_t M,
                   int C, bool relu, bool accumulate, cudaStream_t stream) {
-  if (g_use_stream && bn_stream_supported(M, C))
-    return bn_bwd_apply_stream(dy, x, y, gamma, beta, saved_mean, saved_rstd, dsums, dx, dres,
+  if (mask != nullptr || (g_use_stream && bn_stream_supported(M, C)))
+    return bn_bwd_apply_stream(dy, x, y, mask, gamma, beta, saved_mean, saved_rstd, dsums, dx, dres,
                                dgamma, dbeta, M, C, relu, accumulate, stream);
   BnGrid g = bn_grid(M, C, kNumSMs * 8);
 #define LAUNCH(R, Y)                                                                          \

@@ -68,10 +68,10 @@ constexpr size_t ring_smem_bytes() {
   return (size_t)kStages * NT * kChunkBytes + 2 * kStages * sizeof(uint64_t) + 128;
 }
 
-// Producer loop (one lane of the producer warp).
-template <int NT>
-EDL_DEVICE void produce(const Ring<NT>& r, const __nv_bfloat16* const (&src)[NT], int64_t total_elems,
-                        int64_t n_chunks) {
+// Producer loop (one lane of the producer warp).  Operand MASK_T (if >= 0) is a ReLU mask with one bit per element
+// (uint8 [M, C / 8]): 1/16 of a bf16 operand's bytes, which stay a multiple of 16 when C % 128 == 0.
+template <int NT, int MASK_T = -1>
+EDL_DEVICE void produce(const Ring<NT>& r, const void* const (&src)[NT], int64_t total_elems, int64_t n_chunks) {
   int it = 0;
   for (int64_t ch = blockIdx.x; ch < n_chunks; ch += gridDim.x, ++it) {
     const int s = it % kStages;
@@ -80,14 +80,20 @@ EDL_DEVICE void produce(const Ring<NT>& r, const __nv_bfloat16* const (&src)[NT]
     const int64_t off = ch * kChunkElems;
     int64_t rem = total_elems - off;
     const uint32_t bytes = (uint32_t)((rem < kChunkElems ? rem : kChunkElems) * 2);
-    ptx::mbar_arrive_expect_tx(&r.full[s], bytes * NT);
+    ptx::mbar_arrive_expect_tx(&r.full[s], MASK_T < 0 ? bytes * NT : bytes * (NT - 1) + bytes / 16);
 #pragma unroll
-    for (int t = 0; t < NT; ++t) bulk_load(r.buf(s, t), src[t] + off, bytes, &r.full[s]);
+    for (int t = 0; t < NT; ++t) {
+      if (t == MASK_T)
+        bulk_load(r.buf(s, t), reinterpret_cast<const uint8_t*>(src[t]) + off / 8, bytes / 16, &r.full[s]);
+      else
+        bulk_load(r.buf(s, t), reinterpret_cast<const __nv_bfloat16*>(src[t]) + off, bytes, &r.full[s]);
+    }
   }
 }
 
-// Consumer loop: body(vec_index_in_chunk, global_elem_offset, smem pointers of the NT operands)
-template <int NT, class Body>
+// Consumer loop: body(global_elem_offset, smem pointers of the NT operands); the pointer of a mask operand points at
+// the vector's mask byte
+template <int NT, int MASK_T = -1, class Body>
 EDL_DEVICE void consume(const Ring<NT>& r, int64_t total_elems, int64_t n_chunks, Body body) {
   const int tid = threadIdx.x;
   int it = 0;
@@ -104,7 +110,9 @@ EDL_DEVICE void consume(const Ring<NT>& r, int64_t total_elems, int64_t n_chunks
       if (v < valid_vecs) {
         const bf16x8* ptrs[NT];
 #pragma unroll
-        for (int t = 0; t < NT; ++t) ptrs[t] = reinterpret_cast<const bf16x8*>(r.buf(s, t)) + v;
+        for (int t = 0; t < NT; ++t)
+          ptrs[t] = t == MASK_T ? reinterpret_cast<const bf16x8*>(r.buf(s, t) + v)
+                                : reinterpret_cast<const bf16x8*>(r.buf(s, t)) + v;
         body(off + (int64_t)v * 8, ptrs);
       }
     }
@@ -151,7 +159,7 @@ bn_stats_stream_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ 
   for (int i = 0; i < 16; ++i) acc[i] = 0.f;
   if (!consumer) {
     if (tid == kConsumers) {
-      const __nv_bfloat16* src[1] = {x};
+      const void* src[1] = {x};
       produce<1>(r, src, total, n_chunks);
     }
   } else {
@@ -172,10 +180,11 @@ bn_stats_stream_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ 
   }
 }
 
+// mask (optional, HAS_RES only): uint8 [M, C / 8], bit b of byte j = (stored y[:, 8 j + b] > 0), C % 128 == 0
 template <bool HAS_RES>
 __global__ void __launch_bounds__(kThreads, 1)
 bn_apply_stream_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ res,
-                       __nv_bfloat16* __restrict__ y, const float* __restrict__ sums,
+                       __nv_bfloat16* __restrict__ y, uint8_t* __restrict__ mask, const float* __restrict__ sums,
                        const float* __restrict__ gamma, const float* __restrict__ beta,
                        float* __restrict__ running_mean, float* __restrict__ running_var,
                        float* __restrict__ saved_mean, float* __restrict__ saved_rstd, int64_t total, int C,
@@ -188,16 +197,10 @@ bn_apply_stream_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16*
   const int cvecs = C / 8;
   if (tid >= kConsumers) {
     if (tid == kConsumers) {
-      if (HAS_RES) {
-        const __nv_bfloat16* src[NT];
-        src[0] = x;
-        src[NT - 1] = res;
-        produce<NT>(r, src, total, n_chunks);
-      } else {
-        const __nv_bfloat16* src[NT];
-        src[0] = x;
-        produce<NT>(r, src, total, n_chunks);
-      }
+      const void* src[NT];
+      src[0] = x;
+      if (HAS_RES) src[NT - 1] = res;
+      produce<NT>(r, src, total, n_chunks);
     }
     return;
   }
@@ -237,7 +240,22 @@ bn_apply_stream_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16*
 #pragma unroll
       for (int i = 0; i < 8; ++i) f[i] = fmaxf(f[i], 0.f);
     }
-    st_vec(y + goff, pack8(f));
+    const bf16x8 o = pack8(f);
+    st_vec(y + goff, o);
+    if (HAS_RES && mask != nullptr) {
+      // the bits test the STORED bf16 values (an fp32 result that rounds to a bf16 zero is masked).  Consecutive lanes
+      // hold consecutive vectors and the valid vectors of a chunk are a multiple of 16 (C >= 128), so every group of
+      // four lanes is complete: three shuffles gather four mask bytes into its first lane, which stores them as a word.
+      unpack8(o, f);
+      uint32_t b = 0;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) b |= (f[i] > 0.f ? 1u : 0u) << i;
+      const int lane = tid & 31;
+      const unsigned grp = 0xFu << (lane & ~3);
+#pragma unroll
+      for (int d = 1; d < 4; ++d) b |= __shfl_down_sync(grp, b & 0xFFu, d, 4) << (8 * d);
+      if ((lane & 3) == 0) *reinterpret_cast<uint32_t*>(mask + goff / 8) = b;
+    }
   });
 }
 
@@ -256,29 +274,38 @@ EDL_DEVICE void load_coef(Coef& k, const float* saved_mean, const float* saved_r
   }
 }
 
-template <bool RELU, bool HAS_Y>
+// Where the ReLU mask comes from: recomputed from x, the bf16 BN output y, or the forward's mask bits (one byte per
+// vector of 8 channels)
+enum YKind { kMaskFromX = 0, kMaskFromY = 1, kMaskBits = 2 };
+
+template <bool RELU, int YK>
 EDL_DEVICE void masked_grad(float (&g)[8], const float (&f)[8], const bf16x8* yv, const Coef& k) {
   if (!RELU) return;
-  if (HAS_Y) {
+  if (YK == kMaskFromY) {
     float o[8];
     unpack8(*yv, o);
 #pragma unroll
     for (int i = 0; i < 8; ++i) g[i] = o[i] > 0.f ? g[i] : 0.f;
+  } else if (YK == kMaskBits) {
+    const uint32_t b = *reinterpret_cast<const uint8_t*>(yv);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) g[i] = ((b >> i) & 1u) ? g[i] : 0.f;
   } else {
 #pragma unroll
     for (int i = 0; i < 8; ++i) g[i] = fmaf(f[i], k.scale[i], k.shift[i]) > 0.f ? g[i] : 0.f;
   }
 }
 
-template <bool RELU, bool HAS_Y>
+template <bool RELU, int YK>
 __global__ void __launch_bounds__(kThreads, 1)
 bn_bwd_reduce_stream_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
-                            const __nv_bfloat16* __restrict__ y, const float* __restrict__ gamma,
+                            const void* __restrict__ y, const float* __restrict__ gamma,
                             const float* __restrict__ beta, const float* __restrict__ saved_mean,
                             const float* __restrict__ saved_rstd, float* __restrict__ dsums, int64_t total,
                             int C) {
   extern __shared__ uint8_t smem_raw[];
-  constexpr int NT = HAS_Y ? 3 : 2;
+  constexpr int NT = YK != kMaskFromX ? 3 : 2;
+  constexpr int MT = YK == kMaskBits ? NT - 1 : -1;
   Ring<NT> r = ring_init<NT>(smem_raw);
   const int64_t n_chunks = (total + kChunkElems - 1) / kChunkElems;
   const int tid = threadIdx.x;
@@ -289,20 +316,20 @@ bn_bwd_reduce_stream_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfl
   for (int i = 0; i < 16; ++i) acc[i] = 0.f;
   if (!consumer) {
     if (tid == kConsumers) {
-      const __nv_bfloat16* src[NT];
+      const void* src[NT];
       src[0] = dy;
       src[1] = x;
-      if (HAS_Y) src[NT - 1] = y;
-      produce<NT>(r, src, total, n_chunks);
+      if (YK != kMaskFromX) src[NT - 1] = y;
+      produce<NT, MT>(r, src, total, n_chunks);
     }
   } else {
     Coef k;
     load_coef(k, saved_mean, saved_rstd, gamma, beta, (tid % cvecs) * 8);
-    consume<NT>(r, total, n_chunks, [&](int64_t, const bf16x8* const (&p)[NT]) {
+    consume<NT, MT>(r, total, n_chunks, [&](int64_t, const bf16x8* const (&p)[NT]) {
       float g[8], f[8];
       unpack8(*p[0], g);
       unpack8(*p[1], f);
-      masked_grad<RELU, HAS_Y>(g, f, p[NT - 1], k);
+      masked_grad<RELU, YK>(g, f, p[NT - 1], k);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         acc[i] += g[i];
@@ -317,28 +344,29 @@ bn_bwd_reduce_stream_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfl
   }
 }
 
-template <bool RELU, bool HAS_Y>
+template <bool RELU, int YK>
 __global__ void __launch_bounds__(kThreads, 1)
 bn_bwd_apply_stream_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
-                           const __nv_bfloat16* __restrict__ y, const float* __restrict__ gamma,
+                           const void* __restrict__ y, const float* __restrict__ gamma,
                            const float* __restrict__ beta, const float* __restrict__ saved_mean,
                            const float* __restrict__ saved_rstd, const float* __restrict__ dsums,
                            __nv_bfloat16* __restrict__ dx, __nv_bfloat16* __restrict__ dres,
                            float* __restrict__ dgamma, float* __restrict__ dbeta, int64_t total, int C,
                            int accumulate) {
   extern __shared__ uint8_t smem_raw[];
-  constexpr int NT = HAS_Y ? 3 : 2;
+  constexpr int NT = YK != kMaskFromX ? 3 : 2;
+  constexpr int MT = YK == kMaskBits ? NT - 1 : -1;
   Ring<NT> r = ring_init<NT>(smem_raw);
   const int64_t n_chunks = (total + kChunkElems - 1) / kChunkElems;
   const int tid = threadIdx.x;
   const int cvecs = C / 8;
   if (tid >= kConsumers) {
     if (tid == kConsumers) {
-      const __nv_bfloat16* src[NT];
+      const void* src[NT];
       src[0] = dy;
       src[1] = x;
-      if (HAS_Y) src[NT - 1] = y;
-      produce<NT>(r, src, total, n_chunks);
+      if (YK != kMaskFromX) src[NT - 1] = y;
+      produce<NT, MT>(r, src, total, n_chunks);
     }
     return;
   }
@@ -362,11 +390,11 @@ bn_bwd_apply_stream_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bflo
       }
     }
   }
-  consume<NT>(r, total, n_chunks, [&](int64_t goff, const bf16x8* const (&p)[NT]) {
+  consume<NT, MT>(r, total, n_chunks, [&](int64_t goff, const bf16x8* const (&p)[NT]) {
     float g[8], f[8];
     unpack8(*p[0], g);
     unpack8(*p[1], f);
-    masked_grad<RELU, HAS_Y>(g, f, p[NT - 1], k);
+    masked_grad<RELU, YK>(g, f, p[NT - 1], k);
     if (dres != nullptr) st_vec(dres + goff, pack8(g));
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -417,7 +445,9 @@ void bn_stats_stream(const void* x, float* sums, int64_t M, int C, cudaStream_t 
   launch_pdl(bn_stats_stream_kernel, dim3(reduce_grid(total)), dim3(kThreads), smem, s, BF(x), sums, total, C);
 }
 
-void bn_apply_stream(const void* x, const void* res, void* y, const float* sums, const float* gamma,
+bool bn_mask_supported(int64_t M, int C) { return bn_stream_supported(M, C) && C % 128 == 0; }
+
+void bn_apply_stream(const void* x, const void* res, void* y, void* mask, const float* sums, const float* gamma,
                      const float* beta, float* running_mean, float* running_var, float* saved_mean,
                      float* saved_rstd, int64_t M, int C, float eps, float momentum, bool relu,
                      cudaStream_t s) {
@@ -425,47 +455,49 @@ void bn_apply_stream(const void* x, const void* res, void* y, const float* sums,
   if (res != nullptr) {
     set_smem(bn_apply_stream_kernel<true>, ring_smem_bytes<2>());
     launch_pdl(bn_apply_stream_kernel<true>, dim3(stream_grid(total)), dim3(kThreads), ring_smem_bytes<2>(), s,
-        BF(x), BF(res), BFW(y), sums, gamma, beta, running_mean, running_var, saved_mean, saved_rstd, total, C,
-        eps, momentum, relu ? 1 : 0);
+        BF(x), BF(res), BFW(y), reinterpret_cast<uint8_t*>(mask), sums, gamma, beta, running_mean, running_var,
+        saved_mean, saved_rstd, total, C, eps, momentum, relu ? 1 : 0);
   } else {
     set_smem(bn_apply_stream_kernel<false>, ring_smem_bytes<1>());
     launch_pdl(bn_apply_stream_kernel<false>, dim3(stream_grid(total)), dim3(kThreads), ring_smem_bytes<1>(), s,
-        BF(x), (const __nv_bfloat16*)nullptr, BFW(y), sums, gamma, beta, running_mean, running_var, saved_mean, saved_rstd, total, C,
-        eps, momentum, relu ? 1 : 0);
+        BF(x), (const __nv_bfloat16*)nullptr, BFW(y), (uint8_t*)nullptr, sums, gamma, beta, running_mean, running_var,
+        saved_mean, saved_rstd, total, C, eps, momentum, relu ? 1 : 0);
   }
 }
 
-void bn_bwd_reduce_stream(const void* dy, const void* x, const void* y, const float* gamma, const float* beta,
-                          const float* saved_mean, const float* saved_rstd, float* dsums, int64_t M, int C,
-                          bool relu, cudaStream_t s) {
+void bn_bwd_reduce_stream(const void* dy, const void* x, const void* y, const void* mask, const float* gamma,
+                          const float* beta, const float* saved_mean, const float* saved_rstd, float* dsums, int64_t M,
+                          int C, bool relu, cudaStream_t s) {
   const int64_t total = M * C;
-#define LAUNCH(R, Y, NT)                                                                                   \
+#define LAUNCH(R, Y, NT, YP)                                                                               \
   {                                                                                                        \
     set_smem(bn_bwd_reduce_stream_kernel<R, Y>, ring_smem_bytes<NT>());                                    \
     launch_pdl(bn_bwd_reduce_stream_kernel<R, Y>, dim3(reduce_grid(total)), dim3(kThreads),                \
-               ring_smem_bytes<NT>(), s, BF(dy), BF(x), BF(y), gamma, beta, saved_mean, saved_rstd, dsums, total, C);                       \
+               ring_smem_bytes<NT>(), s, BF(dy), BF(x), YP, gamma, beta, saved_mean, saved_rstd, dsums, total, C);                       \
   }
-  if (!relu) LAUNCH(false, false, 2)
-  else if (y != nullptr) LAUNCH(true, true, 3)
-  else LAUNCH(true, false, 2)
+  if (!relu) LAUNCH(false, kMaskFromX, 2, y)
+  else if (mask != nullptr) LAUNCH(true, kMaskBits, 3, mask)
+  else if (y != nullptr) LAUNCH(true, kMaskFromY, 3, y)
+  else LAUNCH(true, kMaskFromX, 2, y)
 #undef LAUNCH
 }
 
-void bn_bwd_apply_stream(const void* dy, const void* x, const void* y, const float* gamma, const float* beta,
-                         const float* saved_mean, const float* saved_rstd, const float* dsums, void* dx,
-                         void* dres, float* dgamma, float* dbeta, int64_t M, int C, bool relu, bool accumulate,
-                         cudaStream_t s) {
+void bn_bwd_apply_stream(const void* dy, const void* x, const void* y, const void* mask, const float* gamma,
+                         const float* beta, const float* saved_mean, const float* saved_rstd, const float* dsums,
+                         void* dx, void* dres, float* dgamma, float* dbeta, int64_t M, int C, bool relu,
+                         bool accumulate, cudaStream_t s) {
   const int64_t total = M * C;
-#define LAUNCH(R, Y, NT)                                                                                   \
+#define LAUNCH(R, Y, NT, YP)                                                                               \
   {                                                                                                        \
     set_smem(bn_bwd_apply_stream_kernel<R, Y>, ring_smem_bytes<NT>());                                     \
     launch_pdl(bn_bwd_apply_stream_kernel<R, Y>, dim3(stream_grid(total)), dim3(kThreads),                 \
-               ring_smem_bytes<NT>(), s, BF(dy), BF(x), BF(y), gamma, beta, saved_mean, saved_rstd, dsums, BFW(dx), BFW(dres), dgamma, dbeta, \
+               ring_smem_bytes<NT>(), s, BF(dy), BF(x), YP, gamma, beta, saved_mean, saved_rstd, dsums, BFW(dx), BFW(dres), dgamma, dbeta, \
         total, C, accumulate ? 1 : 0);                                                                     \
   }
-  if (!relu) LAUNCH(false, false, 2)
-  else if (y != nullptr) LAUNCH(true, true, 3)
-  else LAUNCH(true, false, 2)
+  if (!relu) LAUNCH(false, kMaskFromX, 2, y)
+  else if (mask != nullptr) LAUNCH(true, kMaskBits, 3, mask)
+  else if (y != nullptr) LAUNCH(true, kMaskFromY, 3, y)
+  else LAUNCH(true, kMaskFromX, 2, y)
 #undef LAUNCH
 }
 

@@ -11,6 +11,8 @@ namespace edl {
 struct BnBwdFuse {
   const void* x = nullptr;       // bf16, BN input (conv output), same shape / layout as D
   const void* y = nullptr;       // bf16, BN output: only for ReLU after a residual add (mask = y > 0)
+  const void* mask = nullptr;    // or uint8 [M, C / 8], bit b of byte j = (y[:, 8 j + b] > 0): D is then stored masked
+                                 // (1x1 dgrad, C % 128 == 0)
   const float* mean = nullptr;
   const float* rstd = nullptr;
   const float* gamma = nullptr;
@@ -148,7 +150,7 @@ const char* encode_tmap(void* out, const void* ptr, int rank, const uint64_t* di
                         const uint64_t* strides_bytes, const uint32_t* box, int elem_bytes);
 const char* encode_tmap_strided(void* out, const void* ptr, int rank, const uint64_t* dims,
                                 const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides,
-                                int elem_bytes);
+                                int elem_bytes, bool swizzle = true);
 
 // FP8 (e4m3) inference GEMM (gemm_fp8.cu): D[M,N] bf16 = relu?((A[M,K] * B[N,K]^T) * col_scale[n] + col_shift[n])
 // A, B e4m3 bytes, K-major; col_scale carries act_scale * weight_scale[n] (* folded BN scale).

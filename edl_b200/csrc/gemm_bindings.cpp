@@ -13,7 +13,8 @@ inline T* optp(const c10::optional<Tensor>& t) {
   return t.has_value() && t->defined() ? reinterpret_cast<T*>(t->data_ptr()) : nullptr;
 }
 
-// bn = [x, y | None, mean, rstd, gamma, beta, dsums] (+ relu flag): see gemm.h BnBwdFuse
+// bn = [x, y | mask | None, mean, rstd, gamma, beta, dsums] (+ relu flag): see gemm.h BnBwdFuse.  The second entry is
+// the bf16 BN output or its uint8 ReLU mask bits [M, C / 8].
 edl::BnBwdFuse parse_bn(const c10::optional<std::vector<c10::optional<Tensor>>>& bn, bool relu, int64_t numel,
                         int64_t channels) {
   edl::BnBwdFuse f;
@@ -23,8 +24,15 @@ edl::BnBwdFuse parse_bn(const c10::optional<std::vector<c10::optional<Tensor>>>&
   TORCH_CHECK(v[0].has_value() && v[0]->scalar_type() == at::kBFloat16 && v[0]->numel() == numel);
   f.x = v[0]->data_ptr();
   if (v[1].has_value() && v[1]->defined()) {
-    TORCH_CHECK(v[1]->scalar_type() == at::kBFloat16 && v[1]->numel() == numel);
-    f.y = v[1]->data_ptr();
+    if (v[1]->scalar_type() == at::kByte) {
+      TORCH_CHECK(v[1]->is_contiguous() && channels % 128 == 0 && v[1]->numel() * 8 == numel &&
+                  reinterpret_cast<uintptr_t>(v[1]->data_ptr()) % 16 == 0,
+                  "bn mask bits: contiguous uint8 [M, C / 8], C % 128 == 0, 16-byte aligned");
+      f.mask = v[1]->data_ptr();
+    } else {
+      TORCH_CHECK(v[1]->scalar_type() == at::kBFloat16 && v[1]->numel() == numel);
+      f.y = v[1]->data_ptr();
+    }
   }
   for (int i = 2; i < 7; ++i)
     TORCH_CHECK(v[i].has_value() && v[i]->scalar_type() == at::kFloat && v[i]->is_contiguous() &&

@@ -52,6 +52,8 @@ struct PersistParams {
   const float* bn_beta;
   float* bn_dsums;                // [2N]: += sum(dy_masked), sum(dy_masked * xhat)
   int bn_relu, bn_has_y;
+  // ReLU mask bits of the BN output instead of y (1x1, N % 128 == 0): D is stored already masked
+  int bn_has_mask;
   // conv view (modes 2, 3)
   int n_img, H, W, kc_blocks, c_in_w, BH, BN, tiles_h;
   int Wb;                         // halo layout: columns per image row of the A tile (W + 1)
@@ -117,7 +119,10 @@ EDL_DEVICE void issue_bn_tiles(const PersistParams& p, int tm, int nn0, int rows
   for (int hh = 0; hh < (BLOCK_N + 63) / 64; ++hh) halves += (nn0 + hh * 64 < p.N) ? 1u : 0u;
   const uint32_t tile_bytes = CONV ? (uint32_t)rows_tile * 128u : (uint32_t)(kBlockM * 128);
   if (ptx::elect_one()) {
-    ptx::mbar_arrive_expect_tx(bar, halves * tile_bytes * (p.bn_has_y ? 2u : 1u));
+    // the mask box is 16 bytes (128 columns) x 128 rows, unswizzled: row r at sy + 16 r
+    const uint32_t mask_bytes = (!CONV && p.bn_has_mask) ? (uint32_t)(kBlockM * 16) : 0u;
+    ptx::mbar_arrive_expect_tx(bar, halves * tile_bytes * (p.bn_has_y ? 2u : 1u) + mask_bytes);
+    if (mask_bytes != 0) ptx::tma_load_2d(sy, tmY, bar, nn0 / 8, mm0);
 #pragma unroll
     for (int hh = 0; hh < (BLOCK_N + 63) / 64; ++hh) {
       if (nn0 + hh * 64 >= p.N) continue;
@@ -516,6 +521,14 @@ gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       }
       if (et == 0) EDL_TRACE(2, tc, 2);
       // ---- accumulators -> addend / scale / shift / ReLU -> bf16 -> swizzled staging tile
+      // BN ReLU mask bits (1x1 dgrad): the gradient is masked BEFORE it is staged, so what reaches HBM is dy * (y > 0)
+      // and neither the reduction below nor the BN backward needs the mask again.  Bit b of byte j of a mask row is
+      // column 8 j + b; this thread's columns are bytes grp * kColsPerGrp / 8 .. + kColsPerGrp / 8 - 1 of rows row, row + 8.
+      // A mask word (four bytes) is loaded when the loop reaches its first column group.
+      const bool bn_mask = BNR != 0 && !kConv && p.bn_has_mask != 0;
+      [[maybe_unused]] uint32_t mword[2] = {0u, 0u};
+      const uint32_t mbase = ptx::smem_u32(sy) + row * 16 + grp * (kColsPerGrp / 8);
+      if (bn_mask) ptx::mbar_wait(bn_bar, tc & 1);
 #pragma unroll
       for (int j = 0; j < kColsPerGrp / 8; ++j) {
         const int tcol = grp * kColsPerGrp + j * 8 + cq;        // column inside the tile
@@ -531,6 +544,18 @@ gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             const float2 t2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
             v[2 * h] += t2.x;
             v[2 * h + 1] += t2.y;
+          }
+        }
+        if (bn_mask) {
+          if ((j & 3) == 0) {
+            mword[0] = ptx::lds32(mbase + (j >> 2) * 4);
+            mword[1] = ptx::lds32(mbase + 8 * 16 + (j >> 2) * 4);
+          }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t bits = mword[h] >> ((j & 3) * 8 + cq);
+            v[2 * h] = (bits & 1u) ? v[2 * h] : 0.f;
+            v[2 * h + 1] = (bits & 2u) ? v[2 * h + 1] : 0.f;
           }
         }
         if (!BNR) {
@@ -590,7 +615,8 @@ gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         const uint32_t based = ptx::smem_u32(sd) + toff, basex = ptx::smem_u32(sx) + toff, basey = ptx::smem_u32(sy) + toff;
         const float4 k0 = reinterpret_cast<const float4*>(sconst)[col];          // mean, rstd, scale, shift
         const float4 k1 = reinterpret_cast<const float4*>(sconst)[col + 1];
-        const bool relu = p.bn_relu != 0, has_y = p.bn_has_y != 0;
+        // with mask bits the staged gradient is already masked
+        const bool relu = p.bn_relu != 0 && !bn_mask, has_y = p.bn_has_y != 0;
         // s = sum(dy_m), q = sum(dy_m * x) over this thread's rows; sum(dy_m * xhat) = rstd * (q - mean * s) is formed once
         // per thread and tile below (two instructions per element less than normalising x in the loop).  With the BN
         // OUTPUT at hand the ReLU mask is a packed bf16 compare and a multiplication by 1.0 / 0.0 (exact).
@@ -893,6 +919,7 @@ void fill_bn(PersistParams& p, const BnBwdFuse& bn) {
   p.bn_dsums = bn.dsums;
   p.bn_relu = bn.relu ? 1 : 0;
   p.bn_has_y = (bn.relu && bn.y != nullptr) ? 1 : 0;
+  p.bn_has_mask = (bn.relu && bn.mask != nullptr) ? 1 : 0;
 }
 }  // namespace
 
@@ -943,11 +970,22 @@ const char* gemm_bf16_persistent(const GemmArgs& g, cudaStream_t stream) {
     alignas(64) CUtensorMap tmBx, tmBy;
     if (const char* e = tmap2d(&tmBx, g.bn.x, g.N, g.M, g.ldd, 64, kBlockM)) return e;
     const bool has_y = g.bn.relu && g.bn.y != nullptr;
+    const bool has_mask = g.bn.relu && g.bn.mask != nullptr;
+    if (has_y && has_mask) return "fused BN-backward reduction: give the BN output or its mask bits, not both";
     if (has_y)
       if (const char* e = tmap2d(&tmBy, g.bn.y, g.N, g.M, g.ldd, 64, kBlockM)) return e;
+    if (has_mask) {
+      // uint8 [M, N / 8], one 16-byte box per 128-column tile
+      if (g.N % 128 != 0) return "fused BN-backward reduction with mask bits needs N % 128 == 0";
+      const uint64_t dims[2] = {(uint64_t)g.N / 8, (uint64_t)g.M};
+      const uint64_t st[1] = {(uint64_t)g.N / 8};
+      const uint32_t box[2] = {16, kBlockM};
+      if (const char* e = encode_tmap_strided(&tmBy, g.bn.mask, 2, dims, st, box, nullptr, 1, false)) return e;
+    }
     fill_bn(p, g.bn);
-    return n64 ? launch_p<64, 4, 1, 2>(tmA, tmB, tmD, p, stream, padd, &tmBx, has_y ? &tmBy : nullptr)
-               : launch_p<128, 3, 1, 2>(tmA, tmB, tmD, p, stream, padd, &tmBx, has_y ? &tmBy : nullptr);
+    const CUtensorMap* pby = (has_y || has_mask) ? &tmBy : nullptr;
+    return n64 ? launch_p<64, 4, 1, 2>(tmA, tmB, tmD, p, stream, padd, &tmBx, pby)
+               : launch_p<128, 3, 1, 2>(tmA, tmB, tmD, p, stream, padd, &tmBx, pby);
   }
   if (!g.b_mn_major) {
     if (wide) return launch_p<256, 3, 0>(tmA, tmB, tmD, p, stream, padd);
@@ -1009,6 +1047,7 @@ const char* conv3x3_bf16_persistent(const Conv3x3Args& a, int BH, int BN, int ti
   p.n_img = a.N; p.H = a.H; p.W = a.W; p.c_in_w = w_cin; p.BH = BH; p.BN = BN; p.tiles_h = tiles_h;
   p.stride = sd;
   if (dg && a.bn.x != nullptr) {
+    if (a.bn.mask != nullptr) return "fused BN-backward reduction with mask bits is a 1x1 dgrad feature";
     alignas(64) CUtensorMap tmBx, tmBy;
     const uint64_t dims[4] = {(uint64_t)cy, (uint64_t)a.W, (uint64_t)a.H, (uint64_t)a.N};
     const uint64_t st[3] = {(uint64_t)cy * 2, (uint64_t)a.W * cy * 2, (uint64_t)a.H * a.W * cy * 2};

@@ -8,32 +8,37 @@ namespace edl {
 
 // ---- bn.cu ----
 void bn_stats(const void* x, float* sums, int64_t M, int C, cudaStream_t stream);
-void bn_apply(const void* x, const void* res, void* y, const float* sums, const float* gamma,
+// mask (optional, residual + ReLU only): also write the ReLU mask bits uint8 [M, C / 8] of the stored output; needs
+// bn_relu_mask_supported(M, C)
+void bn_apply(const void* x, const void* res, void* y, void* mask, const float* sums, const float* gamma,
               const float* beta, float* running_mean, float* running_var, float* saved_mean,
               float* saved_rstd, int64_t M, int C, float eps, float momentum, bool relu,
               cudaStream_t stream);
 void scale_shift_act(const void* x, const void* res, void* y, const float* scale,
                      const float* shift, int64_t M, int C, bool relu, cudaStream_t stream);
-// y == nullptr with relu: the ReLU mask is recomputed from x (no residual case)
-void bn_bwd_reduce(const void* dy, const void* x, const void* y, const float* gamma,
+// ReLU mask: from the mask bits if given, else from y > 0 if given, else recomputed from x (no residual case)
+void bn_bwd_reduce(const void* dy, const void* x, const void* y, const void* mask, const float* gamma,
                    const float* beta, const float* saved_mean, const float* saved_rstd,
                    float* dsums, int64_t M, int C, bool relu, cudaStream_t stream);
-void bn_bwd_apply(const void* dy, const void* x, const void* y, const float* gamma,
+void bn_bwd_apply(const void* dy, const void* x, const void* y, const void* mask, const float* gamma,
                   const float* beta, const float* saved_mean, const float* saved_rstd,
                   const float* dsums, void* dx, void* dres, float* dgamma, float* dbeta, int64_t M,
                   int C, bool relu, bool accumulate, cudaStream_t stream);
+// the streaming kernels run (bn_set_stream_kernels) and can write / read mask bits for this shape
+bool bn_relu_mask_supported(int64_t M, int C);
 
 // ---- bn_stream.cu (cp.async.bulk + mbarrier streaming variants; used when supported) ----
 bool bn_stream_supported(int64_t M, int C);
+bool bn_mask_supported(int64_t M, int C);     // bn_stream_supported and C % 128 == 0
 void bn_stats_stream(const void* x, float* sums, int64_t M, int C, cudaStream_t s);
-void bn_apply_stream(const void* x, const void* res, void* y, const float* sums, const float* gamma,
+void bn_apply_stream(const void* x, const void* res, void* y, void* mask, const float* sums, const float* gamma,
                      const float* beta, float* running_mean, float* running_var, float* saved_mean,
                      float* saved_rstd, int64_t M, int C, float eps, float momentum, bool relu,
                      cudaStream_t s);
-void bn_bwd_reduce_stream(const void* dy, const void* x, const void* y, const float* gamma,
+void bn_bwd_reduce_stream(const void* dy, const void* x, const void* y, const void* mask, const float* gamma,
                           const float* beta, const float* saved_mean, const float* saved_rstd,
                           float* dsums, int64_t M, int C, bool relu, cudaStream_t s);
-void bn_bwd_apply_stream(const void* dy, const void* x, const void* y, const float* gamma,
+void bn_bwd_apply_stream(const void* dy, const void* x, const void* y, const void* mask, const float* gamma,
                          const float* beta, const float* saved_mean, const float* saved_rstd,
                          const float* dsums, void* dx, void* dres, float* dgamma, float* dbeta,
                          int64_t M, int C, bool relu, bool accumulate, cudaStream_t s);

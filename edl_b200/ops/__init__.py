@@ -83,7 +83,8 @@ def reset_fallbacks() -> None:
     _fallbacks.clear()
 
 
-from .bn import batch_norm_act, BatchNormAct2d, scale_shift_act, bn_stats_into, set_fused_bn, drop_bn_hook  # noqa: E402
+from .bn import (batch_norm_act, BatchNormAct2d, scale_shift_act, bn_stats_into, set_fused_bn, set_relu_mask,  # noqa: E402
+                 drop_bn_hook)
 from .loss import soft_cross_entropy, topk_accuracy  # noqa: E402
 from .pool import max_pool_3x3_s2, avg_pool_2x2, global_avg_pool  # noqa: E402
 from .optim import FlatSGDMomentum, FlatAdam, SparseAdam  # noqa: E402
@@ -104,5 +105,6 @@ __all__ = [
     "conv3x3_supported", "conv3x3_infer", "conv3x3_infer_supported", "stem7_infer", "stem7_supported",
     "conv3x3_wgrad", "conv3x3_wgrad_supported", "conv3x3_s2", "conv3x3_s2_infer", "conv3x3_s2_supported",
     "stem_conv", "stem_conv_supported", "conv3x3_pair", "conv3x3_pair_supported",
-    "rope", "rope_tables", "embedding_bag_mean", "normalize_u8", "DynamicLossScaler", "set_fused_bn", "drop_bn_hook",
+    "rope", "rope_tables", "embedding_bag_mean", "normalize_u8", "DynamicLossScaler", "set_fused_bn", "set_relu_mask",
+    "drop_bn_hook",
 ]

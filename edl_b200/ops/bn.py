@@ -23,6 +23,18 @@ def set_fused_bn(enabled: bool) -> None:
     _FUSED = bool(enabled)
 
 
+# ReLU after a residual add keeps its mask as bits (uint8 [M, C/8], written by the streaming apply kernel) instead of
+# the bf16 output; a consumer 1x1 dgrad that carries this BN's reduction then stores the gradient already masked, and
+# the backward needs neither the mask nor a separate residual gradient.  EDL_RELU_MASK=0 / set_relu_mask(False) saves
+# the output as before.
+_RELU_MASK = _os.environ.get("EDL_RELU_MASK", "1") == "1"
+
+
+def set_relu_mask(enabled: bool) -> None:
+    global _RELU_MASK
+    _RELU_MASK = bool(enabled)
+
+
 def _mc(x: torch.Tensor) -> torch.Tensor:
     """View an activation as a contiguous [M, C] matrix (C fastest)."""
     if x.dim() == 2:
@@ -70,18 +82,21 @@ class BNBackwardHook:
     """Left by a train-mode BatchNorm on its output tensor (``y._edl_bn_hook``).  The consumer of ``y`` (a
     wgmma 1x1 / 3x3 convolution) computes d(loss)/dy in its dgrad kernel; with this hook that kernel's
     epilogue also accumulates the BN-backward reduction (sum dy_masked, sum dy_masked * xhat) into ``dsums``
-    and sets ``done``, and the BN backward then skips its own reduction pass over (dy, x)."""
+    and sets ``done``, and the BN backward then skips its own reduction pass over (dy, x).  ``y`` (bf16 output) or
+    ``mask`` (its ReLU mask bits) is set for ReLU after a residual add; with ``mask`` the epilogue stores the gradient
+    already multiplied by the mask."""
 
-    __slots__ = ("x", "y", "mean", "rstd", "gamma", "beta", "relu", "dsums", "done")
+    __slots__ = ("x", "y", "mask", "mean", "rstd", "gamma", "beta", "relu", "dsums", "done")
 
     def __init__(self):
-        self.x = self.y = self.mean = self.rstd = self.gamma = self.beta = self.dsums = None
+        self.x = self.y = self.mask = self.mean = self.rstd = self.gamma = self.beta = self.dsums = None
         self.relu = False
         self.done = False
 
     def as_list(self, rows, channels):
         assert self.x.numel() == rows * channels
-        return [self.x, self.y, self.mean, self.rstd, self.gamma, self.beta, self.dsums]
+        return [self.x, self.mask if self.mask is not None else self.y, self.mean, self.rstd, self.gamma, self.beta,
+                self.dsums]
 
 
 def drop_bn_hook(t):
@@ -120,6 +135,7 @@ class _BNActFn(torch.autograd.Function):
         mean = torch.empty(ch, device=x.device, dtype=torch.float32)
         rstd = torch.empty(ch, device=x.device, dtype=torch.float32)
         res2 = _mc(res) if res is not None else None
+        mask = None
         if sums is None and _FUSED and C.bn_fused_fits(x2.shape[0], ch, 2 if res is not None else 1):
             # statistics + normalise in ONE SM-resident kernel (tensor crosses HBM once)
             sums = fwd_ws if fwd_ws is not None else torch.zeros(2 * ch, device=x.device, dtype=torch.float32)
@@ -131,16 +147,19 @@ class _BNActFn(torch.autograd.Function):
                 sums = fwd_ws if fwd_ws is not None else torch.zeros(2 * ch, device=x.device, dtype=torch.float32)
                 C.bn_stats(x2, sums)
                 count_launch()
-            C.bn_apply(x2, res2, _mc(y), sums, gamma, beta, rm, rv, mean, rstd, eps, momentum, relu)
+            if relu and res is not None and _RELU_MASK and not _FUSED and C.bn_relu_mask_supported(x2.shape[0], ch):
+                mask = torch.empty((x2.shape[0], ch // 8), device=x.device, dtype=torch.uint8)
+            C.bn_apply(x2, res2, _mc(y), sums, gamma, beta, rm, rv, mean, rstd, eps, momentum, relu, mask)
             count_launch()
-        # the saved output is only needed for the ReLU mask when a residual was added; otherwise the
-        # backward kernels recompute the mask from x (one fewer pass over the activation)
-        ctx.save_for_backward(x, y if (relu and res is not None) else None, gamma, mean, rstd, beta)
+        # the ReLU mask is only needed when a residual was added (otherwise the backward kernels recompute it from x):
+        # the mask bits when the apply kernel wrote them, else the saved output
+        y_saved = y if (relu and res is not None and mask is None) else None
+        ctx.save_for_backward(x, mask if mask is not None else y_saved, gamma, mean, rstd, beta)
         if hook is not None:
             # let the consumer's dgrad kernel carry this layer's backward reduction
             if bwd_ws is None:
                 bwd_ws = ctx.bwd_ws = torch.zeros(2 * ch, device=x.device, dtype=torch.float32)
-            hook.x, hook.y = x, (y if (relu and res is not None) else None)
+            hook.x, hook.y, hook.mask = x, y_saved, mask
             hook.mean, hook.rstd, hook.gamma, hook.beta = mean, rstd, gamma, beta
             hook.relu, hook.dsums = relu, bwd_ws
             ctx.hook = hook
@@ -183,16 +202,26 @@ class _BNActFn(torch.autograd.Function):
         if dsums is None:
             dsums = torch.zeros(2 * ch, device=x.device, dtype=torch.float32)
         x2, dy2 = _mc(x), _mc(dy)
-        y2 = _mc(y) if (relu and y is not None) else None
+        # y: the bf16 output, or the uint8 ReLU mask bits [M, C/8] (which the kernels take in its place)
+        is_mask = y is not None and y.dtype == torch.uint8
+        y2 = (y if is_mask else _mc(y)) if (relu and y is not None) else None
+        # the consumer's dgrad epilogue reduced dy AND stored it multiplied by the mask: dy is the residual gradient
+        premasked = is_mask and ctx.hook is not None and ctx.hook.done
         dx = torch.empty_like(x)
-        dres = torch.empty_like(x) if has_res else None
+        dres = torch.empty_like(x) if (has_res and not premasked) else None
         if sink_g is not None:
             dg, db, acc = sink_g, sink_b, True
         else:
             dg = torch.empty_like(gamma)
             db = torch.empty_like(gamma)
             acc = False
-        if _FUSED and C.bn_fused_fits(x2.shape[0], ch, 3 if y2 is not None else 2):
+        if premasked:
+            count_launch(1)
+            C.bn_bwd_apply(dy2, x2, None, gamma, beta, mean, rstd, dsums, _mc(dx), None, dg, db, False, acc)
+            # dres aliases dy.  Whatever later adds into this buffer in place (autograd accumulating gradients) runs
+            # on this stream after the kernel just enqueued, which has then read dy.
+            dres = dy if has_res else None
+        elif _FUSED and not is_mask and C.bn_fused_fits(x2.shape[0], ch, 3 if y2 is not None else 2):
             sync = ctx.sync_ws[1:2] if ctx.sync_ws is not None else torch.zeros(1, device=x.device,
                                                                                dtype=torch.int32)
             C.bn_bwd_fused(dy2, x2, y2, gamma, beta, mean, rstd, dsums, _mc(dx),

@@ -506,7 +506,8 @@ class _Conv3x3Fn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             if conv3x3_supported(dy, w, dgrad=True):
                 dx = torch.empty_like(x)
-                hook = ctx.bn_hook if _bn_fusable(ctx.bn_hook, x, x.shape[1]) else None
+                # (mask bits are a 1x1 dgrad feature; a residual BN does not feed a 3x3 convolution in these models)
+                hook = ctx.bn_hook if _bn_fusable(ctx.bn_hook, x, x.shape[1]) and ctx.bn_hook.mask is None else None
                 if hook is not None:
                     native().conv3x3(dy, w, dx, True, None, hook.as_list(dx.numel() // dx.shape[1], dx.shape[1]), hook.relu)
                     hook.done = True
