@@ -7,6 +7,7 @@ statistics reduced in the GEMM epilogue, and whose BN-apply / residual-add / ReL
 """
 from __future__ import annotations
 
+import functools
 import math
 import os
 from typing import List, Optional
@@ -44,44 +45,31 @@ class ConvBNAct(nn.Module):
                 and x.dtype == torch.bfloat16 and self.cin % 8 == 0 and self.cout % 8 == 0)
 
     def conv(self, x, want_stats, fork=False):
+        op = None
         if self._use_gemm(x):
-            stats = None
-            if want_stats:
-                stats = self.fwd_stats if self.fwd_stats is not None else torch.zeros(
-                    2 * self.cout, device=x.device, dtype=torch.float32)
-            return ops.conv1x1(x, self.weight, stats, fork=fork), stats
-        if (self.k == 3 and self.stride == 1 and self.groups == 1 and self.impl != "cudnn" and self.own_conv3
+            op = functools.partial(ops.conv1x1, fork=fork)
+        elif (self.k == 3 and self.stride == 1 and self.groups == 1 and self.impl != "cudnn" and self.own_conv3
                 and ops.conv3x3_supported(x, self.weight)):
             # own wgmma implicit-GEMM 3x3 (csrc/conv3x3.cu) with the BN statistics in its epilogue
-            stats = None
-            if want_stats:
-                stats = self.fwd_stats if self.fwd_stats is not None else torch.zeros(
-                    2 * self.cout, device=x.device, dtype=torch.float32)
-            return ops.conv3x3(x, self.weight, stats), stats
-        if (self.k == 3 and self.stride == 1 and self.groups == 1 and self.cin == 32 and self.impl != "cudnn"
+            op = ops.conv3x3
+        elif (self.k == 3 and self.stride == 1 and self.groups == 1 and self.cin == 32 and self.impl != "cudnn"
                 and self.own_conv3 and ops.conv3x3_pair_supported(x, self.weight)):
             # EDL_OWN_STEM23=1: 32-channel stem convolutions in pixel-pair form on the wgmma 3x3 kernels
-            stats = None
-            if want_stats:
-                stats = self.fwd_stats if self.fwd_stats is not None else torch.zeros(
-                    2 * self.cout, device=x.device, dtype=torch.float32)
-            return ops.conv3x3_pair(x, self.weight, stats), stats
-        if (self.k == 3 and self.stride == 2 and self.cin == 3 and self.cout == 32 and self.impl != "cudnn"
+            op = ops.conv3x3_pair
+        elif (self.k == 3 and self.stride == 2 and self.cin == 3 and self.cout == 32 and self.impl != "cudnn"
                 and ops.gemm.OWN_STEM1 and ops.stem_conv_supported(x, self.weight)):
             # experimental (EDL_OWN_STEM1=1): direct kernel for the K = 27 stem convolution, statistics fused
-            stats = None
-            if want_stats:
-                stats = self.fwd_stats if self.fwd_stats is not None else torch.zeros(
-                    2 * self.cout, device=x.device, dtype=torch.float32)
-            return ops.stem_conv(x, self.weight, stats), stats
-        if (self.k == 3 and self.stride == 2 and self.groups == 1 and self.impl != "cudnn" and self.own_conv3
+            op = ops.stem_conv
+        elif (self.k == 3 and self.stride == 2 and self.groups == 1 and self.impl != "cudnn" and self.own_conv3
                 and ops.gemm.CONV3_S2 and ops.conv3x3_s2_supported(x, self.weight)):
             # experimental (EDL_CONV3_S2=1): stride-2 fprop on the wgmma kernel, statistics in its epilogue
+            op = ops.conv3x3_s2
+        if op is not None:
             stats = None
             if want_stats:
                 stats = self.fwd_stats if self.fwd_stats is not None else torch.zeros(
                     2 * self.cout, device=x.device, dtype=torch.float32)
-            return ops.conv3x3_s2(x, self.weight, stats), stats
+            return op(x, self.weight, stats), stats
         if self.split_backward and torch.is_grad_enabled() and self.weight.requires_grad:
             # library conv whose wgrad half runs on the side stream (ops/gemm.py:_ConvLibFn)
             return ops.conv_lib(x, self.weight, self.stride, (self.k - 1) // 2, self.groups), None

@@ -113,19 +113,14 @@ def _split_k_for(m, n, k):
 
 
 _WS = {}
-_SIDE = {"stream": None, "streams": [], "next": 0, "keep": []}
+_SIDE = {"streams": [], "next": 0, "keep": []}
 
 
-def set_wgrad_stream(stream):
-    """Run weight-gradient GEMMs on ``stream`` (the DP engine passes its communication stream): they
-    then overlap the dgrad / BN-backward chain of the main stream, and the bucket all-reduces that
-    follow on the same stream are naturally ordered behind them.  ``None`` disables the overlap."""
-    if isinstance(stream, (list, tuple)):
-        _SIDE["streams"] = [st for st in stream if st is not None]
-        _SIDE["stream"] = _SIDE["streams"][0] if _SIDE["streams"] else None
-    else:
-        _SIDE["stream"] = stream
-        _SIDE["streams"] = [stream] if stream is not None else []
+def set_wgrad_stream(streams):
+    """Run the weight gradients that go into a gradient sink on ``streams`` (a list; the DP engine passes its
+    weight-gradient streams): they then overlap the dgrad / BN-backward chain of the main stream.  ``None``
+    disables the overlap."""
+    _SIDE["streams"] = [st for st in streams or () if st is not None]
     _SIDE["next"] = 0
     _SIDE["keep"].clear()
 
@@ -181,29 +176,49 @@ def _splitk_partials(device):
     return buf
 
 
+def _grad_sink(param):
+    """``(sink, ready)`` of a parameter whose gradient goes straight into its window of the flat gradient bucket
+    (parallel/flat.py) instead of ``param.grad``; ``(None, None)`` for any other parameter and outside autograd."""
+    sink = getattr(param, "_edl_grad_sink", None) if torch.is_grad_enabled() else None
+    return sink, (getattr(param, "_edl_grad_ready", None) if sink is not None else None)
+
+
+def _deliver_wgrad(dy, x, sink, ready, compute):
+    """One layer's weight gradient: ``compute(sink)`` adds it into ``sink``, ``compute(None)`` returns it.
+
+    Without a sink it is computed here and returned to autograd.  With one it runs on the next weight-gradient
+    stream, behind the work already queued on the current stream, ``ready()`` is called with that stream still
+    current and None is returned; ``dy`` and ``x`` stay referenced until the engine has joined the streams
+    (``release_wgrad_keepalive``)."""
+    if sink is None:
+        return compute(None)
+    if _SKIP_WGRAD:
+        if ready is not None:
+            ready()
+        return None
+    side = _side_stream() if dy.is_cuda else None
+    if side is not None:
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(dy.device))
+        side.wait_event(ev)
+        _SIDE["keep"].append((dy, x))
+    with torch.cuda.stream(side):        # None: stay on the current stream
+        compute(sink)
+        if ready is not None:
+            ready()
+    return None
+
+
 def _wgrad(dy2, x2, weight_shape, sink, ready):
     """dW[Cout, Cin] = dy2[M, Cout]^T @ x2[M, Cin]: fp32 split-K accumulation whose last CTA per
     tile converts to bf16 straight into the (flat gradient bucket) sink -- no memset / cast / add
     kernels around it."""
-    if _SKIP_WGRAD and sink is not None:
-        if ready is not None:
-            ready()
-        return None
+    return _deliver_wgrad(dy2, x2, sink, ready, lambda s: _wgrad_impl(dy2, x2, weight_shape, s))
+
+
+def _wgrad_impl(dy2, x2, weight_shape, sink):
     cout, cin = dy2.shape[1], x2.shape[1]
     split = _split_k_for(cout, cin, dy2.shape[0])
-    side = _side_stream() if (dy2.is_cuda and sink is not None) else None
-    if side is not None:
-        cur = torch.cuda.current_stream(dy2.device)
-        ev = torch.cuda.Event()
-        ev.record(cur)
-        side.wait_event(ev)
-        _SIDE["keep"].append((dy2, x2))          # operands must outlive the side-stream kernel
-        with torch.cuda.stream(side):
-            return _wgrad_impl(dy2, x2, weight_shape, sink, ready, cout, cin, split)
-    return _wgrad_impl(dy2, x2, weight_shape, sink, ready, cout, cin, split)
-
-
-def _wgrad_impl(dy2, x2, weight_shape, sink, ready, cout, cin, split):
     if dy2.is_cuda and cin % 4 == 0:
         tiles = ((cout + 127) // 128) * ((cin + 63) // 64)
         ws, counters = _splitk_workspace(dy2.device, cout * cin, tiles)
@@ -214,19 +229,12 @@ def _wgrad_impl(dy2, x2, weight_shape, sink, ready, cout, cin, split):
         gemm_bf16(dy2, x2, a_mn_major=True, b_mn_major=True, out_f32=ws[:cout * cin].view(cout, cin),
                   split_k=split, out_bf16=out, tile_counters=counters, accumulate_out=acc,
                   partials=_splitk_partials(dy2.device) if split > 1 else None)
-        if sink is not None:
-            if ready is not None:
-                ready()
-            return None
-        return out.view(weight_shape)
+        return None if sink is not None else out.view(weight_shape)
     acc = torch.zeros((cout, cin), device=dy2.device, dtype=torch.float32)
     gemm_bf16(dy2, x2, a_mn_major=True, b_mn_major=True, out_f32=acc, split_k=split)
-    if sink is not None:
-        sink.view(cout, cin).add_(acc)
-        if ready is not None:
-            ready()
-        return None
-    return acc.to(torch.bfloat16).view(weight_shape)
+    if sink is None:
+        return acc.to(torch.bfloat16).view(weight_shape)
+    sink.view(cout, cin).add_(acc)
 
 
 class _Conv1x1Fn(torch.autograd.Function):
@@ -281,9 +289,7 @@ def conv1x1(x, weight, stats: Optional[torch.Tensor] = None, fork: bool = False)
     """NHWC 1x1 stride-1 convolution as a wgmma GEMM.  ``weight``: [Cout, 1, 1, Cin] or
     [Cout, Cin] bf16.  If ``stats`` (pre-zeroed fp32 [2*Cout]) is given, the epilogue accumulates
     per-channel sum / sum-of-squares of the output for the following train-mode BatchNorm."""
-    sink = getattr(weight, "_edl_grad_sink", None) if torch.is_grad_enabled() else None
-    ready = getattr(weight, "_edl_grad_ready", None) if sink is not None else None
-    return _Conv1x1Fn.apply(x, weight, stats, sink, ready, fork, getattr(x, "_edl_bn_hook", None))
+    return _Conv1x1Fn.apply(x, weight, stats, *_grad_sink(weight), fork, getattr(x, "_edl_bn_hook", None))
 
 
 def _bn_fusable(hook, x, channels) -> bool:
@@ -348,12 +354,7 @@ class _LinearFn(torch.autograd.Function):
 def linear_bf16(x, weight, bias=None, relu=False):
     """y = act(x @ weight^T + bias) on the wgmma GEMM (bias/activation fused in the epilogue).
     x [M, K] bf16, weight [N, K] bf16, bias [N] (any float dtype)."""
-    grad = torch.is_grad_enabled()
-    sink = getattr(weight, "_edl_grad_sink", None) if grad else None
-    ready = getattr(weight, "_edl_grad_ready", None) if sink is not None else None
-    bsink = getattr(bias, "_edl_grad_sink", None) if (grad and bias is not None) else None
-    bready = getattr(bias, "_edl_grad_ready", None) if bsink is not None else None
-    return _LinearFn.apply(x, weight, bias, relu, sink, ready, bsink, bready)
+    return _LinearFn.apply(x, weight, bias, relu, *_grad_sink(weight), *_grad_sink(bias))
 
 
 # EDL_PAIR_WGRAD=0: the library's weight gradient for the 32-channel stem convolutions as well
@@ -379,6 +380,25 @@ def _count_lib_conv(x, what, w_krsc, stride, groups):
                                                                                       cin * groups, cout))
 
 
+def _lib_dgrad(dy, x, w, cfg):
+    """Input gradient of the convolution ``cfg`` = (stride, padding, groups), KRSC weight ``w``, on the library."""
+    stride, padding, groups = cfg
+    _count_lib_conv(x, "dgrad", w, stride, groups)
+    return torch.ops.aten.convolution_backward(dy, x, w.permute(0, 3, 1, 2), None, [stride, stride], [padding, padding],
+                                               [1, 1], False, [0, 0], groups, [True, False, False])[0]
+
+
+def _lib_wgrad(dy, x, w, cfg, sink):
+    """Weight gradient (KRSC) of the same convolution on the library: added into ``sink``, or returned without one."""
+    stride, padding, groups = cfg
+    _count_lib_conv(x, "wgrad", w, stride, groups)
+    gw = torch.ops.aten.convolution_backward(dy, x, w.permute(0, 3, 1, 2), None, [stride, stride], [padding, padding],
+                                             [1, 1], False, [0, 0], groups, [False, True, False])[1].permute(0, 2, 3, 1)
+    if sink is None:
+        return gw.contiguous()
+    sink.view(w.shape).add_(gw)
+
+
 class _ConvLibFn(torch.autograd.Function):
     """k x k / strided / grouped convolution on the library kernel (cuDNN) with the backward split in
     two: dgrad stays on the critical path, wgrad runs on the side stream next to the wgmma wgrad
@@ -396,73 +416,22 @@ class _ConvLibFn(torch.autograd.Function):
         return y
 
     @staticmethod
-    def _bwd(dy, x, wv, cfg, mask):
-        stride, padding, groups = cfg
-        _count_lib_conv(x, "dgrad" if mask[0] else "wgrad", wv.permute(0, 2, 3, 1), stride, groups)
-        return torch.ops.aten.convolution_backward(dy, x, wv, None, [stride, stride], [padding, padding], [1, 1],
-                                                   False, [0, 0], groups, mask)
-
-    @staticmethod
     def backward(ctx, dy):
         x, w = ctx.saved_tensors
-        wv = w.permute(0, 3, 1, 2)
-        dx = None
-        if ctx.needs_input_grad[0]:
-            dx = _ConvLibFn._bwd(dy, x, wv, ctx.cfg, [True, False, False])[0]
+        dx = _lib_dgrad(dy, x, w, ctx.cfg) if ctx.needs_input_grad[0] else None
         dw = None
         if ctx.needs_input_grad[1]:
-            sink, ready = ctx.sink, ctx.ready
-            side = _side_stream() if (dy.is_cuda and sink is not None) else None
-
-            def wgrad():
-                if _SKIP_WGRAD and sink is not None:
-                    if ready is not None:
-                        ready()
-                    return None
-                if _pair_wgrad_ok(x, dy, w, ctx.cfg):
-                    # 32-input-channel 3x3 / stride 1 layer (the stem's conv1_2 / conv1_3): weight gradient in pixel-pair
-                    # form on the wgmma kernel even when fprop / dgrad stay on the library (these two
-                    # layers are the END of backward, where nothing hides a slow kernel)
-                    from . import native, count_launch
-                    xc, dyc = _cl(x), _cl(dy)
-                    x2, dy2 = _pair_view(xc), _pair_view(dyc)
-                    dw2 = conv3x3_wgrad(x2, dy2, (2 * w.shape[0], 3, 3, 64), None)
-                    out = sink.view(w.shape) if sink is not None else torch.empty_like(w)
-                    native().pair_weight_fold(dw2, out, sink is not None)
-                    count_launch()
-                    if sink is None:
-                        return out
-                    if ready is not None:
-                        ready()
-                    return None
-                gw = _ConvLibFn._bwd(dy, x, wv, ctx.cfg, [False, True, False])[1].permute(0, 2, 3, 1)
-                if sink is None:
-                    return gw.contiguous()
-                sink.view(w.shape).add_(gw)
-                if ready is not None:
-                    ready()
-                return None
-
-            if side is not None:
-                cur = torch.cuda.current_stream(dy.device)
-                ev = torch.cuda.Event()
-                ev.record(cur)
-                side.wait_event(ev)
-                _SIDE["keep"].append((dy, x))
-                with torch.cuda.stream(side):
-                    dw = wgrad()
-                    # temporaries of the side stream must not be recycled by main-stream allocations
-                    # before the streams are joined
-                    _SIDE["keep"].append(None)
-            else:
-                dw = wgrad()
+            # 32-input-channel 3x3 / stride 1 layer (the stem's conv1_2 / conv1_3): weight gradient in pixel-pair form
+            # on the wgmma kernel even when fprop / dgrad stay on the library (these two layers are the END of
+            # backward, where nothing hides a slow kernel)
+            pair = _pair_wgrad_ok(x, dy, w, ctx.cfg)
+            dw = _deliver_wgrad(dy, x, ctx.sink, ctx.ready, lambda sink: (
+                _pair_wgrad(x, dy, w, sink) if pair else _lib_wgrad(dy, x, w, ctx.cfg, sink)))
         return dx, dw, None, None, None, None, None
 
 
 def conv_lib(x, weight_krsc, stride=1, padding=0, groups=1):
-    sink = getattr(weight_krsc, "_edl_grad_sink", None) if torch.is_grad_enabled() else None
-    ready = getattr(weight_krsc, "_edl_grad_ready", None) if sink is not None else None
-    return _ConvLibFn.apply(x, weight_krsc, stride, padding, groups, sink, ready)
+    return _ConvLibFn.apply(x, weight_krsc, stride, padding, groups, *_grad_sink(weight_krsc))
 
 
 def conv3x3_supported(x, weight_krsc, dgrad=False) -> bool:
@@ -500,7 +469,6 @@ class _Conv3x3Fn(torch.autograd.Function):
 
         x, w = ctx.saved_tensors
         dy = _cl(dy)
-        wv = w.permute(0, 3, 1, 2)
         cfg = (1, 1, 1)
         dx = None
         if ctx.needs_input_grad[0]:
@@ -515,42 +483,12 @@ class _Conv3x3Fn(torch.autograd.Function):
                     native().conv3x3(dy, w, dx, True, None, None, False)
                 count_launch()
             else:
-                dx = _ConvLibFn._bwd(dy, x, wv, cfg, [True, False, False])[0]
+                dx = _lib_dgrad(dy, x, w, cfg)
         dw = None
         if ctx.needs_input_grad[1]:
-            sink, ready = ctx.sink, ctx.ready
-            side = _side_stream() if sink is not None else None
             own = OWN_WGRAD3 and conv3x3_wgrad_supported(x, w)
-
-            def wgrad():
-                if _SKIP_WGRAD and sink is not None:
-                    if ready is not None:
-                        ready()
-                    return None
-                if own:
-                    out = conv3x3_wgrad(x, dy, w.shape, sink)
-                    if sink is None:
-                        return out
-                    if ready is not None:
-                        ready()
-                    return None
-                gw = _ConvLibFn._bwd(dy, x, wv, cfg, [False, True, False])[1].permute(0, 2, 3, 1)
-                if sink is None:
-                    return gw.contiguous()
-                sink.view(w.shape).add_(gw)
-                if ready is not None:
-                    ready()
-                return None
-
-            if side is not None:
-                ev = torch.cuda.Event()
-                ev.record(torch.cuda.current_stream(dy.device))
-                side.wait_event(ev)
-                _SIDE["keep"].append((dy, x))
-                with torch.cuda.stream(side):
-                    dw = wgrad()
-            else:
-                dw = wgrad()
+            dw = _deliver_wgrad(dy, x, ctx.sink, ctx.ready, lambda sink: (
+                conv3x3_wgrad(x, dy, w.shape, sink) if own else _lib_wgrad(dy, x, w, cfg, sink)))
         return dx, dw, None, None, None, None
 
 
@@ -603,9 +541,7 @@ def conv3x3_wgrad(x, dy, weight_shape, sink=None, split_k: Optional[int] = None)
 def conv3x3(x, weight_krsc, stats: Optional[torch.Tensor] = None):
     """NHWC 3x3 stride-1 pad-1 convolution; ``stats`` (pre-zeroed fp32 [2*Cout]) receives the per-channel
     sum / sum of squares of the output for the following train-mode BatchNorm."""
-    sink = getattr(weight_krsc, "_edl_grad_sink", None) if torch.is_grad_enabled() else None
-    ready = getattr(weight_krsc, "_edl_grad_ready", None) if sink is not None else None
-    return _Conv3x3Fn.apply(x, weight_krsc, stats, sink, ready, getattr(x, "_edl_bn_hook", None))
+    return _Conv3x3Fn.apply(x, weight_krsc, stats, *_grad_sink(weight_krsc), getattr(x, "_edl_bn_hook", None))
 
 
 # 3x3 / pad 1 / STRIDE 2 forward convolutions (student: first block of stages 2-4; teacher: the grouped ones, which
@@ -698,49 +634,16 @@ class _Conv3x3S2Fn(torch.autograd.Function):
                 native().conv3x3_dgrad_s2(dy, w, dx)
                 count_launch(4)
             else:
-                dx = _ConvLibFn._bwd(dy, x, w.permute(0, 3, 1, 2), ctx.cfg, [True, False, False])[0]
+                dx = _lib_dgrad(dy, x, w, ctx.cfg)
         if ctx.needs_input_grad[1]:
-            if _s2_wgrad_supported(x, w):
-                sink, ready = ctx.sink, ctx.ready
-                side = _side_stream() if sink is not None else None
-
-                def wgrad():
-                    out = conv3x3_wgrad(x, dy, w.shape, sink)
-                    if sink is not None and ready is not None:
-                        ready()
-                    return out
-
-                if side is not None:
-                    ev = torch.cuda.Event()
-                    ev.record(torch.cuda.current_stream(dy.device))
-                    side.wait_event(ev)
-                    _SIDE["keep"].append((dy, x))
-                    with torch.cuda.stream(side):
-                        dw = wgrad()
-                else:
-                    dw = wgrad()
-            else:
-                ctx2 = ctx
-                saved = ctx.needs_input_grad
-                dw = _ConvLibFn.backward(_NeedsOnlyWeight(ctx2, saved), dy)[1]
+            own = _s2_wgrad_supported(x, w)
+            dw = _deliver_wgrad(dy, x, ctx.sink, ctx.ready, lambda sink: (
+                conv3x3_wgrad(x, dy, w.shape, sink) if own else _lib_wgrad(dy, x, w, ctx.cfg, sink)))
         return dx, dw, None, None, None
 
 
-class _NeedsOnlyWeight:
-    """View of an autograd ctx that asks _ConvLibFn.backward for the weight gradient only."""
-
-    def __init__(self, ctx, needs):
-        self._ctx = ctx
-        self.needs_input_grad = (False, needs[1]) + tuple(needs[2:])
-
-    def __getattr__(self, k):
-        return getattr(self._ctx, k)
-
-
 def conv3x3_s2(x, weight_krsc, stats: Optional[torch.Tensor] = None):
-    sink = getattr(weight_krsc, "_edl_grad_sink", None) if torch.is_grad_enabled() else None
-    ready = getattr(weight_krsc, "_edl_grad_ready", None) if sink is not None else None
-    return _Conv3x3S2Fn.apply(x, weight_krsc, stats, sink, ready)
+    return _Conv3x3S2Fn.apply(x, weight_krsc, stats, *_grad_sink(weight_krsc))
 
 
 # The first stem convolution (3 -> 32 channels, 3x3 / stride 2) runs on the direct kernel of csrc/stem.cu with the
@@ -817,46 +720,24 @@ class _StemConvFn(torch.autograd.Function):
         dy = _cl(dy)
         dx = None
         if ctx.needs_input_grad[0]:      # nobody asks for the gradient of the images; kept for completeness
-            dx = _ConvLibFn._bwd(dy, x, w.permute(0, 3, 1, 2), ctx.cfg, [True, False, False])[0]
+            dx = _lib_dgrad(dy, x, w, ctx.cfg)
         dw = None
         if ctx.needs_input_grad[1]:
-            if not (x.shape[2] % 2 == 0 and x.shape[3] % 2 == 0 and x.shape[3] <= 4096):
-                dw = _ConvLibFn.backward(_NeedsOnlyWeight(ctx, ctx.needs_input_grad), dy)[1]
-                return dx, dw, None, None, None
-            sink, ready = ctx.sink, ctx.ready
-            side = _side_stream() if sink is not None else None
-
-            def wgrad():
-                if _SKIP_WGRAD and sink is not None:
-                    if ready is not None:
-                        ready()
-                    return None
+            def wgrad(sink):
+                if not (x.shape[2] % 2 == 0 and x.shape[3] % 2 == 0 and x.shape[3] <= 4096):
+                    return _lib_wgrad(dy, x, w, ctx.cfg, sink)
                 ws, counters = _splitk_workspace(x.device, 1024, 1)
                 out = sink.view(w.shape) if sink is not None else torch.empty_like(w)
                 native().stem_wgrad(x, dy, out, ws, counters, sink is not None)
                 count_launch()
-                if sink is not None:
-                    if ready is not None:
-                        ready()
-                    return None
-                return out
+                return None if sink is not None else out
 
-            if side is not None:
-                ev = torch.cuda.Event()
-                ev.record(torch.cuda.current_stream(dy.device))
-                side.wait_event(ev)
-                _SIDE["keep"].append((dy, x))
-                with torch.cuda.stream(side):
-                    dw = wgrad()
-            else:
-                dw = wgrad()
+            dw = _deliver_wgrad(dy, x, ctx.sink, ctx.ready, wgrad)
         return dx, dw, None, None, None
 
 
 def stem_conv(x, weight_krsc, stats: Optional[torch.Tensor] = None):
-    sink = getattr(weight_krsc, "_edl_grad_sink", None) if torch.is_grad_enabled() else None
-    ready = getattr(weight_krsc, "_edl_grad_ready", None) if sink is not None else None
-    return _StemConvFn.apply(x, weight_krsc, stats, sink, ready)
+    return _StemConvFn.apply(x, weight_krsc, stats, *_grad_sink(weight_krsc))
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -874,6 +755,18 @@ def _pair_view(t):
 def _unpair_view(t2):
     n, c2, h, w2 = t2.shape
     return t2.as_strided((n, c2 // 2, h, 2 * w2), (h * w2 * c2, 1, w2 * c2, c2 // 2))
+
+
+def _pair_wgrad(x, dy, w, sink):
+    """Weight gradient of a 3x3 / stride 1 convolution with 32 input channels in pixel-pair form: the 64-channel wgmma
+    weight gradient over pixel pairs, folded back to ``w``'s [Cout, 3, 3, 32] (added into ``sink``, or returned)."""
+    from . import native, count_launch
+
+    dw2 = conv3x3_wgrad(_pair_view(_cl(x)), _pair_view(_cl(dy)), (2 * w.shape[0], 3, 3, 64), None)
+    out = sink.view(w.shape) if sink is not None else torch.empty_like(w)
+    native().pair_weight_fold(dw2, out, sink is not None)
+    count_launch()
+    return None if sink is not None else out
 
 
 def conv3x3_pair_supported(x, weight_krsc) -> bool:
@@ -927,41 +820,12 @@ class _Conv3x3PairFn(torch.autograd.Function):
             dx = _unpair_view(dx2)
         dw = None
         if ctx.needs_input_grad[1]:
-            sink, ready = ctx.sink, ctx.ready
-            side = _side_stream() if sink is not None else None
-
-            def wgrad():
-                if _SKIP_WGRAD and sink is not None:
-                    if ready is not None:
-                        ready()
-                    return None
-                dw2 = conv3x3_wgrad(x2, dy2, w2.shape, None)
-                out = sink.view(w.shape) if sink is not None else torch.empty_like(w)
-                C.pair_weight_fold(dw2, out, sink is not None)
-                count_launch()
-                if sink is not None:
-                    if ready is not None:
-                        ready()
-                    return None
-                return out
-
-            if side is not None:
-                ev = torch.cuda.Event()
-                ev.record(torch.cuda.current_stream(dy.device))
-                side.wait_event(ev)
-                _SIDE["keep"].append((dy, x))
-                with torch.cuda.stream(side):
-                    dw = wgrad()
-                    _SIDE["keep"].append(None)
-            else:
-                dw = wgrad()
+            dw = _deliver_wgrad(dy, x, ctx.sink, ctx.ready, lambda sink: _pair_wgrad(x, dy, w, sink))
         return dx, dw, None, None, None
 
 
 def conv3x3_pair(x, weight_krsc, stats: Optional[torch.Tensor] = None):
-    sink = getattr(weight_krsc, "_edl_grad_sink", None) if torch.is_grad_enabled() else None
-    ready = getattr(weight_krsc, "_edl_grad_ready", None) if sink is not None else None
-    return _Conv3x3PairFn.apply(x, weight_krsc, stats, sink, ready)
+    return _Conv3x3PairFn.apply(x, weight_krsc, stats, *_grad_sink(weight_krsc))
 
 
 def conv3x3_infer_supported(x, weight_krsc, groups=1) -> bool:
