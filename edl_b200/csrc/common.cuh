@@ -91,6 +91,22 @@ EDL_DEVICE void red_add8(float* dst, const float* v) {
   }
 }
 
+// dst[0..3] = bf16(v), or bf16(dst + v) when accumulating (the sum in fp32, one rounding); dst 8-byte aligned
+EDL_DEVICE void store_bf16x4(__nv_bfloat16* dst, float4 v, bool accumulate) {
+  if (accumulate) {
+    const uint2 old = *reinterpret_cast<const uint2*>(dst);
+    const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.x));
+    const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.y));
+    v.x += a.x; v.y += a.y; v.z += b.x; v.w += b.y;
+  }
+  const __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y);
+  const __nv_bfloat162 hi = __floats2bfloat162_rn(v.z, v.w);
+  uint2 packed;
+  packed.x = *reinterpret_cast<const uint32_t*>(&lo);
+  packed.y = *reinterpret_cast<const uint32_t*>(&hi);
+  *reinterpret_cast<uint2*>(dst) = packed;
+}
+
 EDL_DEVICE float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));

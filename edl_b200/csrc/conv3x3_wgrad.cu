@@ -11,14 +11,13 @@
 //                                                              unit (= the padding; no im2col, no index math)
 // One CTA owns a 128 (Cout) x 64 (Cin) tile of ONE FILTER ROW r: the dY tile of a pixel block is loaded once
 // and multiplied with the three shifted X tiles (s = 0, 1, 2) into three register accumulators, so dY crosses
-// L2 -> SM once per row instead of once per tap.  The pixel reduction is split over gridDim.z CTAs; partial
-// tiles are pushed with coalesced red.global.add.v4.f32 into an all-zero fp32 workspace laid out like the
-// KRSC weight, and the LAST CTA of a tile converts it to bf16 straight into the flat gradient bucket
-// (+= when accumulating) and re-zeroes the workspace -- the same fused finalize as the 1x1 wgrad GEMM (gemm.cu).
+// L2 -> SM once per row instead of once per tap.  Without a split of the pixel reduction the CTA writes its tile as
+// bf16 straight into the flat gradient bucket (+= when accumulating); split over gridDim.z CTAs, every CTA stores its
+// fp32 partial tile and splitk_reduce sums them into the bucket -- the same scheme as the 1x1 wgrad GEMM (gemm.cu).
 //
 //   warp 0      : TMA producer (2 + 3 box loads per pixel block into a 3-stage ring)
 //   warps 4..11 : two consumer warpgroups, one per 64-channel chunk of dY: wgmma.mma_async into three 64 x 64 fp32
-//                 register accumulators (one per tap), then the epilogue (smem staging -> vector reductions / finalize)
+//                 register accumulators (one per tap), then the epilogue (smem staging -> bf16 or partial-tile stores)
 #include <cuda.h>
 
 #include "gemm.h"
@@ -48,12 +47,10 @@ struct WgradParams {
   int KB;                    // pixel rows per block = W * BH * NB (multiple of 16, <= kMaxKB)
   int total_kb, kb_per_split;
   int tiles_n;
-  float* ws;                 // fp32 [Cout][9*Cin], all zero on entry and on exit
   __nv_bfloat16* out;        // bf16 [Cout][9*Cin] (KRSC)
-  int* counters;             // [tiles * 3], zero on entry and on exit
   int accumulate;
   int stride;                // 1, or 2: X rows 2*h + r - 1 (the columns are subsampled by the tensor map)
-  float* part;               // split-K partial tiles [split][ctas][128 x 192] (no atomics) or nullptr
+  float* part;               // split-K partial tiles [split][ctas][128 x 192] (gridDim.z > 1)
 };
 
 __global__ void __launch_bounds__(kThreads, 1)
@@ -64,7 +61,6 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kBarOffset);
   uint64_t* empty_bar = full_bar + kStages;
-  uint32_t* s_last = reinterpret_cast<uint32_t*>(empty_bar + kStages);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -158,71 +154,19 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");
         const int64_t col0 = (int64_t)(r * 3 + s) * p.Cin + n0;
+#pragma unroll 1   // one 16-byte piece per iteration, as in version 2 below
         for (int f = et; f < rows_valid * kVecPerRow; f += kEpiThreads) {
           const int rr = f / kVecPerRow, c4 = (f % kVecPerRow) * 4;
-          float4 t = *reinterpret_cast<const float4*>(sf + rr * kPitch + c4 * 4);
-          const int64_t off = (int64_t)(m0 + rr) * ldw + col0 + c4;
+          const float4 t = *reinterpret_cast<const float4*>(sf + rr * kPitch + c4 * 4);
           if (direct) {
             // this CTA saw every pixel: bf16 (+= bucket) straight from the staged tile
-            __nv_bfloat16* o = p.out + off;
-            if (p.accumulate) {
-              const uint2 old = *reinterpret_cast<const uint2*>(o);
-              const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.x));
-              const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.y));
-              t.x += a.x; t.y += a.y; t.z += b.x; t.w += b.y;
-            }
-            const __nv_bfloat162 lo = __floats2bfloat162_rn(t.x, t.y);
-            const __nv_bfloat162 hi = __floats2bfloat162_rn(t.z, t.w);
-            uint2 packed;
-            packed.x = *reinterpret_cast<const uint32_t*>(&lo);
-            packed.y = *reinterpret_cast<const uint32_t*>(&hi);
-            *reinterpret_cast<uint2*>(o) = packed;
-          } else if (p.part != nullptr) {
+            store_bf16x4(p.out + (int64_t)(m0 + rr) * ldw + col0 + c4, t, p.accumulate);
+          } else {
             *reinterpret_cast<float4*>(p.part + ((int64_t)blockIdx.z * gridDim.x + blockIdx.x) * (kBlockM * 3 * kBlockN) +
                                        rr * (3 * kBlockN) + s * kBlockN + c4) = t;
-          } else {
-            red_add_v4(p.ws + off, t.x, t.y, t.z, t.w);
           }
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");   // staging tile is reused by the next tap
-      }
-      if (!direct && p.part == nullptr) {
-        // ---- fused finalize by the last-arriving CTA of this (tile, filter row) ----
-        __threadfence();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (et == 0) {
-          const int old = atomicAdd(&p.counters[blockIdx.x], 1);
-          const int last = old == (int)gridDim.z - 1;
-          if (last) p.counters[blockIdx.x] = 0;
-          *s_last = (uint32_t)last;
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (*s_last != 0u) {
-          __threadfence();
-          const int total = rows_valid * (3 * kVecPerRow);      // the three taps of a row are adjacent in KRSC
-          // when n0 spans the whole Cin they are contiguous; in general tap s starts at (r*3+s)*Cin + n0
-          for (int f = et; f < total; f += kEpiThreads) {
-            const int rr = f / (3 * kVecPerRow);
-            const int rem = f % (3 * kVecPerRow);
-            const int s = rem / kVecPerRow, c4 = (rem % kVecPerRow) * 4;
-            const int64_t off = (int64_t)(m0 + rr) * ldw + (int64_t)(r * 3 + s) * p.Cin + n0 + c4;
-            float4 t = __ldcg(reinterpret_cast<const float4*>(p.ws + off));
-            *reinterpret_cast<float4*>(p.ws + off) = make_float4(0.f, 0.f, 0.f, 0.f);
-            __nv_bfloat16* o = p.out + off;
-            if (p.accumulate) {
-              const uint2 old = *reinterpret_cast<const uint2*>(o);
-              const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.x));
-              const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.y));
-              t.x += a.x; t.y += a.y; t.z += b.x; t.w += b.y;
-            }
-            const __nv_bfloat162 lo = __floats2bfloat162_rn(t.x, t.y);
-            const __nv_bfloat162 hi = __floats2bfloat162_rn(t.z, t.w);
-            uint2 packed;
-            packed.x = *reinterpret_cast<const uint32_t*>(&lo);
-            packed.y = *reinterpret_cast<const uint32_t*>(&hi);
-            *reinterpret_cast<uint2*>(o) = packed;
-          }
-        }
       }
     }
   }
@@ -262,11 +206,9 @@ struct Wgrad2Params {
   int total_kb, kb_per_split;
   int tiles_n;
   int base_offset_mode;      // 0: descriptor base offset 0 (address-based swizzle); 1: (addr >> 7) & 7
-  float* ws;
   __nv_bfloat16* out;
-  int* counters;
   int accumulate;
-  float* part;               // split-K partial tiles [split][ctas][128 x 3*BLOCK_N] (no atomics) or nullptr
+  float* part;               // split-K partial tiles [split][ctas][128 x 3*BLOCK_N] (gridDim.z > 1)
 };
 
 template <int BLOCK_N>
@@ -279,7 +221,6 @@ conv3x3_wgrad2_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_con
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBar);
   uint64_t* empty_bar = full_bar + kStages2;
-  uint32_t* s_last = reinterpret_cast<uint32_t*>(empty_bar + kStages2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -377,68 +318,18 @@ conv3x3_wgrad2_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_con
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");
         const int64_t col0 = (int64_t)(r * 3 + s) * p.Cin + n0;
+#pragma unroll 1   // unrolled, this loop costs registers: the 128-column kernel spills more
         for (int f = et; f < rows_valid * kVec; f += kEpiThreads) {
           const int rr = f / kVec, c4 = (f % kVec) * 4;
-          float4 t = *reinterpret_cast<const float4*>(sf + rr * L::kPitch + c4 * 4);
-          const int64_t off = (int64_t)(m0 + rr) * ldw + col0 + c4;
+          const float4 t = *reinterpret_cast<const float4*>(sf + rr * L::kPitch + c4 * 4);
           if (direct) {
-            __nv_bfloat16* o = p.out + off;
-            if (p.accumulate) {
-              const uint2 old = *reinterpret_cast<const uint2*>(o);
-              const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.x));
-              const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.y));
-              t.x += a.x; t.y += a.y; t.z += b.x; t.w += b.y;
-            }
-            const __nv_bfloat162 lo = __floats2bfloat162_rn(t.x, t.y);
-            const __nv_bfloat162 hi = __floats2bfloat162_rn(t.z, t.w);
-            uint2 packed;
-            packed.x = *reinterpret_cast<const uint32_t*>(&lo);
-            packed.y = *reinterpret_cast<const uint32_t*>(&hi);
-            *reinterpret_cast<uint2*>(o) = packed;
-          } else if (p.part != nullptr) {
+            store_bf16x4(p.out + (int64_t)(m0 + rr) * ldw + col0 + c4, t, p.accumulate);
+          } else {
             *reinterpret_cast<float4*>(p.part + ((int64_t)blockIdx.z * gridDim.x + blockIdx.x) * (kBlockM * 3 * BLOCK_N) +
                                        rr * (3 * BLOCK_N) + s * BLOCK_N + c4) = t;
-          } else {
-            red_add_v4(p.ws + off, t.x, t.y, t.z, t.w);
           }
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");
-      }
-      if (!direct && p.part == nullptr) {
-        __threadfence();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (et == 0) {
-          const int old = atomicAdd(&p.counters[blockIdx.x], 1);
-          const int last = old == (int)gridDim.z - 1;
-          if (last) p.counters[blockIdx.x] = 0;
-          *s_last = (uint32_t)last;
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (*s_last != 0u) {
-          __threadfence();
-          const int total = rows_valid * (3 * kVec);
-          for (int f = et; f < total; f += kEpiThreads) {
-            const int rr = f / (3 * kVec);
-            const int rem = f % (3 * kVec);
-            const int s = rem / kVec, c4 = (rem % kVec) * 4;
-            const int64_t off = (int64_t)(m0 + rr) * ldw + (int64_t)(r * 3 + s) * p.Cin + n0 + c4;
-            float4 t = __ldcg(reinterpret_cast<const float4*>(p.ws + off));
-            *reinterpret_cast<float4*>(p.ws + off) = make_float4(0.f, 0.f, 0.f, 0.f);
-            __nv_bfloat16* o = p.out + off;
-            if (p.accumulate) {
-              const uint2 old = *reinterpret_cast<const uint2*>(o);
-              const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.x));
-              const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.y));
-              t.x += a.x; t.y += a.y; t.z += b.x; t.w += b.y;
-            }
-            const __nv_bfloat162 lo = __floats2bfloat162_rn(t.x, t.y);
-            const __nv_bfloat162 hi = __floats2bfloat162_rn(t.z, t.w);
-            uint2 packed;
-            packed.x = *reinterpret_cast<const uint32_t*>(&lo);
-            packed.y = *reinterpret_cast<const uint32_t*>(&hi);
-            *reinterpret_cast<uint2*>(o) = packed;
-          }
-        }
       }
     }
   }
@@ -482,6 +373,13 @@ int g_wgrad3_bo = [] {
   return (e != nullptr && e[0] == '1') ? 1 : 0;
 }();
 
+// a split reduction needs a partial tile per (split, CTA); one that does not fit is an error, never a different path
+const char* check_partials(const Conv3x3WgradArgs& a, int split, int64_t elems_per_split) {
+  if (split > 1 && (a.partials == nullptr || a.partials_elems < split * elems_per_split))
+    return "conv3x3_wgrad: split_k > 1 needs a partial-tile buffer of split * conv3x3_wgrad_tiles * 128 * 192 floats";
+  return nullptr;
+}
+
 template <int BLOCK_N>
 const char* launch_wgrad2(const Conv3x3WgradArgs& a, const Wgrad2Geometry& geo, cudaStream_t stream) {
   using L = W2Smem<BLOCK_N>;
@@ -518,18 +416,15 @@ const char* launch_wgrad2(const Conv3x3WgradArgs& a, const Wgrad2Geometry& geo, 
   p.tiles_n = a.Cin / BLOCK_N;
   p.base_offset_mode = g_wgrad3_bo;
   const int tiles_m = (a.Cout + kBlockM - 1) / kBlockM;
-  p.ws = a.ws;
   p.out = reinterpret_cast<__nv_bfloat16*>(a.dW);
-  p.counters = a.counters;
   p.accumulate = a.accumulate ? 1 : 0;
   dim3 grid(tiles_m * p.tiles_n * 3, 1, split);
-  const bool use_part = split > 1 && a.partials != nullptr &&
-                        a.partials_elems >= (int64_t)split * grid.x * kBlockM * 3 * BLOCK_N;
-  p.part = use_part ? a.partials : nullptr;
+  if (const char* e = check_partials(a, split, (int64_t)grid.x * kBlockM * 3 * BLOCK_N)) return e;
+  p.part = a.partials;
   kern<<<grid, kThreads, L::kTotal, stream>>>(tmDy, tmX, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cudaGetErrorString(e);
-  if (use_part) {
+  if (split > 1) {
     splitk_reduce(a.partials, split, (int)grid.x, p.tiles_n, kBlockM, 3 * BLOCK_N, 3, a.Cin, a.Cout, 9 * a.Cin, a.dW,
                   (int64_t)9 * a.Cin, a.accumulate, stream);
     e = cudaGetLastError();
@@ -588,7 +483,7 @@ const char* conv3x3_wgrad_bf16(const Conv3x3WgradArgs& a, cudaStream_t stream) {
   if (s2 ? !conv3x3_wgrad_s2_supported(a.N, a.H, a.W, a.Cin, a.Cout)
          : !conv3x3_wgrad_supported(a.N, a.H, a.W, a.Cin, a.Cout))
     return "conv3x3_wgrad: unsupported shape";
-  if (a.ws == nullptr || a.counters == nullptr || a.dW == nullptr) return "conv3x3_wgrad: missing buffers";
+  if (a.dW == nullptr) return "conv3x3_wgrad: missing output";
   if (a.device >= 0) {
     cudaError_t e = cudaSetDevice(a.device);   // tensor-map encoding needs a bound context (see gemm.cu)
     if (e != cudaSuccess) return cudaGetErrorString(e);
@@ -638,19 +533,16 @@ const char* conv3x3_wgrad_bf16(const Conv3x3WgradArgs& a, cudaStream_t stream) {
   split = (p.total_kb + p.kb_per_split - 1) / p.kb_per_split;
   p.tiles_n = a.Cin / kBlockN;
   const int tiles_m = (a.Cout + kBlockM - 1) / kBlockM;
-  p.ws = a.ws;
   p.out = reinterpret_cast<__nv_bfloat16*>(a.dW);
-  p.counters = a.counters;
   p.accumulate = a.accumulate ? 1 : 0;
   p.stride = s2 ? 2 : 1;
   dim3 grid(tiles_m * p.tiles_n * 3, 1, split);
-  const bool use_part = split > 1 && a.partials != nullptr &&
-                        a.partials_elems >= (int64_t)split * grid.x * kBlockM * 3 * kBlockN;
-  p.part = use_part ? a.partials : nullptr;
+  if (const char* e = check_partials(a, split, (int64_t)grid.x * kBlockM * 3 * kBlockN)) return e;
+  p.part = a.partials;
   conv3x3_wgrad_kernel<<<grid, kThreads, kSmemTotal, stream>>>(tmDy, tmX, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cudaGetErrorString(e);
-  if (use_part) {
+  if (split > 1) {
     splitk_reduce(a.partials, split, (int)grid.x, p.tiles_n, kBlockM, 3 * kBlockN, 3, a.Cin, a.Cout, 9 * a.Cin, a.dW,
                   (int64_t)9 * a.Cin, a.accumulate, stream);
     e = cudaGetLastError();
@@ -658,7 +550,7 @@ const char* conv3x3_wgrad_bf16(const Conv3x3WgradArgs& a, cudaStream_t stream) {
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
-// upper bound over both kernel versions (sizes the tile-counter array)
+// upper bound over both kernel versions, in CTAs of 64 Cin columns (sizes the partial-tile buffer)
 int conv3x3_wgrad_tiles(int Cin, int Cout) { return ((Cout + kBlockM - 1) / kBlockM) * (Cin / kBlockN) * 3; }
 // (tile, filter row) CTAs per split of the active version: what the split-K heuristic divides the SMs by
 int conv3x3_wgrad_ctas(int Cin, int Cout) {

@@ -14,7 +14,8 @@
 //                 bf16 -> swizzled smem -> TMA store; per-channel sum / sum^2 of the stored values
 //                 (train-mode BatchNorm statistics) reduced from the staged tile and pushed with
 //                 fp32 atomics, so BN needs no extra pass over the conv output.
-//                 Split-K variant: fp32 vector reductions (red.global.add.v4.f32) instead.
+//                 Weight-gradient variant (EPI 1): coalesced bf16 stores, or fp32 partial tiles per K split
+//                 that splitk_reduce_kernel sums.
 #include <cuda.h>
 #include <cstdio>
 #include <mutex>
@@ -39,14 +40,10 @@ struct GemmParams {
   const float* col_shift;
   int relu;
   float* col_stats;  // [2N]
-  float* out_f32;    // split-K accumulation target, row-major [M, N]
-  // fused split-K finalize: the last CTA of each output tile converts the fp32 tile to bf16 into
-  // out_bf16 (+= when accumulate) and re-zeroes the fp32 workspace + its tile counter
-  __nv_bfloat16* out_bf16;
+  __nv_bfloat16* out_bf16;   // EPI 1: bf16 [M, N], row pitch ldo (+= when accumulate)
   long long ldo;
-  int* tile_counters;
   int accumulate;
-  float* part;       // split-K partial tiles [split][tiles][BLOCK_M x BLOCK_N] (no atomics) or nullptr
+  float* part;       // EPI 1 with a K split: partial tiles [split][tiles][BLOCK_M x BLOCK_N]
   // GEMM -> peer ship (see gemm.h)
   uint32_t* ship_flag;
   const uint32_t* ship_seq_ptr;
@@ -76,7 +73,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint32_t* s_last = reinterpret_cast<uint32_t*>(empty_bar + STAGES);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -244,10 +240,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           }
         }
       } else {
-        // split-K: stage the fp32 partial tile in smem (the pipeline stages are drained), then push
-        // it to the fp32 workspace with COALESCED vector reductions: consecutive threads cover
-        // consecutive 16-byte pieces of a row (row-per-thread reds touch 32 cache lines per warp
-        // instruction).
+        // weight gradient: stage the fp32 tile in smem (the pipeline stages are drained), then store it COALESCED:
+        // consecutive threads cover consecutive 16-byte pieces of a row.  Without a K split this CTA owns the tile and
+        // writes bf16 (+= when accumulating); with one it stores its partial tile for splitk_reduce_kernel.
         constexpr int kPitch = BLOCK_N * 4 + 32;        // bytes; +32 spreads the eight rows of a warp's store over the banks
         constexpr int kVecPerRow = BLOCK_N / 4;         // float4 per row
         uint8_t* sf = smem;
@@ -257,106 +252,22 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           *reinterpret_cast<float2*>(sf + (row + 8) * kPitch + (j * 8 + cq) * 4) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");
-        int rows_valid = p.M - m0;
-        if (rows_valid > BLOCK_M) rows_valid = BLOCK_M;
-        int cols_valid = p.N - n0;
-        if (cols_valid > BLOCK_N) cols_valid = BLOCK_N;
-        const bool vec_ok = (p.N % 4) == 0;
-        if (gridDim.z == 1 && p.out_bf16 != nullptr) {
-          // no split: this CTA owns the tile -> write bf16 (+= sink) straight from the staged tile,
-          // coalesced, without touching the fp32 workspace, atomics or tile counters
+        if (gridDim.z == 1) {
+          int rows_valid = p.M - m0;
+          if (rows_valid > BLOCK_M) rows_valid = BLOCK_M;
+          int cols_valid = p.N - n0;
+          if (cols_valid > BLOCK_N) cols_valid = BLOCK_N;
           for (int f = et; f < rows_valid * kVecPerRow; f += kEpiThreads) {
             const int rr = f / kVecPerRow, c4 = (f % kVecPerRow) * 4;
             if (c4 + 3 >= cols_valid) continue;
-            float4 t = *reinterpret_cast<const float4*>(sf + rr * kPitch + c4 * 4);
-            __nv_bfloat16* o = p.out_bf16 + (int64_t)(m0 + rr) * p.ldo + n0 + c4;
-            if (p.accumulate) {
-              const uint2 old = *reinterpret_cast<const uint2*>(o);
-              const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.x));
-              const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.y));
-              t.x += a.x; t.y += a.y; t.z += b.x; t.w += b.y;
-            }
-            const __nv_bfloat162 lo = __floats2bfloat162_rn(t.x, t.y);
-            const __nv_bfloat162 hi = __floats2bfloat162_rn(t.z, t.w);
-            uint2 packed;
-            packed.x = *reinterpret_cast<const uint32_t*>(&lo);
-            packed.y = *reinterpret_cast<const uint32_t*>(&hi);
-            *reinterpret_cast<uint2*>(o) = packed;
+            store_bf16x4(p.out_bf16 + (int64_t)(m0 + rr) * p.ldo + n0 + c4,
+                         *reinterpret_cast<const float4*>(sf + rr * kPitch + c4 * 4), p.accumulate);
           }
-        } else if (p.part != nullptr) {
-          // split-K partial tile: plain coalesced 16-byte stores, summed by splitk_reduce_kernel afterwards
+        } else {
           float* dst = p.part + ((int64_t)blockIdx.z * gridDim.x + tile) * (BLOCK_M * BLOCK_N);
           for (int f = et; f < BLOCK_M * kVecPerRow; f += kEpiThreads) {
             const int rr = f / kVecPerRow, c4 = (f % kVecPerRow) * 4;
             *reinterpret_cast<float4*>(dst + rr * BLOCK_N + c4) = *reinterpret_cast<const float4*>(sf + rr * kPitch + c4 * 4);
-          }
-        } else {
-        for (int f = et; f < rows_valid * kVecPerRow; f += kEpiThreads) {
-          const int rr = f / kVecPerRow, c4 = (f % kVecPerRow) * 4;
-          if (c4 >= cols_valid) continue;
-          const float4 v = *reinterpret_cast<const float4*>(sf + rr * kPitch + c4 * 4);
-          float* dst = p.out_f32 + (int64_t)(m0 + rr) * p.N + n0 + c4;
-          if (vec_ok && c4 + 3 < cols_valid) {
-            asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(dst), "f"(v.x), "f"(v.y),
-                         "f"(v.z), "f"(v.w)
-                         : "memory");
-          } else {
-            const float vv[4] = {v.x, v.y, v.z, v.w};
-            for (int j = 0; j < 4; ++j)
-              if (c4 + j < cols_valid) atomicAdd(dst + j, vv[j]);
-          }
-        }
-        }
-        if (p.tile_counters != nullptr && gridDim.z > 1 && p.part == nullptr) {
-          // ---- fused finalize by the last-arriving CTA of this output tile (coalesced) ----
-          __threadfence();
-          asm volatile("bar.sync 1, 256;" ::: "memory");
-          if (et == 0) {
-            const int old = atomicAdd(&p.tile_counters[tile], 1);
-            const int last = old == (int)gridDim.z - 1;
-            if (last) p.tile_counters[tile] = 0;
-            *s_last = (uint32_t)last;
-          }
-          asm volatile("bar.sync 1, 256;" ::: "memory");
-          if (*s_last != 0u) {
-            __threadfence();
-            const int total = rows_valid * kVecPerRow;
-            constexpr int U = 4;
-            for (int f0 = et; f0 < total; f0 += kEpiThreads * U) {
-              float4 v[U];
-              bool ok[U];
-#pragma unroll
-              for (int u = 0; u < U; ++u) {
-                const int f = f0 + u * kEpiThreads;
-                const int rr = f / kVecPerRow, c4 = (f % kVecPerRow) * 4;
-                ok[u] = f < total && c4 + 3 < cols_valid;
-                if (ok[u])
-                  v[u] = __ldcg(reinterpret_cast<const float4*>(
-                      p.out_f32 + (int64_t)(m0 + rr) * p.N + n0 + c4));
-              }
-#pragma unroll
-              for (int u = 0; u < U; ++u) {
-                if (!ok[u]) continue;
-                const int f = f0 + u * kEpiThreads;
-                const int rr = f / kVecPerRow, c4 = (f % kVecPerRow) * 4;
-                float* w = p.out_f32 + (int64_t)(m0 + rr) * p.N + n0 + c4;
-                __nv_bfloat16* o = p.out_bf16 + (int64_t)(m0 + rr) * p.ldo + n0 + c4;
-                *reinterpret_cast<float4*>(w) = make_float4(0.f, 0.f, 0.f, 0.f);
-                float4 t = v[u];
-                if (p.accumulate) {
-                  const uint2 old = *reinterpret_cast<const uint2*>(o);
-                  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.x));
-                  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.y));
-                  t.x += a.x; t.y += a.y; t.z += b.x; t.w += b.y;
-                }
-                const __nv_bfloat162 lo = __floats2bfloat162_rn(t.x, t.y);
-                const __nv_bfloat162 hi = __floats2bfloat162_rn(t.z, t.w);
-                uint2 packed;
-                packed.x = *reinterpret_cast<const uint32_t*>(&lo);
-                packed.y = *reinterpret_cast<const uint32_t*>(&hi);
-                *reinterpret_cast<uint2*>(o) = packed;
-              }
-            }
           }
         }
       }
@@ -483,12 +394,10 @@ const char* launch_variant(const GemmArgs& g, cudaStream_t stream) {
   p.col_shift = g.col_shift;
   p.relu = g.relu ? 1 : 0;
   p.col_stats = g.col_stats;
-  p.out_f32 = g.out_f32;
-  p.out_bf16 = reinterpret_cast<__nv_bfloat16*>(g.out_bf16);
-  p.ldo = g.ldo;
-  p.tile_counters = g.tile_counters;
-  p.accumulate = g.accumulate_out ? 1 : 0;
-  p.part = nullptr;
+  p.out_bf16 = reinterpret_cast<__nv_bfloat16*>(g.D);
+  p.ldo = g.ldd;
+  p.accumulate = g.accumulate ? 1 : 0;
+  p.part = split > 1 ? g.partials : nullptr;
   p.ship_flag = EPI == 0 ? reinterpret_cast<uint32_t*>(g.ship_flag) : nullptr;
   p.ship_seq_ptr = reinterpret_cast<const uint32_t*>(g.ship_seq_ptr);
   p.ship_seq_imm = g.ship_seq_imm;
@@ -496,15 +405,14 @@ const char* launch_variant(const GemmArgs& g, cudaStream_t stream) {
   const int tiles_m = (g.M + BLOCK_M - 1) / BLOCK_M;
   const int tiles_n = (g.N + BLOCK_N - 1) / BLOCK_N;
   dim3 grid(tiles_m * tiles_n, 1, split);
-  const bool use_part = EPI == 1 && split > 1 && g.partials != nullptr && g.out_bf16 != nullptr && (g.N % 4) == 0 &&
-                        g.partials_elems >= (int64_t)split * grid.x * BLOCK_M * BLOCK_N;
-  if (use_part) p.part = g.partials;
+  if (split > 1 && (g.partials == nullptr || g.partials_elems < (int64_t)split * grid.x * BLOCK_M * BLOCK_N))
+    return "gemm_bf16: split_k > 1 needs a partial-tile buffer of split * tiles * 128 * BLOCK_N floats";
   kern<<<grid, kGemmThreads, L::kTotal, stream>>>(tmA, tmB, tmD, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cudaGetErrorString(e);
-  if (use_part) {
-    splitk_reduce(g.partials, split, (int)grid.x, tiles_n, BLOCK_M, BLOCK_N, 1, 0, g.M, g.N, g.out_bf16, g.ldo,
-                  g.accumulate_out, stream);
+  if (split > 1) {
+    splitk_reduce(g.partials, split, (int)grid.x, tiles_n, BLOCK_M, BLOCK_N, 1, 0, g.M, g.N, g.D, g.ldd, g.accumulate,
+                  stream);
     e = cudaGetLastError();
   }
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
@@ -572,19 +480,7 @@ splitk_reduce_kernel(const float* __restrict__ part, int split, int ctas, int ti
         const float4 o = sm[k][vl];
         acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w;
       }
-      __nv_bfloat16* o = out + (int64_t)m * ldo + n;
-      if (accumulate) {
-        const uint2 old = *reinterpret_cast<const uint2*>(o);
-        const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.x));
-        const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old.y));
-        acc.x += a.x; acc.y += a.y; acc.z += b.x; acc.w += b.y;
-      }
-      const __nv_bfloat162 lo = __floats2bfloat162_rn(acc.x, acc.y);
-      const __nv_bfloat162 hi = __floats2bfloat162_rn(acc.z, acc.w);
-      uint2 packed;
-      packed.x = *reinterpret_cast<const uint32_t*>(&lo);
-      packed.y = *reinterpret_cast<const uint32_t*>(&hi);
-      *reinterpret_cast<uint2*>(o) = packed;
+      store_bf16x4(out + (int64_t)m * ldo + n, acc, accumulate);
     }
     __syncthreads();
   }
@@ -619,19 +515,10 @@ const char* gemm_bf16(const GemmArgs& g, cudaStream_t stream) {
     if (e != cudaSuccess) return cudaGetErrorString(e);
   }
   const bool n64 = g.N <= 64;
-  if (g.out_f32 == nullptr && !g.a_mn_major && g.ship_flag == nullptr && persistent_gemm_enabled())
-    return gemm_bf16_persistent(g, stream);
+  if (!g.a_mn_major && g.ship_flag == nullptr && persistent_gemm_enabled()) return gemm_bf16_persistent(g, stream);
   if (g.add_src != nullptr) return "gemm add_src is implemented by the persistent kernel only";
-  if (g.out_f32 != nullptr) {
-    // split-K fp32 accumulation (wgrad): both operands MN-major or both K-major
-    if (g.a_mn_major && g.b_mn_major)
-      return n64 ? launch_variant<64, 4, true, true, 1>(g, stream)
-                 : launch_variant<128, 3, true, true, 1>(g, stream);
-    if (!g.a_mn_major && !g.b_mn_major)
-      return n64 ? launch_variant<64, 4, false, false, 1>(g, stream)
-                 : launch_variant<128, 3, false, false, 1>(g, stream);
-    return "unsupported split-K operand layout";
-  }
+  if (g.a_mn_major && g.b_mn_major)   // weight gradient
+    return n64 ? launch_variant<64, 4, true, true, 1>(g, stream) : launch_variant<128, 3, true, true, 1>(g, stream);
   if (!g.a_mn_major && !g.b_mn_major)
     return n64 ? launch_variant<64, 4, false, false, 0>(g, stream)
                : launch_variant<128, 3, false, false, 0>(g, stream);

@@ -24,7 +24,7 @@ struct BnBwdFuse {
 struct GemmArgs {
   const void* A = nullptr;  // bf16
   const void* B = nullptr;  // bf16
-  void* D = nullptr;        // bf16 [M, N] (ignored when out_f32 != nullptr)
+  void* D = nullptr;        // bf16 [M, N]
   int M = 0, N = 0, K = 0;
   int64_t lda = 0, ldb = 0, ldd = 0;  // row pitches in elements of the *stored* 2-D arrays
   bool a_mn_major = false;            // A stored as [K, M] (M contiguous)
@@ -33,18 +33,12 @@ struct GemmArgs {
   const float* col_shift = nullptr;   // per-output-column shift / bias or nullptr
   bool relu = false;
   float* col_stats = nullptr;         // [2N] fp32: += sum, sum of squares of the stored outputs
-  float* out_f32 = nullptr;           // split-K target: fp32 [M, N], += A*B
+  // Weight-gradient form (A and B both MN-major, N % 4 == 0): D (+= when accumulate) is written with plain 8-byte
+  // stores.  With split_k > 1 the K reduction is split over CTAs: every CTA stores its fp32 partial tile into
+  // partials[split][tile][128 x BLOCK_N] with plain coalesced stores and splitk_reduce sums the splits into D.  The
+  // partials are required then (partials_elems >= split * tiles * 128 * BLOCK_N).
   int split_k = 1;
-  // fused split-K finalize (optional, with out_f32 as an all-zero workspace on entry):
-  // the last CTA per tile writes bf16(out_f32 tile) (+= if accumulate_out) to out_bf16 [M, N] with
-  // row pitch ldo, then re-zeroes the workspace tile and its counter.
-  void* out_bf16 = nullptr;
-  int64_t ldo = 0;
-  int* tile_counters = nullptr;       // >= ceil(M/128)*ceil(N/BLOCK_N) zero-initialised ints
-  bool accumulate_out = false;
-  // split-K WITHOUT atomics (preferred when given and large enough): every CTA stores its fp32 partial tile into
-  // partials[split][tile][128 x BLOCK_N] with plain coalesced stores and a second small kernel sums the splits into
-  // out_bf16.  fp32 reductions into L2 queue behind each other on the few hot lines; plain stores do not.
+  bool accumulate = false;
   float* partials = nullptr;
   int64_t partials_elems = 0;
   int device = -1;                    // CUDA device ordinal of the operands (binds the context)
@@ -100,19 +94,19 @@ bool conv3x3_dgrad_s2_supported(int N, int Ho, int Wo, int Cin, int Cout);
 const char* conv3x3_dgrad_s2_bf16(const Conv3x3Args& args, cudaStream_t stream);
 
 // Weight gradient of the same convolution (conv3x3_wgrad.cu): dW[Cout,3,3,Cin] (+)= sum_pixels dY x shifted X, pixel
-// reduction split over `split_k` CTAs with the fused fp32 -> bf16 finalize of the 1x1 wgrad GEMM.
+// reduction split over `split_k` CTAs through partial tiles like the 1x1 weight-gradient GEMM.
 struct Conv3x3WgradArgs {
   const void* X = nullptr;    // bf16 NHWC [N, H, W, Cin]   (the convolution's input)
   const void* dY = nullptr;   // bf16 NHWC [N, H, W, Cout]
   void* dW = nullptr;         // bf16 KRSC [Cout, 3, 3, Cin] (e.g. a window of the flat gradient bucket)
-  float* ws = nullptr;        // fp32 [Cout * 9 * Cin] all-zero workspace (left all-zero)
-  int* counters = nullptr;    // >= conv3x3_wgrad_tiles(Cin, Cout) zero ints (left zero)
   int N = 0, H = 0, W = 0, Cin = 0, Cout = 0;   // H, W: OUTPUT (= dY) size; the input is stride times as large
   int split_k = 1;
   bool accumulate = false;    // dW += result instead of dW = result
   int device = -1;
   int stride = 1;             // 2: X is [N, 2H, 2W, Cin], read through the TMA traversal stride (version-1 kernel)
-  float* partials = nullptr;  // split-K without atomics (see GemmArgs::partials): [split][ctas][128 x 3*BLOCK_N]
+  // fp32 partial tiles [split][ctas][128 x 3*BLOCK_N], required when split_k > 1: split_k *
+  // conv3x3_wgrad_tiles(Cin, Cout) * 128 * 192 elements cover both kernel versions
+  float* partials = nullptr;
   int64_t partials_elems = 0;
 };
 bool conv3x3_wgrad_supported(int N, int H, int W, int Cin, int Cout);

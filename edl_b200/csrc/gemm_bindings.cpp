@@ -46,17 +46,8 @@ edl::BnBwdFuse parse_bn(const c10::optional<std::vector<c10::optional<Tensor>>>&
   return f;
 }
 
-// D[M,N] = A * B with the operand layouts described in gemm.h.  A, B, D are 2-D bf16 tensors whose
-// last dimension is contiguous (row pitch = stride(0)).
-void gemm_bf16(const Tensor& A, const Tensor& B, const c10::optional<Tensor>& D, bool a_mn_major,
-               bool b_mn_major, const c10::optional<Tensor>& col_scale,
-               const c10::optional<Tensor>& col_shift, bool relu,
-               const c10::optional<Tensor>& col_stats, const c10::optional<Tensor>& out_f32,
-               int64_t split_k, const c10::optional<Tensor>& out_bf16,
-               const c10::optional<Tensor>& tile_counters, bool accumulate_out,
-               const c10::optional<Tensor>& add_src,
-               const c10::optional<std::vector<c10::optional<Tensor>>>& bn, bool bn_relu,
-               const c10::optional<Tensor>& partials) {
+// The operands of a GEMM: A, B are 2-D bf16 CUDA tensors whose last dimension is contiguous (row pitch = stride(0)).
+edl::GemmArgs gemm_operands(const Tensor& A, const Tensor& B, bool a_mn_major, bool b_mn_major) {
   TORCH_CHECK(A.is_cuda() && B.is_cuda() && A.dim() == 2 && B.dim() == 2);
   TORCH_CHECK(A.scalar_type() == at::kBFloat16 && B.scalar_type() == at::kBFloat16);
   TORCH_CHECK(A.stride(1) == 1 && B.stride(1) == 1, "operands need a contiguous last dim");
@@ -74,29 +65,22 @@ void gemm_bf16(const Tensor& A, const Tensor& B, const c10::optional<Tensor>& D,
   g.ldb = B.stride(0);
   TORCH_CHECK(g.lda % 8 == 0 && g.ldb % 8 == 0, "row pitch must be a multiple of 16 bytes");
   TORCH_CHECK(reinterpret_cast<uintptr_t>(g.A) % 16 == 0 && reinterpret_cast<uintptr_t>(g.B) % 16 == 0);
-  if (out_f32.has_value() && out_f32->defined()) {
-    TORCH_CHECK(out_f32->scalar_type() == at::kFloat && out_f32->is_contiguous());
-    TORCH_CHECK(out_f32->numel() >= (int64_t)g.M * g.N);
-    g.out_f32 = out_f32->data_ptr<float>();
-    g.split_k = (int)split_k;
-    if (out_bf16.has_value() && out_bf16->defined()) {
-      TORCH_CHECK(out_bf16->scalar_type() == at::kBFloat16 && out_bf16->dim() == 2);
-      TORCH_CHECK(out_bf16->size(0) == g.M && out_bf16->size(1) == g.N && out_bf16->stride(1) == 1);
-      TORCH_CHECK(g.N % 4 == 0 && out_bf16->stride(0) % 4 == 0, "fused finalize needs N % 4 == 0");
-      TORCH_CHECK(tile_counters.has_value() && tile_counters->scalar_type() == at::kInt);
-      TORCH_CHECK(tile_counters->numel() >= (int64_t)((g.M + 127) / 128) * ((g.N + 63) / 64));
-      g.out_bf16 = out_bf16->data_ptr();
-      g.ldo = out_bf16->stride(0);
-      g.tile_counters = tile_counters->data_ptr<int>();
-      g.accumulate_out = accumulate_out;
-    }
-  } else {
-    TORCH_CHECK(D.has_value() && D->defined() && D->scalar_type() == at::kBFloat16);
-    TORCH_CHECK(D->dim() == 2 && D->size(0) == g.M && D->size(1) == g.N && D->stride(1) == 1);
-    g.D = D->data_ptr();
-    g.ldd = D->stride(0);
-    TORCH_CHECK(g.ldd % 8 == 0 && reinterpret_cast<uintptr_t>(g.D) % 16 == 0);
-  }
+  g.device = A.device().index();
+  return g;
+}
+
+// D[M,N] = A * B with the operand layouts described in gemm.h (fprop: both K-major; dgrad: B MN-major).
+void gemm_bf16(const Tensor& A, const Tensor& B, const Tensor& D, bool a_mn_major, bool b_mn_major,
+               const c10::optional<Tensor>& col_scale, const c10::optional<Tensor>& col_shift, bool relu,
+               const c10::optional<Tensor>& col_stats, const c10::optional<Tensor>& add_src,
+               const c10::optional<std::vector<c10::optional<Tensor>>>& bn, bool bn_relu) {
+  TORCH_CHECK(!(a_mn_major && b_mn_major), "both operands MN-major is the weight gradient: use gemm_wgrad_bf16");
+  edl::GemmArgs g = gemm_operands(A, B, a_mn_major, b_mn_major);
+  TORCH_CHECK(D.scalar_type() == at::kBFloat16);
+  TORCH_CHECK(D.dim() == 2 && D.size(0) == g.M && D.size(1) == g.N && D.stride(1) == 1);
+  g.D = D.data_ptr();
+  g.ldd = D.stride(0);
+  TORCH_CHECK(g.ldd % 8 == 0 && reinterpret_cast<uintptr_t>(g.D) % 16 == 0);
   g.col_scale = optp<float>(col_scale);
   g.col_shift = optp<float>(col_shift);
   g.relu = relu;
@@ -111,16 +95,37 @@ void gemm_bf16(const Tensor& A, const Tensor& B, const c10::optional<Tensor>& D,
     TORCH_CHECK(g.D != nullptr && g.ldd == g.N, "fused BN reduction needs a dense bf16 output");
     g.bn = parse_bn(bn, bn_relu, (int64_t)g.M * g.N, g.N);
   }
-  if (partials.has_value() && partials->defined()) {
-    TORCH_CHECK(partials->scalar_type() == at::kFloat && partials->is_contiguous() &&
-                reinterpret_cast<uintptr_t>(partials->data_ptr()) % 16 == 0);
-    g.partials = partials->data_ptr<float>();
-    g.partials_elems = partials->numel();
-  }
-  g.device = A.device().index();
   c10::cuda::CUDAGuard guard(A.device());
   const char* err = edl::gemm_bf16(g, at::cuda::getCurrentCUDAStream().stream());
   TORCH_CHECK(err == nullptr, "edl gemm_bf16 failed: ", err);
+}
+
+// fp32 scratch for the partial tiles of a split reduction (optional: the kernels report it missing or too small)
+void set_partials(const c10::optional<Tensor>& partials, float** ptr, int64_t* elems) {
+  if (!partials.has_value() || !partials->defined()) return;
+  TORCH_CHECK(partials->is_cuda() && partials->scalar_type() == at::kFloat && partials->is_contiguous() &&
+              reinterpret_cast<uintptr_t>(partials->data_ptr()) % 16 == 0, "partials: contiguous, aligned fp32");
+  *ptr = partials->data_ptr<float>();
+  *elems = partials->numel();
+}
+
+// Weight gradient of a 1x1 convolution / linear layer: out[N1, N2] (+)= dy[M, N1]^T @ x[M, N2] (bf16, accumulated in
+// fp32, one rounding).  split_k > 1 splits the M reduction over CTAs and needs `partials` (see gemm.h GemmArgs).
+void gemm_wgrad_bf16(const Tensor& dy, const Tensor& x, Tensor& out, int64_t split_k, bool accumulate,
+                     const c10::optional<Tensor>& partials) {
+  edl::GemmArgs g = gemm_operands(dy, x, true, true);
+  TORCH_CHECK(out.scalar_type() == at::kBFloat16 && out.dim() == 2 && out.size(0) == g.M && out.size(1) == g.N &&
+              out.stride(1) == 1, "out must be bf16 [N1, N2] with a contiguous last dim");
+  TORCH_CHECK(g.N % 4 == 0 && out.stride(0) % 4 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 8 == 0,
+              "the weight-gradient stores need N2 % 4 == 0 and 8-byte aligned rows");
+  g.D = out.data_ptr();
+  g.ldd = out.stride(0);
+  g.split_k = (int)split_k;
+  g.accumulate = accumulate;
+  set_partials(partials, &g.partials, &g.partials_elems);
+  c10::cuda::CUDAGuard guard(dy.device());
+  const char* err = edl::gemm_bf16(g, at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl gemm_wgrad_bf16 failed: ", err);
 }
 
 // Fused "linear -> peer ship": D = A[M,K] * B[N,K]^T (+ bias) TMA-stored straight into a peer GPU's
@@ -318,20 +323,18 @@ bool conv3x3_supported(int64_t n, int64_t h, int64_t w, int64_t cin, int64_t cou
 }
 
 // dW (+)= wgrad of the 3x3 / stride 1 / pad 1 conv.  x [N,Cin,H,W], dy [N,Cout,H,W] channels_last; dw KRSC
-// [Cout,3,3,Cin] bf16 contiguous; ws fp32 zeros (>= dw.numel()), counters int32 zeros.
-void conv3x3_wgrad(const Tensor& x, const Tensor& dy, Tensor& dw, Tensor& ws, Tensor& counters, int64_t split_k,
-                   bool accumulate, const c10::optional<Tensor>& partials) {
+// [Cout,3,3,Cin] bf16 contiguous; split_k > 1 needs `partials` (see gemm.h Conv3x3WgradArgs).
+void conv3x3_wgrad(const Tensor& x, const Tensor& dy, Tensor& dw, int64_t split_k, bool accumulate,
+                   const c10::optional<Tensor>& partials) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 4 && dy.dim() == 4 && dw.dim() == 4);
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && dy.scalar_type() == at::kBFloat16 && dw.scalar_type() == at::kBFloat16);
   TORCH_CHECK(x.is_contiguous(at::MemoryFormat::ChannelsLast) && dy.is_contiguous(at::MemoryFormat::ChannelsLast),
               "conv3x3_wgrad needs channels_last activations");
   TORCH_CHECK(dw.is_contiguous() && dw.size(1) == 3 && dw.size(2) == 3, "dw must be KRSC [Cout,3,3,Cin]");
-  TORCH_CHECK(ws.scalar_type() == at::kFloat && ws.is_contiguous() && ws.numel() >= dw.numel());
   edl::Conv3x3WgradArgs a;
   a.X = x.data_ptr();
   a.dY = dy.data_ptr();
   a.dW = dw.data_ptr();
-  a.ws = ws.data_ptr<float>();
   a.N = x.size(0);
   a.H = dy.size(2);
   a.W = dy.size(3);
@@ -341,18 +344,10 @@ void conv3x3_wgrad(const Tensor& x, const Tensor& dy, Tensor& dw, Tensor& ws, Te
   a.stride = (x.size(2) == 2 * a.H && x.size(3) == 2 * a.W && a.H != x.size(2)) ? 2 : 1;
   TORCH_CHECK(dy.size(0) == a.N && x.size(2) == a.stride * a.H && x.size(3) == a.stride * a.W &&
               dw.size(0) == a.Cout && dw.size(3) == a.Cin, "conv3x3_wgrad: x / dy / dw shapes do not belong together");
-  TORCH_CHECK(counters.scalar_type() == at::kInt && counters.is_contiguous() &&
-              counters.numel() >= edl::conv3x3_wgrad_tiles(a.Cin, a.Cout));
   TORCH_CHECK(reinterpret_cast<uintptr_t>(a.dW) % 8 == 0, "dw window must be 8-byte aligned");
-  a.counters = counters.data_ptr<int>();
   a.split_k = (int)split_k;
   a.accumulate = accumulate;
-  if (partials.has_value() && partials->defined()) {
-    TORCH_CHECK(partials->scalar_type() == at::kFloat && partials->is_contiguous() &&
-                reinterpret_cast<uintptr_t>(partials->data_ptr()) % 16 == 0);
-    a.partials = partials->data_ptr<float>();
-    a.partials_elems = partials->numel();
-  }
+  set_partials(partials, &a.partials, &a.partials_elems);
   a.device = x.device().index();
   c10::cuda::CUDAGuard guard(x.device());
   const char* err = edl::conv3x3_wgrad_bf16(a, at::cuda::getCurrentCUDAStream().stream());
@@ -436,6 +431,7 @@ void conv3x3_infer(const Tensor& x, const Tensor& w, Tensor& y, const c10::optio
 
 void register_gemm_bindings(pybind11::module_& m) {
   m.def("gemm_bf16", &gemm_bf16);
+  m.def("gemm_wgrad_bf16", &gemm_wgrad_bf16);
   m.def("conv3x3", &conv3x3);
   m.def("set_persistent_gemm", &edl::set_persistent_gemm);
   m.def("get_bnr_mode", &edl::get_bnr_mode);

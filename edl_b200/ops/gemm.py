@@ -15,16 +15,13 @@ _NUM_SMS = 132
 
 
 def gemm_bf16(a, b, out=None, a_mn_major=False, b_mn_major=False, col_scale=None, col_shift=None,
-              relu=False, col_stats=None, out_f32=None, split_k=1, out_bf16=None, tile_counters=None,
-              accumulate_out=False, add=None, bn=None, partials=None):
-    """D = op(A) @ op(B): see csrc/gemm.h for the operand conventions.
+              relu=False, col_stats=None, add=None, bn=None):
+    """D = op(A) @ op(B): see csrc/gemm.h for the operand conventions.  The weight-gradient form (both operands
+    MN-major) is ``_wgrad_impl``.
 
     default        : A [M, K], B [N, K]  -> D [M, N] = A @ B^T
     b_mn_major     : B [K, N]            -> D = A @ B
     a_mn_major     : A [K, M]            -> D = A^T @ op(B)
-    out_f32 given  : fp32 [M, N] += result, split over K across CTAs (no bf16 output).
-    out_bf16 given : (with out_f32 as an all-zero workspace) the last CTA of every output tile writes
-                     bf16(result) (+= if accumulate_out) into out_bf16 and re-zeroes the workspace.
     add given      : D = result + add (bf16 [M, N]) in the epilogue (gradient accumulation fused into dgrad).
     bn given       : a ``BNBackwardHook`` (ops/bn.py): D is the gradient of that BatchNorm's output and the
                      epilogue accumulates its backward reduction (sum dy, sum dy * xhat) into hook.dsums."""
@@ -44,12 +41,6 @@ def gemm_bf16(a, b, out=None, a_mn_major=False, b_mn_major=False, col_scale=None
         d = af @ bf
         if add is not None:
             d = d + add.float()
-        if out_bf16 is not None:
-            out_bf16.copy_((out_bf16.float() + d) if accumulate_out else d)
-            return out_bf16
-        if out_f32 is not None:
-            out_f32.add_(d)
-            return out_f32
         if col_scale is not None:
             d = d * col_scale.float()
         if col_shift is not None:
@@ -64,27 +55,21 @@ def gemm_bf16(a, b, out=None, a_mn_major=False, b_mn_major=False, col_scale=None
             out.copy_(d)
             return out
         return d
-    if out_f32 is None and out is None:
+    if out is None:
         out = torch.empty((m, n), device=a.device, dtype=torch.bfloat16)
     if add is not None and not (native().persistent_gemm_enabled() and n % 8 == 0 and add.stride(-1) == 1
-                                and add.stride(0) % 8 == 0 and add.data_ptr() % 16 == 0 and out_f32 is None):
+                                and add.stride(0) % 8 == 0 and add.data_ptr() % 16 == 0):
         # the fused addend lives in the persistent kernel's epilogue; otherwise one extra elementwise pass
-        native().gemm_bf16(a, b, out, a_mn_major, b_mn_major, col_scale, col_shift, relu, col_stats,
-                           out_f32, int(split_k), out_bf16, tile_counters, bool(accumulate_out), None, None, False,
-                           partials)
+        native().gemm_bf16(a, b, out, a_mn_major, b_mn_major, col_scale, col_shift, relu, col_stats, None, None, False)
         count_launch()
         out.add_(add)
         return out
     bn_list, bn_relu = (bn.as_list(m, n), bn.relu) if bn is not None else (None, False)
-    native().gemm_bf16(a, b, out, a_mn_major, b_mn_major, col_scale, col_shift, relu, col_stats,
-                       out_f32, int(split_k), out_bf16, tile_counters, bool(accumulate_out), add, bn_list, bn_relu,
-                       partials)
+    native().gemm_bf16(a, b, out, a_mn_major, b_mn_major, col_scale, col_shift, relu, col_stats, add, bn_list, bn_relu)
     count_launch()
     if bn is not None:
         bn.done = True
-    if out_bf16 is not None:
-        return out_bf16
-    return out if out_f32 is None else out_f32
+    return out
 
 
 def _tma_compatible(a, b, out, n):
@@ -97,8 +82,7 @@ def _tma_compatible(a, b, out, n):
 
 
 def _split_k_for(m, n, k):
-    """Split-K factor of the wgrad GEMM.  fp32 atomics queue in the L2,
-    so the split is chosen to fill ~one wave of SMs and never more: outputs
+    """Split-K factor of the wgrad GEMM.  The split is chosen to fill ~one wave of SMs and never more: outputs
     with >= 132 tiles are not split at all (direct bf16 store), tiny outputs (stage-2 layers, 1-8
     tiles with K ~ 100k) take the full 132-way split because they have few elements to update."""
     tiles = ((m + 127) // 128) * ((n + 127) // 128 if n > 64 else 1)
@@ -112,7 +96,6 @@ def _split_k_for(m, n, k):
     return max(1, min(want, max(1, kb // 2)))
 
 
-_WS = {}
 _SIDE = {"streams": [], "next": 0, "keep": []}
 
 
@@ -143,36 +126,34 @@ def release_wgrad_keepalive():
 
 
 
-def _splitk_workspace(device, numel, tiles):
-    """Persistent all-zero fp32 workspace + tile counters (per device and stream): the fused
-    split-K finalize leaves both zeroed again, so no per-call memset is needed."""
-    key = (device.index, torch.cuda.current_stream(device).cuda_stream)
-    ws = _WS.get(key)
-    if ws is None or ws[0].numel() < numel or ws[1].numel() < tiles:
-        ws = (torch.zeros(max(numel, 4 << 20), device=device, dtype=torch.float32),
-              torch.zeros(max(tiles, 4096), device=device, dtype=torch.int32))
-        _WS[key] = ws
-    return ws
-
-
 # TIMING EXPERIMENT ONLY (never set in a real run: the model does not learn): EDL_DEBUG_SKIP_WGRAD=1 drops every
 # weight-gradient kernel of the wgmma / library conv paths, which bounds what faster wgrad kernels could buy.
 _SKIP_WGRAD = __import__("os").environ.get("EDL_DEBUG_SKIP_WGRAD", "0") == "1"
 
 
 _PART = {}
-# split-K without atomics (csrc/gemm.h GemmArgs::partials): EDL_SPLITK_PARTIALS=0 goes back to fp32 reductions
-SPLITK_PARTIALS = __import__("os").environ.get("EDL_SPLITK_PARTIALS", "1") == "1"
+_STEM_SCRATCH = {}
 
 
-def _splitk_partials(device):
-    """Per (device, stream) scratch for the split-K partial tiles: 132-264 CTAs x (128 x 384) fp32 at most."""
-    if not SPLITK_PARTIALS:
-        return None
+def _splitk_partials(device, numel):
+    """Per (device, stream) scratch of at least ``numel`` fp32 for the split-K partial tiles (csrc/gemm.h
+    GemmArgs::partials).  It starts at 64 MB, more than the ResNet50_vd weight gradients at batch 32 need, so a
+    training step never grows it; a larger request replaces it."""
     key = (device.index, torch.cuda.current_stream(device).cuda_stream)
     buf = _PART.get(key)
+    if buf is None or buf.numel() < numel:
+        buf = _PART[key] = torch.empty(max(numel, 16 << 20), device=device, dtype=torch.float32)
+    return buf
+
+
+def _stem_scratch(device):
+    """Per (device, stream) all-zero fp32 [1024] + int32 [1] of the stem weight gradient's in-kernel reduction
+    (csrc/stem.cu), which leaves both zeroed again."""
+    key = (device.index, torch.cuda.current_stream(device).cuda_stream)
+    buf = _STEM_SCRATCH.get(key)
     if buf is None:
-        buf = _PART[key] = torch.empty(16 << 20, device=device, dtype=torch.float32)      # 64 MB
+        buf = _STEM_SCRATCH[key] = (torch.zeros(1024, device=device, dtype=torch.float32),
+                                    torch.zeros(1, device=device, dtype=torch.int32))
     return buf
 
 
@@ -210,31 +191,33 @@ def _deliver_wgrad(dy, x, sink, ready, compute):
 
 
 def _wgrad(dy2, x2, weight_shape, sink, ready):
-    """dW[Cout, Cin] = dy2[M, Cout]^T @ x2[M, Cin]: fp32 split-K accumulation whose last CTA per
-    tile converts to bf16 straight into the (flat gradient bucket) sink -- no memset / cast / add
-    kernels around it."""
+    """dW[Cout, Cin] = dy2[M, Cout]^T @ x2[M, Cin], written as bf16 straight into the (flat gradient bucket) sink --
+    no memset / cast / add kernels around it."""
     return _deliver_wgrad(dy2, x2, sink, ready, lambda s: _wgrad_impl(dy2, x2, weight_shape, s))
 
 
-def _wgrad_impl(dy2, x2, weight_shape, sink):
+def _wgrad_impl(dy2, x2, weight_shape, sink, split_k: Optional[int] = None):
+    from . import native, count_launch
+
     cout, cin = dy2.shape[1], x2.shape[1]
-    split = _split_k_for(cout, cin, dy2.shape[0])
-    if dy2.is_cuda and cin % 4 == 0:
-        tiles = ((cout + 127) // 128) * ((cin + 63) // 64)
-        ws, counters = _splitk_workspace(dy2.device, cout * cin, tiles)
-        if sink is not None:
-            out, acc = sink.view(cout, cin), True
-        else:
-            out, acc = torch.empty((cout, cin), device=dy2.device, dtype=torch.bfloat16), False
-        gemm_bf16(dy2, x2, a_mn_major=True, b_mn_major=True, out_f32=ws[:cout * cin].view(cout, cin),
-                  split_k=split, out_bf16=out, tile_counters=counters, accumulate_out=acc,
-                  partials=_splitk_partials(dy2.device) if split > 1 else None)
+    if dy2.is_cuda and _tma_compatible(dy2, x2, None, cin):
+        split = split_k if split_k is not None else _split_k_for(cout, cin, dy2.shape[0])
+        out = sink.view(cout, cin) if sink is not None else torch.empty((cout, cin), device=dy2.device,
+                                                                        dtype=torch.bfloat16)
+        block_n = 64 if cin <= 64 else 128      # the kernel's tile width (csrc/gemm.cu)
+        tiles = ((cout + 127) // 128) * ((cin + block_n - 1) // block_n)
+        partials = _splitk_partials(dy2.device, split * tiles * 128 * block_n) if split > 1 else None
+        native().gemm_wgrad_bf16(dy2, x2, out, split, sink is not None, partials)
+        count_launch()
         return None if sink is not None else out.view(weight_shape)
-    acc = torch.zeros((cout, cin), device=dy2.device, dtype=torch.float32)
-    gemm_bf16(dy2, x2, a_mn_major=True, b_mn_major=True, out_f32=acc, split_k=split)
+    if dy2.is_cuda:
+        from . import count_fallback
+        count_fallback("gemm_bf16: operand not TMA-describable (pitch / base not 16-byte aligned or not bf16): "
+                       "fp32 matmul on the library, %s x %s" % (tuple(dy2.shape), tuple(x2.shape)))
+    d = dy2.float().t() @ x2.float()
     if sink is None:
-        return acc.to(torch.bfloat16).view(weight_shape)
-    sink.view(cout, cin).add_(acc)
+        return d.to(torch.bfloat16).view(weight_shape)
+    sink.view(cout, cin).add_(d)
 
 
 class _Conv1x1Fn(torch.autograd.Function):
@@ -510,7 +493,7 @@ def conv3x3_wgrad_supported(x, weight_krsc) -> bool:
 def conv3x3_wgrad(x, dy, weight_shape, sink=None, split_k: Optional[int] = None):
     """dW [Cout, 3, 3, Cin] of the 3x3 / stride 1 / pad 1 convolution on the wgmma kernel
     (csrc/conv3x3_wgrad.cu).  With ``sink`` (a flat bf16 window of the gradient bucket) the result is ADDED
-    into it by the kernel's fused finalize and ``None`` is returned; otherwise a new tensor is returned."""
+    into it and ``None`` is returned; otherwise a new tensor is returned."""
     from . import native, count_launch
 
     x, dy = _cl(x), _cl(dy)
@@ -518,7 +501,6 @@ def conv3x3_wgrad(x, dy, weight_shape, sink=None, split_k: Optional[int] = None)
     n, _, h, w = dy.shape                 # stride 2: x is twice as large; the pixel blocks tile dy
     s2 = x.shape[2] != h
     tiles = native().conv3x3_wgrad_tiles(cin, cout)
-    ws, counters = _splitk_workspace(x.device, cout * 9 * cin, tiles)
     if split_k is None:
         if s2:                           # always the version-1 kernel (its pixel-block plan, 64-wide Cin tiles)
             kblocks, ctas = native().conv3x3_wgrad_s2_kblocks(n, h, w), tiles
@@ -532,9 +514,9 @@ def conv3x3_wgrad(x, dy, weight_shape, sink=None, split_k: Optional[int] = None)
         out, acc = sink.view(weight_shape), True
     else:
         out, acc = torch.empty(tuple(weight_shape), device=x.device, dtype=torch.bfloat16), False
-    native().conv3x3_wgrad(x, dy, out, ws, counters, int(split_k), acc,
-                           _splitk_partials(x.device) if split_k > 1 else None)
-    count_launch(2 if (split_k > 1 and SPLITK_PARTIALS) else 1)
+    partials = _splitk_partials(x.device, split_k * tiles * 128 * 192) if split_k > 1 else None
+    native().conv3x3_wgrad(x, dy, out, int(split_k), acc, partials)
+    count_launch(2 if split_k > 1 else 1)
     return None if sink is not None else out
 
 
@@ -726,7 +708,7 @@ class _StemConvFn(torch.autograd.Function):
             def wgrad(sink):
                 if not (x.shape[2] % 2 == 0 and x.shape[3] % 2 == 0 and x.shape[3] <= 4096):
                     return _lib_wgrad(dy, x, w, ctx.cfg, sink)
-                ws, counters = _splitk_workspace(x.device, 1024, 1)
+                ws, counters = _stem_scratch(x.device)
                 out = sink.view(w.shape) if sink is not None else torch.empty_like(w)
                 native().stem_wgrad(x, dy, out, ws, counters, sink is not None)
                 count_launch()

@@ -50,13 +50,22 @@ def test_gemm_b_mn_major(m, n, k):
 
 @pytest.mark.parametrize("m,n,k,split", [(256, 64, 1000, 4), (512, 128, 6272, 16), (64, 64, 100352 // 8, 32),
                                          (1000, 2048, 32, 1)])
-def test_gemm_wgrad_splitk(m, n, k, split):
+def test_gemm_wgrad_bf16_splitk(m, n, k, split):
+    from edl_b200.ops import gemm as G
+
     torch.manual_seed(0)
     a = torch.randn(k, m, device=DEV).bfloat16()   # [K, M]
     b = torch.randn(k, n, device=DEV).bfloat16()   # [K, N]
-    acc = torch.zeros(m, n, device=DEV)
-    ops.gemm_bf16(a, b, a_mn_major=True, b_mn_major=True, out_f32=acc, split_k=split)
-    assert _rel(acc, a.float().t() @ b.float()) < 5e-3
+    ref = a.float().t() @ b.float()
+    ops.reset_launches()
+    d = G._wgrad_impl(a, b, (m, n), None, split_k=split)
+    assert ops.launches() == 1                      # the wgmma kernel, not the library fallback
+    assert d.dtype == torch.bfloat16 and _rel(d, ref) < 5e-3
+    # accumulate into a prefilled output (a window of the flat gradient bucket)
+    sink = torch.randn(m * n, device=DEV).bfloat16()
+    want = sink.float().view(m, n) + ref
+    assert G._wgrad_impl(a, b, (m, n), sink, split_k=split) is None
+    assert _rel(sink.view(m, n), want) < 5e-3
 
 
 @pytest.mark.parametrize("n,cin,cout,hw", [(2, 64, 256, 56), (4, 256, 64, 14), (3, 512, 2048, 7), (2, 1024, 256, 14)])

@@ -33,14 +33,13 @@ for (m,n,k) in [(128,128,64),(300,128,64),(1568,512,2048),(500,64,256)]:
     print('bmn',m,n,k,'rel',((d.float()-ref).norm()/ref.norm()).item())
 """,
     "gemm_wgrad": """
-import torch; from edl_b200 import ops
+import torch; from edl_b200.ops import gemm as G
 torch.manual_seed(0)
 for (m,n,k,s) in [(128,128,64,1),(256,64,1000,4),(512,128,6272,16),(1000,2048,32,1)]:
     a=torch.randn(k,m,device='cuda').bfloat16(); b=torch.randn(k,n,device='cuda').bfloat16()
-    acc=torch.zeros(m,n,device='cuda')
-    ops.gemm_bf16(a,b,a_mn_major=True,b_mn_major=True,out_f32=acc,split_k=s); torch.cuda.synchronize()
+    out=G._wgrad_impl(a,b,(m,n),None,split_k=s); torch.cuda.synchronize()
     ref=a.float().t()@b.float()
-    print('wgrad',m,n,k,s,'rel',((acc-ref).norm()/ref.norm()).item())
+    print('wgrad',m,n,k,s,'rel',((out.float()-ref).norm()/ref.norm()).item())
 """,
     "gemm_stats": """
 import torch; from edl_b200 import ops

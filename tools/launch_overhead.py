@@ -40,7 +40,7 @@ def B():   # plain elementwise, no smem
 
 
 def G():   # wgmma GEMM, 99 KB dynamic smem
-    C.gemm_bf16(x2, w, out, False, False, None, None, False, None, None, 1, None, None, False, None, None, False, None)
+    C.gemm_bf16(x2, w, out, False, False, None, None, False, None, None, None, False)
 
 
 def D():   # cuDNN conv
