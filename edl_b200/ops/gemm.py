@@ -59,7 +59,11 @@ def gemm_bf16(a, b, out=None, a_mn_major=False, b_mn_major=False, col_scale=None
         out = torch.empty((m, n), device=a.device, dtype=torch.bfloat16)
     if add is not None and not (native().persistent_gemm_enabled() and n % 8 == 0 and add.stride(-1) == 1
                                 and add.stride(0) % 8 == 0 and add.data_ptr() % 16 == 0):
-        # the fused addend lives in the persistent kernel's epilogue; otherwise one extra elementwise pass
+        # the fused addend lives in the persistent kernel's epilogue; otherwise one extra elementwise pass, which is
+        # only the same operation when nothing follows the addition in the epilogue
+        if col_scale is not None or col_shift is not None or relu or col_stats is not None:
+            raise RuntimeError("gemm_bf16: an addend together with scale / shift / ReLU / statistics needs the persistent "
+                               "kernel's fused addend (persistent GEMM on, N % 8 == 0, 16-byte aligned addend rows)")
         native().gemm_bf16(a, b, out, a_mn_major, b_mn_major, col_scale, col_shift, relu, col_stats, None, None, False)
         count_launch()
         out.add_(add)
@@ -490,6 +494,20 @@ def conv3x3_wgrad_supported(x, weight_krsc) -> bool:
     return kh == 3 and kw == 3 and cin == c and native().conv3x3_wgrad_supported(n, h, w, cin, cout)
 
 
+def conv3x3_wgrad_split(n, h, w, cin, cout, s2=False) -> int:
+    """Split-K factor ``conv3x3_wgrad`` uses when it is not given one; (n, h, w) is the geometry of dy."""
+    from . import native
+
+    if s2:                               # always the version-1 kernel (its pixel-block plan, 64-wide Cin tiles)
+        kblocks, ctas = native().conv3x3_wgrad_s2_kblocks(n, h, w), native().conv3x3_wgrad_tiles(cin, cout)
+    else:
+        kblocks = native().conv3x3_wgrad_kblocks(n, h, w)
+        ctas = native().conv3x3_wgrad_ctas(cin, cout)
+    # one wave of CTAs, at least two pixel blocks per CTA; no split once a third of the SMs have a CTA (same rule as
+    # the 1x1 wgrad split)
+    return 1 if ctas >= 48 else max(1, min(max(1, _NUM_SMS // ctas), max(1, kblocks // 2)))
+
+
 def conv3x3_wgrad(x, dy, weight_shape, sink=None, split_k: Optional[int] = None):
     """dW [Cout, 3, 3, Cin] of the 3x3 / stride 1 / pad 1 convolution on the wgmma kernel
     (csrc/conv3x3_wgrad.cu).  With ``sink`` (a flat bf16 window of the gradient bucket) the result is ADDED
@@ -502,14 +520,7 @@ def conv3x3_wgrad(x, dy, weight_shape, sink=None, split_k: Optional[int] = None)
     s2 = x.shape[2] != h
     tiles = native().conv3x3_wgrad_tiles(cin, cout)
     if split_k is None:
-        if s2:                           # always the version-1 kernel (its pixel-block plan, 64-wide Cin tiles)
-            kblocks, ctas = native().conv3x3_wgrad_s2_kblocks(n, h, w), tiles
-        else:
-            kblocks = native().conv3x3_wgrad_kblocks(n, h, w)
-            ctas = native().conv3x3_wgrad_ctas(cin, cout)
-        # one wave of CTAs, at least two pixel blocks per CTA; no split once a third of the SMs have a CTA (same rule
-        # as the 1x1 wgrad split)
-        split_k = 1 if ctas >= 48 else max(1, min(max(1, _NUM_SMS // ctas), max(1, kblocks // 2)))
+        split_k = conv3x3_wgrad_split(n, h, w, cin, cout, s2)
     if sink is not None:
         out, acc = sink.view(weight_shape), True
     else:
@@ -655,13 +666,15 @@ def stem7_infer(x, weight_krsc, scale=None, shift=None, relu=False):
     n, _, h, w = x.shape
     ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
     cout = weight_krsc.shape[0]
-    key = (weight_krsc.data_ptr(), weight_krsc._version, str(weight_krsc.device))
-    wp = _STEM7_W.get(key)
-    if wp is None:
-        _STEM7_W.clear()
+    # the padded weight is cached per weight tensor (held, so that its address cannot be reused by another tensor and
+    # alias a stale entry) and version
+    hit = _STEM7_W.get("w")
+    if hit is not None and hit[0] is weight_krsc and hit[1] == weight_krsc._version:
+        wp = hit[2]
+    else:
         wp = torch.zeros((cout, 160), device=x.device, dtype=torch.bfloat16)
         wp[:, :147] = weight_krsc.reshape(cout, 147)
-        _STEM7_W[key] = wp
+        _STEM7_W["w"] = (weight_krsc, weight_krsc._version, wp)
     a = torch.empty((n * ho * wo, 160), device=x.device, dtype=torch.bfloat16)
     native().stem7_im2col(x, a)
     count_launch()

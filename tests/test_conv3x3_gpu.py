@@ -2,16 +2,12 @@
 fp32 PyTorch convolution; autograd wrapper incl. the side-stream library wgrad."""
 import pytest
 import torch
-import torch.nn.functional as F
 
+import f64_bounds as fb
 from edl_b200 import ops
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-
-
-def _rel(a, b):
-    return ((a.float() - b.float()).norm() / (b.float().norm() + 1e-12)).item()
 
 
 SHAPES = [  # n, cin, cout, h, w
@@ -27,12 +23,10 @@ def test_conv3x3_fprop_and_stats(n, cin, cout, h, w):
     assert ops.conv3x3_supported(x, wt)
     stats = torch.zeros(2 * cout, device=DEV)
     y = ops.conv3x3(x, wt, stats)
-    ref = F.conv2d(x.float(), wt.permute(0, 3, 1, 2).float(), None, 1, 1)
-    assert y.shape == ref.shape and y.is_contiguous(memory_format=torch.channels_last)
-    assert _rel(y, ref) < 1e-2
-    yf = y.float()
-    assert _rel(stats[:cout], yf.sum((0, 2, 3))) < 2e-3
-    assert _rel(stats[cout:], (yf * yf).sum((0, 2, 3))) < 2e-3
+    ref = fb.conv_ref(x, wt)
+    assert y.shape == ref[0].shape and y.is_contiguous(memory_format=torch.channels_last)
+    fb.check_bf16(y, *ref, 9 * cin, what="conv3x3 fprop")
+    fb.check_sums(stats, *fb.stats_ref(y), n * h * w, what="conv3x3 stats")
 
 
 @pytest.mark.parametrize("n,cin,cout,h,w", [s for s in SHAPES if s[1] % 64 == 0 and (s[1] <= 64 or s[1] % 128 == 0)])
@@ -43,11 +37,13 @@ def test_conv3x3_dgrad_and_wgrad(n, cin, cout, h, w):
     y = ops.conv3x3(x, wt)
     dy = torch.randn_like(y)
     y.backward(dy)
-    xr = x.detach().float().requires_grad_(True)
-    wr = wt.detach().float().requires_grad_(True)
-    F.conv2d(xr, wr.permute(0, 3, 1, 2), None, 1, 1).backward(dy.float())
-    assert _rel(x.grad, xr.grad) < 1e-2
-    assert _rel(wt.grad, wr.grad) < 1e-2
+    xd, wd = x.detach(), wt.detach()
+    fb.check_bf16(x.grad, *fb.dgrad_ref(dy, wd, x.shape), 9 * cout, what="conv3x3 dgrad")
+    # the weight gradient of this path is the library's (EDL_OWN_WGRAD3 off): its split-K is unknown, so allow one
+    # partial per 64-pixel block
+    k = n * h * w
+    fb.check_bf16(wt.grad.view(cout, -1), *[t.reshape(cout, -1) for t in fb.wgrad_ref(xd, dy, wd.shape)], k, k // 64 + 1,
+                  what="conv3x3 library wgrad")
 
 
 def test_conv3x3_unsupported_shapes_are_reported():

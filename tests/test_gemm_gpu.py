@@ -1,16 +1,13 @@
-"""wgmma GEMM / 1x1-conv kernel numerics vs fp32 PyTorch matmul / conv2d."""
+"""wgmma GEMM / 1x1-conv kernel numerics against float64 references, element by element (tests/f64_bounds.py)."""
 import pytest
 import torch
-import torch.nn.functional as F
 
+import f64_bounds as fb
 from edl_b200 import ops
+from edl_b200.ops import gemm as G
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-
-
-def _rel(a, b):
-    return ((a.float() - b.float()).norm() / (b.float().norm() + 1e-12)).item()
 
 
 @pytest.mark.parametrize("m,n,k", [(128, 128, 64), (300, 128, 64), (1568, 2048, 512), (257, 64, 256),
@@ -20,8 +17,7 @@ def test_gemm_tn(m, n, k):
     a = torch.randn(m, k, device=DEV).bfloat16()
     b = torch.randn(n, k, device=DEV).bfloat16()
     d = ops.gemm_bf16(a, b)
-    ref = a.float() @ b.float().t()
-    assert _rel(d, ref) < 1e-2
+    fb.check_bf16(d, *fb.gemm_ref(a, b), k, what="gemm")
 
 
 def test_gemm_epilogue_scale_shift_relu_stats():
@@ -33,10 +29,8 @@ def test_gemm_epilogue_scale_shift_relu_stats():
     shift = torch.randn(n, device=DEV)
     stats = torch.zeros(2 * n, device=DEV)
     d = ops.gemm_bf16(a, b, col_scale=scale, col_shift=shift, relu=True, col_stats=stats)
-    ref = torch.relu((a.float() @ b.float().t()) * scale + shift)
-    assert _rel(d, ref) < 1e-2
-    assert _rel(stats[:n], d.float().sum(0)) < 1e-3
-    assert _rel(stats[n:], (d.float() ** 2).sum(0)) < 1e-3
+    fb.check_bf16(d, *fb.gemm_ref(a, b, scale=scale, shift=shift, relu=True), k, what="gemm ssr")
+    fb.check_sums(stats, *fb.stats_ref(d), m, what="gemm stats")
 
 
 @pytest.mark.parametrize("m,n,k", [(300, 128, 64), (1568, 512, 2048), (500, 64, 256), (32, 2048, 1000)])
@@ -45,27 +39,25 @@ def test_gemm_b_mn_major(m, n, k):
     a = torch.randn(m, k, device=DEV).bfloat16()
     b = torch.randn(k, n, device=DEV).bfloat16()
     d = ops.gemm_bf16(a, b, b_mn_major=True)
-    assert _rel(d, a.float() @ b.float()) < 1e-2
+    fb.check_bf16(d, *fb.gemm_ref(a, b, b_mn_major=True), k, what="dgrad gemm")
 
 
 @pytest.mark.parametrize("m,n,k,split", [(256, 64, 1000, 4), (512, 128, 6272, 16), (64, 64, 100352 // 8, 32),
                                          (1000, 2048, 32, 1)])
 def test_gemm_wgrad_bf16_splitk(m, n, k, split):
-    from edl_b200.ops import gemm as G
-
     torch.manual_seed(0)
     a = torch.randn(k, m, device=DEV).bfloat16()   # [K, M]
     b = torch.randn(k, n, device=DEV).bfloat16()   # [K, N]
-    ref = a.float().t() @ b.float()
     ops.reset_launches()
     d = G._wgrad_impl(a, b, (m, n), None, split_k=split)
     assert ops.launches() == 1                      # the wgmma kernel, not the library fallback
-    assert d.dtype == torch.bfloat16 and _rel(d, ref) < 5e-3
+    assert d.dtype == torch.bfloat16
+    fb.check_bf16(d, *fb.gemm_ref(a, b, a_mn_major=True, b_mn_major=True), k, split, what="wgrad gemm")
     # accumulate into a prefilled output (a window of the flat gradient bucket)
     sink = torch.randn(m * n, device=DEV).bfloat16()
-    want = sink.float().view(m, n) + ref
+    want = fb.gemm_ref(a, b, a_mn_major=True, b_mn_major=True, add=sink.view(m, n))
     assert G._wgrad_impl(a, b, (m, n), sink, split_k=split) is None
-    assert _rel(sink.view(m, n), want) < 5e-3
+    fb.check_bf16(sink.view(m, n), *want, k, split, what="wgrad gemm sink")
 
 
 @pytest.mark.parametrize("n,cin,cout,hw", [(2, 64, 256, 56), (4, 256, 64, 14), (3, 512, 2048, 7), (2, 1024, 256, 14)])
@@ -78,14 +70,13 @@ def test_conv1x1_fwd_bwd(n, cin, cout, hw):
     y = ops.conv1x1(x, w, stats)
     dy = torch.randn_like(y)
     y.backward(dy)
-    xr = x.detach().float().requires_grad_(True)
-    wr = w.detach().float().permute(0, 3, 1, 2).contiguous().requires_grad_(True)
-    yr = F.conv2d(xr, wr)
-    yr.backward(dy.float())
-    assert _rel(y, yr) < 1e-2
-    assert _rel(x.grad, xr.grad) < 1e-2
-    assert _rel(w.grad.permute(0, 3, 1, 2), wr.grad) < 1e-2
-    assert _rel(stats[:cout], y.float().sum((0, 2, 3))) < 1e-3
+    xd, wd = x.detach(), w.detach()
+    fb.check_bf16(y, *fb.conv_ref(xd, wd, padding=0), cin, what="conv1x1 fprop")
+    fb.check_sums(stats, *fb.stats_ref(y), y.numel() // cout, what="conv1x1 stats")
+    fb.check_bf16(x.grad, *fb.dgrad_ref(dy, wd, x.shape, padding=0), cout, what="conv1x1 dgrad")
+    m = n * hw * hw
+    fb.check_bf16(w.grad.reshape(cout, cin), *fb.gemm_ref(fb.rows(dy), fb.rows(xd), a_mn_major=True, b_mn_major=True), m,
+                  G._split_k_for(cout, cin, m), what="conv1x1 wgrad")
 
 
 def test_linear_bf16():
@@ -96,8 +87,10 @@ def test_linear_bf16():
     y = ops.linear_bf16(x, w, b)
     dy = torch.randn_like(y)
     y.backward(dy)
-    xr, wr, br = [t.detach().float().requires_grad_(True) for t in (x, w, b)]
-    yr = F.linear(xr, wr, br)
-    yr.backward(dy.float())
-    assert _rel(y, yr) < 1e-2 and _rel(x.grad, xr.grad) < 1e-2
-    assert _rel(w.grad, wr.grad) < 1e-2 and _rel(b.grad, br.grad) < 1e-2
+    xd, wd = x.detach(), w.detach()
+    fb.check_bf16(y, *fb.gemm_ref(xd, wd, shift=b.detach().float()), 2048, what="linear")
+    fb.check_bf16(x.grad, *fb.gemm_ref(dy, wd, b_mn_major=True), 1000, what="linear dgrad")
+    fb.check_bf16(w.grad, *fb.gemm_ref(dy, xd, a_mn_major=True, b_mn_major=True), 32, G._split_k_for(1000, 2048, 32),
+                  what="linear wgrad")
+    # the bias gradient is an fp32 column sum of dy (one rounding per row)
+    fb.check_sums(b.grad, dy.double().sum(0), dy.double().abs().sum(0), 32, what="linear bias grad", tau_s=33 * fb.EPS32)

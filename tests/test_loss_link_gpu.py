@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from edl_b200 import ops
+from f64_bounds import ulp
 from edl_b200.ops.loss import _MODE, _ref_loss, _smoothed_onehot_plogp
 
 gpu = pytest.mark.gpu
@@ -39,12 +40,6 @@ def ref_soft_ce(z, target, kind, ts=1.0, tt=1.0, eps=0.0, kl=False, scale=1.0):
         row = row + torch.xlogy(p, p).sum(-1)
     grad = (torch.softmax(z64, -1) * p.sum(-1, keepdim=True) - p) * (scale / ts / n)
     return row.mean().item() * scale, grad
-
-
-def ulp(x, mant_bits):
-    """Unit in the last place of float64 values ``x`` in a format with ``mant_bits`` significant bits (0 at 0)."""
-    _, e = torch.frexp(x)
-    return torch.where(x == 0, torch.zeros_like(x), torch.ldexp(torch.ones_like(x), e - mant_bits))
 
 
 def assert_loss(got, ref, what):

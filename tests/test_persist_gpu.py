@@ -2,16 +2,12 @@
 the fp32 reference: many tiles per CTA (ring wrap-around across tiles)."""
 import pytest
 import torch
-import torch.nn.functional as F
 
+import f64_bounds as fb
 from edl_b200 import ops
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-
-
-def _rel(a, b):
-    return ((a.float() - b.float()).norm() / (b.float().norm() + 1e-12)).item()
 
 
 @pytest.fixture(autouse=True)
@@ -27,16 +23,15 @@ def test_persistent_gemm_matches_reference_and_stats(m, n, k, b_mn):
     torch.manual_seed(0)
     a = torch.randn(m, k, device=DEV).bfloat16()
     b = (torch.randn(k, n, device=DEV) if b_mn else torch.randn(n, k, device=DEV)).bfloat16()
-    ref = a.float() @ (b.float() if b_mn else b.float().t())
+    ref = fb.gemm_ref(a, b, b_mn_major=b_mn)
     outs = []
     for persistent in (True, False):
         ops.native().set_persistent_gemm(persistent)
         stats = torch.zeros(2 * n, device=DEV)
         d = ops.gemm_bf16(a, b, b_mn_major=b_mn, col_stats=None if b_mn else stats)
-        assert _rel(d, ref) < 1e-2, persistent
+        fb.check_bf16(d, *ref, k, what="gemm persistent=%s" % persistent)
         if not b_mn:
-            assert _rel(stats[:n], d.float().sum(0)) < 2e-3
-            assert _rel(stats[n:], (d.float() ** 2).sum(0)) < 2e-3
+            fb.check_sums(stats, *fb.stats_ref(d), m, what="gemm stats persistent=%s" % persistent)
         outs.append(d)
     assert torch.equal(outs[0], outs[1])          # same MMA order => bit-identical results
 
@@ -51,13 +46,13 @@ def test_wide_tile_gemm_matches_the_128_wide_tiles(m, n, k, res):
     b = (torch.randn(n, k, device=DEV) * 0.05).bfloat16()
     sh = torch.randn(n, device=DEV)
     add = torch.randn(m, n, device=DEV).bfloat16() if res else None
-    ref = a.float() @ b.float().t() + sh + (add.float() if res else 0.0)
+    ref = fb.gemm_ref(a, b, add=add, shift=sh, relu=True)
     outs = []
     try:
         for wide in (True, False):
             ops.native().set_wide_gemm_tiles(wide)
             d = ops.gemm_bf16(a, b, col_shift=sh, relu=True, add=add)
-            assert _rel(d, torch.relu(ref)) < 1e-2, wide
+            fb.check_bf16(d, *ref, k, what="gemm wide=%s" % wide)
             outs.append(d)
     finally:
         ops.native().set_wide_gemm_tiles(True)
@@ -77,10 +72,8 @@ def test_inference_gemm_epilogue_on_large_shapes(m, n, k, res, scale):
     sh = torch.randn(n, device=DEV)
     sc = (torch.rand(n, device=DEV) + 0.5) if scale else None
     add = torch.randn(m, n, device=DEV).bfloat16() if res else None
-    ref = a.float() @ b.float().t() + (add.float() if res else 0.0)
-    ref = torch.relu((ref * sc if scale else ref) + sh)
     d = ops.gemm_bf16(a, b, col_scale=sc, col_shift=sh, relu=True, add=add)
-    assert _rel(d, ref) < 1e-2
+    fb.check_bf16(d, *fb.gemm_ref(a, b, add=add, scale=sc, shift=sh, relu=True), k, what="gemm epilogue")
     if not res:
         nat.set_persistent_gemm(False)
         assert torch.equal(d, ops.gemm_bf16(a, b, col_scale=sc, col_shift=sh, relu=True))
@@ -100,7 +93,7 @@ def test_sixteen_epilogue_warps_match_eight(m, n, k):
     xc = torch.randn(8, 128, 28, 28, device=DEV).bfloat16().contiguous(memory_format=torch.channels_last)
     wc = (torch.randn(128, 3, 3, 128, device=DEV) * 0.05).bfloat16()
     res = []
-    h = _hook(x, None, n, True)
+    h = fb.bn_hook(x, None, n, True)
     try:
         for warps in (16, 8):
             nat.set_epilogue_warps(warps)
@@ -115,10 +108,15 @@ def test_sixteen_epilogue_warps_match_eight(m, n, k):
         nat.set_epilogue_warps(8)
     for i in (0, 2, 4):
         assert torch.equal(res[0][i], res[1][i]), i
-    for i in (1, 3, 5):
-        assert _rel(res[0][i], res[1][i]) < 1e-4, i
-    assert _rel(res[0][0], a.float() @ b.float().t()) < 1e-2
-    assert _rel(res[0][3], _bn_ref_sums(res[0][2], x, None, h.mean, h.rstd, h.gamma, h.beta, True)) < 5e-3
+    for warps, (d, st, g, dsums, yc, cst) in zip((16, 8), res):
+        # the statistics sum in a different order per warp count: both pass the oracle
+        fb.check_bf16(d, *fb.gemm_ref(a, b), k, what="gemm %d warps" % warps)
+        fb.check_sums(st, *fb.stats_ref(d), m, what="gemm stats %d warps" % warps)
+        fb.check_bf16(g, *fb.gemm_ref(a, wmn, b_mn_major=True), k, what="dgrad %d warps" % warps)
+        ref, mag, extra = fb.bn_dsums_ref(g, x, h.mean, h.rstd, h.gamma, h.beta, True)
+        fb.check_sums(dsums, ref, mag, m, what="dgrad dsums %d warps" % warps, extra=extra)
+        fb.check_bf16(yc, *fb.conv_ref(xc, wc), 9 * 128, what="conv3x3 %d warps" % warps)
+        fb.check_sums(cst, *fb.stats_ref(yc), yc.numel() // 128, what="conv3x3 stats %d warps" % warps)
 
 
 @pytest.mark.parametrize("kind,shape", [("gemm", (100352, 256, 64)), ("gemm", (5000, 192, 192)), ("gemm", (6272, 1024, 256)),
@@ -138,11 +136,11 @@ def test_forward_bn_statistics_match_fp32_sums_of_the_stored_output(kind, shape)
         wt = (torch.randn(n, 3, 3, c, device=DEV) * 0.05).bfloat16()
     st = torch.zeros(2 * n, device=DEV)
     y = ops.gemm_bf16(a, b, col_stats=st) if kind == "gemm" else ops.conv3x3(x, wt, st)
-    yf = y.float()
-    dims = 0 if kind == "gemm" else (0, 2, 3)
-    ref = torch.cat([yf.sum(dims), (yf * yf).sum(dims)])
-    assert _rel(st[n:], ref[n:]) < 1e-4          # sums of squares: no cancellation
-    assert (st[:n] - ref[:n]).abs().max().item() < 2e-3 * ref[n:].sqrt().max().item() + 1e-3
+    if kind == "gemm":
+        fb.check_bf16(y, *fb.gemm_ref(a, b), k, what="gemm")
+    else:
+        fb.check_bf16(y, *fb.conv_ref(x, wt), 9 * c, what="conv3x3")
+    fb.check_sums(st, *fb.stats_ref(y), y.numel() // n, what="%s stats" % kind)
 
 
 def test_persistent_gemm_epilogue_scale_shift_relu():
@@ -152,7 +150,7 @@ def test_persistent_gemm_epilogue_scale_shift_relu():
     b = torch.randn(n, k, device=DEV).bfloat16()
     sc, sh = torch.rand(n, device=DEV) + 0.5, torch.randn(n, device=DEV)
     d = ops.gemm_bf16(a, b, col_scale=sc, col_shift=sh, relu=True)
-    assert _rel(d, torch.relu((a.float() @ b.float().t()) * sc + sh)) < 1e-2
+    fb.check_bf16(d, *fb.gemm_ref(a, b, scale=sc, shift=sh, relu=True), k, what="gemm ssr")
 
 
 @pytest.mark.parametrize("n,cin,cout,h,w", [(32, 64, 64, 56, 56), (32, 128, 128, 28, 28), (32, 256, 256, 14, 14),
@@ -167,20 +165,20 @@ def test_persistent_conv3x3_matches_tile_kernel(n, cin, cout, h, w):
         st = torch.zeros(2 * cout, device=DEV)
         y = ops.conv3x3(x, wt, st)
         res.append((y, st))
-    # the haloed-tile version accumulates in (filter row, k-block, tap) order, the tile kernel in (tap, k-block) order
-    assert _rel(res[0][0], res[1][0]) < 2e-3
-    assert _rel(res[0][1], res[1][1]) < 2e-3
-    ref = F.conv2d(x.float(), wt.permute(0, 3, 1, 2).float(), None, 1, 1)
-    assert _rel(res[0][0], ref) < 1e-2
+    # the haloed-tile version accumulates in (filter row, k-block, tap) order, the tile kernel in (tap, k-block) order:
+    # both pass the oracle
+    ref = fb.conv_ref(x, wt)
+    for persistent, (y, st) in zip((True, False), res):
+        fb.check_bf16(y, *ref, 9 * cin, what="conv3x3 persistent=%s" % persistent)
+        fb.check_sums(st, *fb.stats_ref(y), n * h * w, what="conv3x3 stats persistent=%s" % persistent)
     if cin <= 64 or cin % 128 == 0:
         dy = torch.randn_like(res[0][0])
-        dxs = []
+        dref = fb.dgrad_ref(dy, wt, x.shape)
         for persistent in (True, False):
             ops.native().set_persistent_gemm(persistent)
             dx = torch.empty_like(x)
             ops.native().conv3x3(dy, wt, dx, True, None, None, False)
-            dxs.append(dx)
-        assert _rel(dxs[0], dxs[1]) < 2e-3
+            fb.check_bf16(dx, *dref, 9 * cout, what="conv3x3 dgrad persistent=%s" % persistent)
 
 
 @pytest.mark.parametrize("n,cin,cout,h,w,groups", [(32, 64, 64, 56, 56, 1), (8, 128, 128, 28, 28, 1), (9, 256, 256, 14, 14, 1),
@@ -217,22 +215,16 @@ def test_haloed_conv3x3_tiles_match_the_shifted_box_version(n, cin, cout, h, w, 
     finally:
         nat.set_conv_halo(True)
         nat.set_conv_resident_weights(True)
-    wf = wt.permute(0, 3, 1, 2).float()
-    ref = F.conv2d(x.float(), wf, None, 1, 1, 1, groups)
-    if groups > 1:
-        ref = torch.relu(ref * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
-    assert _rel(outs[0][0], ref) < 1e-2
-    assert _rel(outs[0][0], outs[2][0]) < 2e-3
+    epi = dict(scale=scale.view(1, -1, 1, 1), shift=shift.view(1, -1, 1, 1), relu=True) if groups > 1 else {}
+    ref = fb.conv_ref(x, wt, groups=groups, **epi)
     assert torch.equal(outs[0][0], outs[1][0])          # same accumulation order, only the tile schedule differs
-    if outs[0][1] is not None:
-        assert _rel(outs[0][1], outs[1][1]) < 1e-4
-        yf = outs[0][0].float()
-        assert _rel(outs[0][1][:cout], yf.sum((0, 2, 3))) < 2e-3
-        assert _rel(outs[0][1][cout:], (yf * yf).sum((0, 2, 3))) < 2e-3
-    if outs[0][2] is not None:
-        for y, _, dx, dy in outs:
-            dref = torch.nn.grad.conv2d_input(x.shape, wf, dy.float(), 1, 1)
-            assert _rel(dx, dref) < 1e-2
+    for (halo, resident), (y, st, dx, dy) in zip(((True, True), (True, False), (False, False)), outs):
+        what = "conv3x3 halo=%s resident=%s" % (halo, resident)
+        fb.check_bf16(y, *ref, 9 * cin // groups, what=what)
+        if st is not None:
+            fb.check_sums(st, *fb.stats_ref(y), n * h * w, what=what + " stats")
+        if dx is not None:
+            fb.check_bf16(dx, *fb.dgrad_ref(dy, wt, x.shape), 9 * cout, what=what + " dgrad")
 
 
 def test_conv1x1_fork_sums_both_gradients_in_the_dgrad_epilogue():
@@ -243,38 +235,15 @@ def test_conv1x1_fork_sums_both_gradients_in_the_dgrad_epilogue():
     dy = torch.randn(8, 64, 14, 14, device=DEV).bfloat16().contiguous(memory_format=torch.channels_last)
     y, xa = ops.conv1x1(x, w, None, fork=True)
     torch.autograd.backward([y, xa], [dy, r])
-    xr = x.detach().float().requires_grad_(True)
-    wr = w.detach().float().requires_grad_(True)
-    yr = F.conv2d(xr, wr.view(64, 256, 1, 1))
-    torch.autograd.backward([yr, xr * 1.0], [dy.float(), r.float()])
-    assert _rel(x.grad, xr.grad) < 1e-2
-    assert _rel(w.grad, wr.grad.view_as(w)) < 1e-2
+    wd = w.detach()
+    fb.check_bf16(x.grad, *fb.dgrad_ref(dy, wd, x.shape, padding=0, add=r), 64, what="fork dgrad + addend")
+    fb.check_bf16(w.grad.view(64, 256), *fb.gemm_ref(fb.rows(dy), fb.rows(x.detach()), a_mn_major=True, b_mn_major=True),
+                  8 * 14 * 14, ops.gemm._split_k_for(64, 256, 8 * 14 * 14), what="fork wgrad")
     # alias unused downstream: plain dgrad
     x2 = x.detach().clone().requires_grad_(True)
     y2, _ = ops.conv1x1(x2, w, None, fork=True)
     y2.backward(dy)
-    xr2 = x.detach().float().requires_grad_(True)
-    F.conv2d(xr2, wr.detach().view(64, 256, 1, 1)).backward(dy.float())
-    assert _rel(x2.grad, xr2.grad) < 1e-2
-
-
-def _bn_ref_sums(dy, x, y, mean, rstd, gamma, beta, relu):
-    dyf, xf = dy.float(), x.float()
-    if relu:
-        mask = (y.float() > 0) if y is not None else (torch.addcmul(beta - mean * gamma * rstd, xf, gamma * rstd) > 0)
-        dyf = dyf * mask
-    return torch.cat([dyf.sum(0), (dyf * ((xf - mean) * rstd)).sum(0)])
-
-
-def _hook(x, y, n, relu):
-    from edl_b200.ops.bn import BNBackwardHook
-
-    h = BNBackwardHook()
-    h.x, h.y, h.relu = x, y, relu
-    h.mean, h.rstd = torch.randn(n, device=DEV) * 0.1, torch.rand(n, device=DEV) + 0.5
-    h.gamma, h.beta = torch.rand(n, device=DEV) + 0.5, torch.randn(n, device=DEV) * 0.2
-    h.dsums = torch.zeros(2 * n, device=DEV)
-    return h
+    fb.check_bf16(x2.grad, *fb.dgrad_ref(dy, wd, x.shape, padding=0), 64, what="fork dgrad")
 
 
 @pytest.mark.parametrize("m,k,n", [(2048, 64, 32), (5000, 64, 128), (6272, 512, 256), (300, 64, 1024)])
@@ -286,10 +255,11 @@ def test_dgrad_epilogue_bn_backward_reduction_gemm(m, k, n, relu, has_y):
     w = (torch.randn(k, n, device=DEV) * 0.1).bfloat16()
     x = torch.randn(m, n, device=DEV).bfloat16()
     y = torch.randn(m, n, device=DEV).bfloat16() if has_y else None
-    h = _hook(x, y, n, relu)
+    h = fb.bn_hook(x, y, n, relu)
     d = ops.gemm_bf16(a, w, b_mn_major=True, bn=h)
-    assert h.done and _rel(d, a.float() @ w.float()) < 1e-2
-    assert _rel(h.dsums, _bn_ref_sums(d, x, y, h.mean, h.rstd, h.gamma, h.beta, relu)) < 1e-4
+    assert h.done
+    fb.check_bf16(d, *fb.gemm_ref(a, w, b_mn_major=True), k, what="dgrad")
+    fb.check_dsums(h, d, m, "dgrad dsums")
 
 
 @pytest.mark.parametrize("nb,c,hh,ww", [(8, 64, 16, 16), (32, 256, 14, 14), (5, 64, 11, 20), (8, 256, 2, 2)])
@@ -298,11 +268,11 @@ def test_dgrad_epilogue_bn_backward_reduction_conv3x3(nb, c, hh, ww):
     dy = torch.randn(nb, c, hh, ww, device=DEV).bfloat16().contiguous(memory_format=torch.channels_last)
     wt = (torch.randn(c, 3, 3, c, device=DEV) * 0.05).bfloat16()
     x = torch.randn(nb, c, hh, ww, device=DEV).bfloat16().contiguous(memory_format=torch.channels_last)
-    h = _hook(x, None, c, True)
+    h = fb.bn_hook(x, None, c, True)
     dx = torch.empty_like(x)
     ops.native().conv3x3(dy, wt, dx, True, None, h.as_list(nb * hh * ww, c), True)
-    d2, x2 = dx.permute(0, 2, 3, 1).reshape(-1, c), x.permute(0, 2, 3, 1).reshape(-1, c)
-    assert _rel(h.dsums, _bn_ref_sums(d2, x2, None, h.mean, h.rstd, h.gamma, h.beta, True)) < 1e-4
+    fb.check_bf16(dx, *fb.dgrad_ref(dy, wt, x.shape), 9 * c, what="conv3x3 dgrad")
+    fb.check_dsums(h, dx, nb * hh * ww, "conv3x3 dgrad dsums")
 
 
 @pytest.mark.parametrize("n,c,cout,h,w,groups", [(4, 2048, 2048, 14, 14, 32), (4, 4096, 4096, 7, 7, 32), (2, 256, 256, 12, 12, 4),
@@ -314,9 +284,8 @@ def test_grouped_conv3x3_inference_with_folded_bn_epilogue(n, c, cout, h, w, gro
     scale, shift = torch.rand(cout, device=DEV) + 0.5, torch.randn(cout, device=DEV) * 0.1
     assert ops.conv3x3_infer_supported(x, wt, groups)
     y = ops.conv3x3_infer(x, wt, scale, shift, True, groups)
-    ref = F.conv2d(x.float(), wt.permute(0, 3, 1, 2).float(), None, 1, 1, 1, groups)
-    ref = torch.relu(ref * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
-    assert _rel(y, ref) < 1e-2
+    ref = fb.conv_ref(x, wt, groups=groups, scale=scale.view(1, -1, 1, 1), shift=shift.view(1, -1, 1, 1), relu=True)
+    fb.check_bf16(y, *ref, 9 * c // groups, what="grouped conv3x3 infer")
 
 
 def test_phase_trace_of_the_persistent_kernel():
@@ -353,7 +322,6 @@ def test_stem7_im2col_gemm_matches_the_convolution(n, h, w, cout):
     sc, sh = torch.rand(cout, device=DEV) + 0.5, torch.randn(cout, device=DEV) * 0.1
     assert ops.stem7_supported(x, wt)
     y = ops.stem7_infer(x, wt, sc, sh, relu=True)
-    ref = F.conv2d(x.float(), wt.permute(0, 3, 1, 2).float(), None, 2, 3)
-    ref = torch.relu(ref * sc.view(1, -1, 1, 1) + sh.view(1, -1, 1, 1))
-    assert y.shape == ref.shape and y.is_contiguous(memory_format=torch.channels_last)
-    assert _rel(y, ref) < 1e-2
+    ref = fb.conv_ref(x, wt, 2, 3, scale=sc.view(1, -1, 1, 1), shift=sh.view(1, -1, 1, 1), relu=True)
+    assert y.shape == ref[0].shape and y.is_contiguous(memory_format=torch.channels_last)
+    fb.check_bf16(y, *ref, 160, what="stem7 infer")

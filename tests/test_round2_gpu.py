@@ -5,8 +5,8 @@ import os
 
 import pytest
 import torch
-import torch.nn.functional as F
 
+import f64_bounds as fb
 from edl_b200 import ops
 
 pytestmark = [pytest.mark.gpu]
@@ -15,6 +15,10 @@ DEV = "cuda"
 
 def _rel(a, b):
     return ((a.float() - b.float()).norm() / (b.float().norm() + 1e-12)).item()
+
+
+# the stem weight gradient (csrc/stem.cu) sums one fp32 partial per CTA: at most one CTA per SM
+STEM_WGRAD_SPLIT = 132
 
 
 WGRAD_SHAPES = [  # n, cin, cout, h, w      (ResNet50_vd stages first, then odd geometries)
@@ -31,17 +35,16 @@ def test_conv3x3_wgrad_repeatable(n, cin, cout, h, w, split):
     wt = torch.zeros(cout, 3, 3, cin, device=DEV, dtype=torch.bfloat16)
     if not ops.conv3x3_wgrad_supported(x, wt):
         pytest.skip("geometry not supported by the pixel-box planner")
-    xr = x.float()
-    wr = torch.zeros(cout, cin, 3, 3, device=DEV, requires_grad=True)
-    F.conv2d(xr, wr, None, 1, 1).backward(dy.float())
-    ref = wr.grad.permute(0, 2, 3, 1)                       # KRSC
+    k, sp = n * h * w, split if split is not None else ops.gemm.conv3x3_wgrad_split(n, h, w, cin, cout)
     got = ops.conv3x3_wgrad(x, dy, wt.shape, None, split_k=split)
-    assert got.shape == ref.shape
-    assert _rel(got, ref) < 1e-2, (split, _rel(got, ref))
+    assert got.shape == wt.shape
+    fb.check_bf16(got.view(cout, -1), *[t.reshape(cout, -1) for t in fb.wgrad_ref(x, dy, wt.shape)], k, sp,
+                  what="conv3x3 wgrad")
     # accumulate into a sink (the flat gradient bucket): sink += dW, twice
     sink = torch.full((cout * 9 * cin,), 0.25, device=DEV, dtype=torch.bfloat16)
+    want = fb.wgrad_ref(x, dy, wt.shape, sink=sink.clone())
     assert ops.conv3x3_wgrad(x, dy, wt.shape, sink, split_k=split) is None
-    assert _rel(sink.view(ref.shape), ref + 0.25) < 1e-2
+    fb.check_bf16(sink.view(cout, -1), *[t.reshape(cout, -1) for t in want], k, sp, what="conv3x3 wgrad sink")
     # a second identical call gives the same bits, with and without a sink: no state carries over between calls
     assert torch.equal(ops.conv3x3_wgrad(x, dy, wt.shape, None, split_k=split), got)
     sink2 = torch.full_like(sink, 0.25)
@@ -59,11 +62,10 @@ def test_conv3x3_autograd_with_own_wgrad(monkeypatch):
     y = ops.conv3x3(x, wt)
     dy = torch.randn_like(y)
     y.backward(dy)
-    xr = x.detach().float().requires_grad_(True)
-    wr = wt.detach().float().requires_grad_(True)
-    F.conv2d(xr, wr.permute(0, 3, 1, 2), None, 1, 1).backward(dy.float())
-    assert _rel(x.grad, xr.grad) < 1e-2
-    assert _rel(wt.grad, wr.grad) < 1e-2
+    xd, wd = x.detach(), wt.detach()
+    fb.check_bf16(x.grad, *fb.dgrad_ref(dy, wd, x.shape), 9 * 128, what="conv3x3 dgrad")
+    fb.check_bf16(wt.grad.view(128, -1), *[t.reshape(128, -1) for t in fb.wgrad_ref(xd, dy, wd.shape)], 4 * 28 * 28,
+                  ops.gemm.conv3x3_wgrad_split(4, 28, 28, 64, 128), what="conv3x3 own wgrad")
 
 
 def _chain(x, w1, w3, bn1, bn2, reps):
@@ -223,10 +225,18 @@ def test_teacher_residual_fused_into_the_gemm_epilogue(monkeypatch):
     ops.reset_launches()
     one = conv(x, residual=res)
     assert ops.launches() == 1
-    w = conv.weight.view(512, 256).float()
-    ref = torch.relu(torch.einsum("nchw,oc->nohw", x.float(), w) * conv.scale[None, :, None, None]
-                     + conv.shift[None, :, None, None] + res.float())
-    assert _rel(two, ref) < 1e-2 and _rel(one, ref) < 1e-2, (_rel(two, ref), _rel(one, ref))
+    # the fused launch folds the scale into the weights: relu(x @ (w * scale) + shift + res), where w * scale is the bf16
+    # weight the kernel reads; the two-kernel path applies scale and shift to the GEMM output, then adds the residual
+    sc, sh = conv.scale.view(1, -1, 1, 1), conv.shift.view(1, -1, 1, 1)
+    w = conv.weight.view(512, 1, 1, 256)
+    fb.check_bf16(one, *fb.conv_ref(x, (w.float() * conv.scale.view(-1, 1, 1, 1)).bfloat16(), padding=0, add=res,
+                                     shift=sh, relu=True), 256, what="teacher fused residual")
+    # two kernels: the GEMM's bf16 output, then relu(y * scale + shift + residual) in fp32 on that output
+    y1 = ops.gemm_bf16(fb.rows(x), w.view(512, 256))
+    fb.check_bf16(y1, *fb.gemm_ref(fb.rows(x), w.view(512, 256)), 256, what="teacher gemm")
+    y1 = y1.view(8, 14, 14, 512).permute(0, 3, 1, 2).double()
+    two_ref = (torch.relu(y1 * sc + sh + res.double()), y1.abs() * sc.abs() + sh.abs() + res.double().abs())
+    fb.check_bf16(two, *two_ref, 1, what="teacher scale_shift_act")
     # whole teacher: same logits either way
     m = resnext.to_inference_dtype(resnext.ResNeXt_tiny(), torch.bfloat16, DEV).eval()
     xi = torch.randn(4, 3, 64, 64, device=DEV).bfloat16().contiguous(memory_format=torch.channels_last)
@@ -305,12 +315,13 @@ def test_conv3x3_stride2_fprop(n, cin, cout, h, w, groups):
     wt = (torch.randn(cout, 3, 3, cin // groups, device=DEV) * 0.05).bfloat16()
     if not ops.conv3x3_s2_supported(x, wt, groups):
         pytest.skip("shape not supported")
-    ref = F.conv2d(x.float(), wt.permute(0, 3, 1, 2).float(), None, 2, 1, 1, groups)
+    ref = fb.conv_ref(x, wt, 2, 1, groups)
     scale = torch.rand(cout, device=DEV) + 0.5
     shift = torch.randn(cout, device=DEV) * 0.1
     y = ops.conv3x3_s2_infer(x, wt, scale, shift, True, groups)
-    want = torch.relu(ref * scale[None, :, None, None] + shift[None, :, None, None])
-    assert y.shape == want.shape and _rel(y, want) < 1e-2
+    want = fb.conv_ref(x, wt, 2, 1, groups, scale=scale.view(1, -1, 1, 1), shift=shift.view(1, -1, 1, 1), relu=True)
+    assert y.shape == want[0].shape
+    fb.check_bf16(y, *want, 9 * cin // groups, what="conv3x3 s2 infer")
     if groups == 1:
         from edl_b200.ops import gemm as G
 
@@ -323,16 +334,17 @@ def test_conv3x3_stride2_fprop(n, cin, cout, h, w, groups):
                 xg = x.clone().requires_grad_(True)
                 wg = wt.clone().requires_grad_(True)
                 yt = ops.conv3x3_s2(xg, wg, stats)
-                assert _rel(yt, ref) < 1e-2
-                assert _rel(stats[:cout], yt.float().sum((0, 2, 3))) < 2e-3
+                fb.check_bf16(yt, *ref, 9 * cin, what="conv3x3 s2")
+                fb.check_sums(stats, *fb.stats_ref(yt), yt.numel() // cout, what="conv3x3 s2 stats")
                 dy = torch.randn_like(yt)
                 ops.reset_fallbacks()
                 yt.backward(dy)
                 assert bool(ops.fallbacks()) != own or not (G._s2_dgrad_supported(x, wt) and G._s2_wgrad_supported(x, wt))
-                xr = x.float().requires_grad_(True)
-                wr = wt.float().requires_grad_(True)
-                F.conv2d(xr, wr.permute(0, 3, 1, 2), None, 2, 1).backward(dy.float())
-                assert _rel(xg.grad, xr.grad) < 1e-2 and _rel(wg.grad, wr.grad) < 1e-2, own
+                # own kernels or the library's: both pass the oracle (k of the weight gradient = output pixels,
+                # split up to one per SM)
+                fb.check_bf16(xg.grad, *fb.dgrad_ref(dy, wt, x.shape, 2), 9 * cout, what="conv3x3 s2 dgrad own=%s" % own)
+                fb.check_bf16(wg.grad.view(cout, -1), *[t.reshape(cout, -1) for t in fb.wgrad_ref(x, dy, wt.shape, 2)],
+                              dy.numel() // cout, 132, what="conv3x3 s2 wgrad own=%s" % own)
             finally:
                 G.OWN_S2_BWD = prev
 
@@ -342,32 +354,29 @@ def test_conv3x3_stride2_fprop(n, cin, cout, h, w, groups):
 def test_bnr_mode2_gemm(m, k, n, relu, has_y):
     """Fused BatchNorm-backward reduction, column loop over the staged tiles: same contract as
     tests/test_persist_gpu.py, 1x1 dgrad epilogue."""
-    from test_persist_gpu import _bn_ref_sums, _hook
-
     torch.manual_seed(5)
     a = torch.randn(m, k, device=DEV).bfloat16()
     w = (torch.randn(k, n, device=DEV) * 0.1).bfloat16()
     x = torch.randn(m, n, device=DEV).bfloat16()
     y = torch.randn(m, n, device=DEV).bfloat16() if has_y else None
-    h = _hook(x, y, n, relu)
+    h = fb.bn_hook(x, y, n, relu)
     d = ops.gemm_bf16(a, w, b_mn_major=True, bn=h)
-    assert h.done and _rel(d, a.float() @ w.float()) < 1e-2
-    assert _rel(h.dsums, _bn_ref_sums(d, x, y, h.mean, h.rstd, h.gamma, h.beta, relu)) < 1e-4
+    assert h.done
+    fb.check_bf16(d, *fb.gemm_ref(a, w, b_mn_major=True), k, what="dgrad")
+    fb.check_dsums(h, d, m, "dgrad dsums")
 
 
 @pytest.mark.parametrize("nb,c,hh,ww", [(8, 64, 16, 16), (32, 256, 14, 14), (5, 64, 11, 20), (8, 256, 2, 2), (32, 64, 56, 56)])
 def test_bnr_mode2_conv3x3(nb, c, hh, ww):
-    from test_persist_gpu import _bn_ref_sums, _hook
-
     torch.manual_seed(6)
     dy = torch.randn(nb, c, hh, ww, device=DEV).bfloat16().contiguous(memory_format=torch.channels_last)
     wt = (torch.randn(c, 3, 3, c, device=DEV) * 0.05).bfloat16()
     x = torch.randn(nb, c, hh, ww, device=DEV).bfloat16().contiguous(memory_format=torch.channels_last)
-    h = _hook(x, None, c, True)
+    h = fb.bn_hook(x, None, c, True)
     dx = torch.empty_like(x)
     ops.native().conv3x3(dy, wt, dx, True, None, h.as_list(nb * hh * ww, c), True)
-    d2, x2 = dx.permute(0, 2, 3, 1).reshape(-1, c), x.permute(0, 2, 3, 1).reshape(-1, c)
-    assert _rel(h.dsums, _bn_ref_sums(d2, x2, None, h.mean, h.rstd, h.gamma, h.beta, True)) < 1e-4
+    fb.check_bf16(dx, *fb.dgrad_ref(dy, wt, x.shape), 9 * c, what="conv3x3 dgrad")
+    fb.check_dsums(h, dx, nb * hh * ww, "conv3x3 dgrad dsums")
 
 
 @pytest.mark.parametrize("mode", [2])       # the only reduction mode; the parameter keeps the test ids stable
@@ -380,8 +389,6 @@ def test_bnr_many_tiles_per_cta_and_addend(mode, m, k, n, with_add):
     """What the round-1 kernel tests did not cover and the model needs: several tiles per persistent CTA (x / y prefetch,
     barrier parities, constant reloads when the N tile changes) and the residual-gradient addend together with the
     BatchNorm reduction (every block's first 1x1 convolution)."""
-    from test_persist_gpu import _bn_ref_sums, _hook
-
     assert ops.native().get_bnr_mode() == mode
     torch.manual_seed(7)
     a = torch.randn(m, k, device=DEV).bfloat16()
@@ -389,11 +396,11 @@ def test_bnr_many_tiles_per_cta_and_addend(mode, m, k, n, with_add):
     x = torch.randn(m, n, device=DEV).bfloat16()
     y = torch.randn(m, n, device=DEV).bfloat16()
     add = torch.randn(m, n, device=DEV).bfloat16() if with_add else None
-    h = _hook(x, y, n, True)
+    h = fb.bn_hook(x, y, n, True)
     d = ops.gemm_bf16(a, w, b_mn_major=True, bn=h, add=add)
-    ref = a.float() @ w.float() + (add.float() if with_add else 0.0)
-    assert h.done and _rel(d, ref) < 1e-2
-    assert _rel(h.dsums, _bn_ref_sums(d, x, y, h.mean, h.rstd, h.gamma, h.beta, True)) < 1e-4
+    assert h.done
+    fb.check_bf16(d, *fb.gemm_ref(a, w, b_mn_major=True, add=add), k, what="dgrad")
+    fb.check_dsums(h, d, m, "dgrad dsums")
 
 
 @pytest.mark.parametrize("mode,batch", [pytest.param(2, 8, id="2"), pytest.param(2, 5, id="2-batch5")])
@@ -440,16 +447,14 @@ def test_stem_conv_direct_kernel(n, h, w):
     wt = (torch.randn(32, 3, 3, 3, device=DEV) * 0.2).bfloat16().requires_grad_(True)
     stats = torch.zeros(64, device=DEV)
     y = ops.stem_conv(x, wt, stats)
-    ref = F.conv2d(x.float(), wt.detach().permute(0, 3, 1, 2).float(), None, 2, 1)
-    assert y.shape == ref.shape and y.is_contiguous(memory_format=torch.channels_last)
-    assert _rel(y, ref) < 1e-2
-    yf = y.float()
-    assert _rel(stats[:32], yf.sum((0, 2, 3))) < 2e-3 and _rel(stats[32:], (yf * yf).sum((0, 2, 3))) < 2e-3
+    ref = fb.conv_ref(x, wt.detach(), 2, 1)
+    assert y.shape == ref[0].shape and y.is_contiguous(memory_format=torch.channels_last)
+    fb.check_bf16(y, *ref, 27, what="stem conv")
+    fb.check_sums(stats, *fb.stats_ref(y), y.numel() // 32, what="stem conv stats")
     dy = torch.randn_like(y)
     y.backward(dy)
-    wr = wt.detach().float().requires_grad_(True)
-    F.conv2d(x.float(), wr.permute(0, 3, 1, 2), None, 2, 1).backward(dy.float())
-    assert _rel(wt.grad, wr.grad) < 1e-2
+    fb.check_bf16(wt.grad.view(32, -1), *[t.reshape(32, -1) for t in fb.wgrad_ref(x, dy, wt.shape, 2)],
+                  dy.numel() // 32, STEM_WGRAD_SPLIT, what="stem wgrad")
 
 
 # ------------------------------------------------------------------ DALI-style input path (nvJPEG + fused augmentation)
@@ -540,15 +545,16 @@ def test_32_channel_conv_in_pixel_pair_form(monkeypatch, n, cout, h, w):
     stats = torch.zeros(2 * cout, device=DEV)
     ops.reset_fallbacks()
     y = ops.conv3x3_pair(x, wt, stats)
-    xr = x.detach().float().requires_grad_(True)
-    wr = wt.detach().float().requires_grad_(True)
-    ref = F.conv2d(xr, wr.permute(0, 3, 1, 2), None, 1, 1)
-    assert y.shape == ref.shape and y.is_contiguous(memory_format=torch.channels_last)
-    assert _rel(y, ref) < 1e-2
-    yf = y.float()
-    assert _rel(stats[:cout], yf.sum((0, 2, 3))) < 2e-3 and _rel(stats[cout:], (yf * yf).sum((0, 2, 3))) < 2e-3
+    xd, wd = x.detach(), wt.detach()
+    ref = fb.conv_ref(xd, wd)
+    assert y.shape == ref[0].shape and y.is_contiguous(memory_format=torch.channels_last)
+    fb.check_bf16(y, *ref, 9 * 64, what="pair conv")
+    # the pair-form statistics are folded from 2 Cout channels: one more addition per channel
+    fb.check_sums(stats, *fb.stats_ref(y), y.numel() // cout, what="pair conv stats")
     dy = torch.randn_like(y)
     y.backward(dy)
-    ref.backward(dy.float())
-    assert _rel(x.grad, xr.grad) < 1e-2 and _rel(wt.grad, wr.grad) < 1e-2
+    fb.check_bf16(x.grad, *fb.dgrad_ref(dy, wd, x.shape), 9 * 2 * cout, what="pair dgrad")
+    # pixel-pair weight gradient, then two of its bf16 taps folded into each of ours
+    fb.check_pair_wgrad(wt.grad, xd, dy, wd.shape, n * h * w // 2,
+                        ops.gemm.conv3x3_wgrad_split(n, h, w // 2, 64, 2 * cout) + 1)
     assert not ops.fallbacks(), ops.fallbacks()

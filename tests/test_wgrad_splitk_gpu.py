@@ -3,8 +3,8 @@ by one reduce kernel in a fixed order, so repeated calls give the same bits; the
 that do not fit it; a split without (enough) partial tiles is an error, never a different path."""
 import pytest
 import torch
-import torch.nn.functional as F
 
+import f64_bounds as fb
 from edl_b200 import ops
 from edl_b200.ops import gemm as G
 
@@ -12,8 +12,8 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda"
 
 
-def _rel(a, b):
-    return ((a.float() - b.float()).norm() / (b.float().norm() + 1e-12)).item()
+def _wref(x, dy, shape, stride=1):
+    return [t.reshape(shape[0], -1) for t in fb.wgrad_ref(x, dy, shape, stride)]
 
 
 def _nhwc(*shape, scale=1.0):
@@ -32,7 +32,10 @@ def test_wgrad1x1_splitk_bitwise_reproducible():
     for s in sinks:
         G._wgrad_impl(a, b, (m, n), s, split_k=split)
     assert torch.equal(sinks[0], sinks[1])
-    assert _rel(d1, a.float().t() @ b.float()) < 5e-3
+    fb.check_bf16(d1, *fb.gemm_ref(a, b, a_mn_major=True, b_mn_major=True), k, split, what="wgrad gemm")
+    fb.check_bf16(sinks[0].view(m, n), *fb.gemm_ref(a, b, a_mn_major=True, b_mn_major=True,
+                                                     add=torch.full((m, n), 0.5, device=DEV)), k, split,
+                  what="wgrad gemm sink")
 
 
 def test_wgrad3x3_stride2_bitwise_reproducible():
@@ -47,9 +50,7 @@ def test_wgrad3x3_stride2_bitwise_reproducible():
         d1 = G.conv3x3_wgrad(x, dy, shape, None, split_k=split)
         d2 = G.conv3x3_wgrad(x, dy, shape, None, split_k=split)
         assert torch.equal(d1, d2), split
-        wr = torch.zeros(cout, cin, 3, 3, device=DEV, requires_grad=True)
-        F.conv2d(x.float(), wr, None, 2, 1).backward(dy.float())
-        assert _rel(d1, wr.grad.permute(0, 2, 3, 1)) < 1e-2, split
+        fb.check_bf16(d1.view(cout, -1), *_wref(x, dy, shape, 2), n * ho * wo, split, what="wgrad3x3 s2")
 
 
 def test_wgrad3x3_split_beyond_initial_partials_buffer():
@@ -61,9 +62,7 @@ def test_wgrad3x3_split_beyond_initial_partials_buffer():
     x = _nhwc(n, cin, h, w)
     dy = _nhwc(n, cout, h, w, scale=0.1)
     got = G.conv3x3_wgrad(x, dy, (cout, 3, 3, cin), None, split_k=split)
-    wr = torch.zeros(cout, cin, 3, 3, device=DEV, requires_grad=True)
-    F.conv2d(x.float(), wr, None, 1, 1).backward(dy.float())
-    assert _rel(got, wr.grad.permute(0, 2, 3, 1)) < 1e-2
+    fb.check_bf16(got.view(cout, -1), *_wref(x, dy, (cout, 3, 3, cin)), n * h * w, split, what="wgrad3x3 split 8")
 
 
 def test_split_without_enough_partials_raises():
