@@ -702,6 +702,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("relu"), pybind11::arg("mask") = pybind11::none());
   m.def("bn_relu_mask_supported", &edl::bn_relu_mask_supported,
         "the streaming BN kernels run for [M, C] and can keep the residual ReLU mask as bits");
+  m.def("bn_stream_supported", &edl::bn_stream_supported,
+        "[M, C] has a streaming (cp.async.bulk) BN kernel; it runs unless bn_set_stream_kernels(False)");
   m.def("scale_shift_act", &scale_shift_act);
   m.def("bn_bwd_reduce", &bn_bwd_reduce);
   m.def("bn_bwd_apply", &bn_bwd_apply);

@@ -1,6 +1,6 @@
 """Float64 oracle for the bf16 GEMM and convolution kernels (csrc/gemm.cu, gemm_persist.cu, conv3x3.cu,
-conv3x3_wgrad.cu, stem.cu): element-wise bounds instead of a global relative norm, which hides one wrong row, column,
-tile or tail.
+conv3x3_wgrad.cu, stem.cu) and the BatchNorm and pooling kernels (bn.cu, bn_stream.cu, bn_fused.cu, pool.cu):
+element-wise bounds instead of a global relative norm, which hides one wrong row, column, channel, tile or tail.
 
 Every reference is built in float64 from exactly the bf16 tensors the kernel read: ``ref`` is the value and ``mag`` the
 same operation on absolute values (``sum_k |a_k b_k|``, then the epilogue with ``|add|``, ``|scale|``, ``|shift|`` and
@@ -39,6 +39,19 @@ worst |out - ref| / bound, criterion 2 = worst RMS over tiles and columns / yard
     stem weight gradient                                     c1 1.000   c2 1.00
     pixel-pair weight gradient (two bf16 partials, ``terms``)   c1 0.972   c2 1.00
     statistics and BN-backward sums (check_sums)             c1 0.05
+
+and over tests/test_bn_pool_bounds_gpu.py, test_kernels_gpu.py and test_relu_mask_gpu.py (NVIDIA H100 80GB HBM3,
+700 W power limit; register, streaming and SM-resident BatchNorm kernels alike):
+
+    BatchNorm y, dx from the kernel's statistics (tau)       c1 1.000
+    BatchNorm y, dx end to end (exact statistics)                        c2 1.01
+    ops.batch_norm_act end to end (y, dx, dres)                          c2 1.00
+    BatchNorm sums / dsums (bn_reduce_tau)                   c1 0.13
+    saved mean / running statistics (staged)                 c1 0.50 / 0.28
+    saved mean vs exact statistics (propagated bound)        c1 0.07
+    saved rstd, staged and vs exact                          c1 1.000 (the constant channel: rsqrtf(eps) at the
+                                                             interval's end, since the variance cannot go below 0)
+    scale_shift_act, max-pool dx, average pool, global pool  c1 1.000   c2 1.00
 c1 sits at 1 because a correctly rounded element near a rounding midpoint has an error of half an ulp.
 
 Set ``EDL_F64_BOUNDS_LOG`` to a file name to append one JSON line per check with both ratios."""
@@ -63,6 +76,9 @@ def ulp(x, mant_bits):
 
 def tau(k, split=1):
     return (math.ceil(k / 16) + split + 1) * EPS32
+
+
+_gemm_tau = tau
 
 
 def bf16_round(x64):
@@ -144,14 +160,17 @@ def _tile_sums(x, tile):
     return p.view(tm, tile, tn, tile).sum((1, 3))
 
 
-def _tile_counts(m, n, tile, dev):
-    return _tile_sums(torch.ones(m, n, dtype=torch.float64, device=dev), tile)
-
-
-def check_bf16(out, ref, mag, k, split=1, what="", tile=TILE, c2_factor=C2_FACTOR, terms=None):
+def check_bf16(out, ref, mag, k=0, split=1, what="", tile=TILE, c2_factor=C2_FACTOR, terms=None, tau=None,
+               criteria=(1, 2), columns=None):
     """Criteria 1 and 2 above on a bf16 kernel output against its float64 (ref, mag).  4-D NCHW-shaped tensors are
     checked as [pixels, channels]; KRSC weight gradients are passed as [Cout, 9 Cin].  Returns the worst ratios
     (criterion 1: worst error / bound; criterion 2: worst RMS error / yardstick, failing above ``c2_factor``).
+
+    ``tau``: the per-element slack factor of a non-GEMM operation (a count of fp32 roundings times ``EPS32``) in place
+    of ``tau(k, split)``.  ``criteria``: the criteria that must hold (both by default); an end-to-end reference whose
+    inputs differ from the kernel's by their own rounding bound is judged by criterion 2 alone.  ``columns``: a bool [N]
+    of the columns criterion 2 judges (the others are left out of the tile and column RMS; indices in messages stay
+    those of the full output).
 
     ``terms``: for a path that stores partial results as bf16 and then adds them (the pixel-pair weight gradient), the
     float64 (ref, mag) of each partial, with ``ref`` their sum.  Criterion 1 then also allows each partial its own half
@@ -159,7 +178,8 @@ def check_bf16(out, ref, mag, k, split=1, what="", tile=TILE, c2_factor=C2_FACTO
     ``bf16(sum bf16(term))``."""
     o, r, g = rows(out).double(), rows(ref).double().to(out.device), rows(mag).double().to(out.device)
     assert o.shape == r.shape == g.shape, (what, o.shape, r.shape, g.shape)
-    slack = tau(k, split) * g
+    t_el = _gemm_tau(k, split) if tau is None else tau
+    slack = t_el * g
     bound = 0.5 * ulp(r.abs() + slack, 8) + slack
     yard = bf16_round(r)
     if terms:
@@ -167,26 +187,29 @@ def check_bf16(out, ref, mag, k, split=1, what="", tile=TILE, c2_factor=C2_FACTO
         tm = [rows(t).double().to(out.device) for _, t in terms]
         assert all(t.shape == r.shape for t in tr + tm), what
         for t, tg in zip(tr, tm):
-            bound = bound + 0.5 * ulp(t.abs() + tau(k, split) * tg, 8)
+            bound = bound + 0.5 * ulp(t.abs() + t_el * tg, 8)
         yard = bf16_round(sum(bf16_round(t) for t in tr))
     err = (o - r).abs()
     bad = ~(err <= bound)                                    # NaN fails
     c1 = float((err / bound.clamp_min(1e-300)).nan_to_num(float("inf")).max()) if o.numel() else 0.0
     m, n = o.shape
-    e2 = (o - r).square().nan_to_num(float("inf"))
-    y2 = (yard - r).square()
-    g2 = g.square()
+    judged = (torch.ones(n, dtype=torch.float64, device=o.device) if columns is None
+              else columns.to(o.device, torch.float64)).expand(m, n)
+    e2 = ((o - r).square().nan_to_num(float("inf")) * judged).nan_to_num(0.0, posinf=float("inf"))
+    y2 = (yard - r).square() * judged
+    g2 = g.square() * judged
     msgs = []
     c2 = 0.0
     for name, esum, ysum, gsum, cnt in (
-            ("tile", _tile_sums(e2, tile), _tile_sums(y2, tile), _tile_sums(g2, tile), _tile_counts(m, n, tile, o.device)),
-            ("column", e2.sum(0), y2.sum(0), g2.sum(0), torch.full((n,), float(m), dtype=torch.float64, device=o.device))):
+            ("tile", _tile_sums(e2, tile), _tile_sums(y2, tile), _tile_sums(g2, tile), _tile_sums(judged, tile)),
+            ("column", e2.sum(0), y2.sum(0), g2.sum(0), judged.sum(0))):
+        cnt = cnt.clamp_min(1)                               # a tile or column with nothing judged has 0 / 1
         rms_e, rms_y, rms_g = (esum / cnt).sqrt(), (ysum / cnt).sqrt(), (gsum / cnt).sqrt()
         allowed = c2_factor * rms_y + C2_MAG * rms_g
         ratio = rms_e / (allowed / c2_factor).clamp_min(1e-300)
         c2 = max(c2, float(ratio.max())) if ratio.numel() else c2
         over = ~(rms_e <= allowed)
-        if over.any():
+        if over.any() and 2 in criteria:
             worst = torch.argsort(ratio.flatten(), descending=True)[:4].tolist()
             if name == "tile":
                 desc = ["(%d, %d): %.3g x yardstick" % (i // ratio.shape[1], i % ratio.shape[1], float(ratio.flatten()[i]))
@@ -195,8 +218,10 @@ def check_bf16(out, ref, mag, k, split=1, what="", tile=TILE, c2_factor=C2_FACTO
                 desc = ["%d: %.3g x yardstick" % (i, float(ratio[i])) for i in worst]
             msgs.append("criterion 2: %d of %d %ss over %.2f x the RMS error of correct rounding, worst %s" % (
                 int(over.sum()), over.numel(), name, c2_factor, ", ".join(desc)))
+    c1 = c1 if 1 in criteria else None
+    c2 = c2 if 2 in criteria else None
     _log(what, c1, c2)
-    if bad.any():
+    if bad.any() and c1 is not None:
         excess = torch.where(bad, (err - bound).nan_to_num(float("inf")), torch.zeros_like(err))
         cnt_t = _tile_sums(bad.double(), tile)
         ex_t = F.max_pool2d(F.pad(excess, (0, (-n) % tile, 0, (-m) % tile))[None, None], tile)[0, 0]
@@ -254,6 +279,24 @@ def bn_mask_fp32(x, mean, rstd, gamma, beta):
     pre_fma = x64 * sc.double() + sh_fma.double()
     tol = 4 * EPS32 * ((x64 * sc.double()).abs() + sh_mul.double().abs())
     return pre_mul > 0, ((pre_mul > 0) != (pre_fma > 0)) | (pre_mul.abs() <= tol)
+
+
+def bn_mask_edge(mean, rstd, gamma):
+    """(gamma, beta, residual) that put every x == 0 element on the ReLU's edge, for saved statistics that do not depend
+    on gamma and beta (integer inputs: their fp32 sums are exact, so every path saves the same mean and rstd).  With
+    ``sc = fl(gamma rstd)`` and ``p = mean sc`` (exact in float64), ``beta = fl(p)`` makes the shift ``beta - mean sc``
+    exactly 0 when it is formed as a product and a subtraction, and the product's rounding residual ``fl(p) - p`` when it
+    is formed with one fma.  gamma's sign is chosen per channel so that the residual is positive: an x == 0 element is
+    then masked (pre-activation 0) under one contraction and kept (pre-activation > 0) under the other.  ``residual`` is
+    float64 [C], 0 in a channel whose product is exact."""
+    def prod(g):
+        sc = (g.float() * rstd.float()).double()
+        return mean.double() * sc
+    p = prod(gamma)
+    gamma = torch.where(p.float().double() < p, -gamma, gamma)
+    p = prod(gamma)
+    pf = p.float().double()
+    return gamma, pf.float(), pf - p
 
 
 def bn_dsums_ref(d, x, mean, rstd, gamma, beta, relu, y=None, mask=None):
@@ -319,6 +362,289 @@ def mask_bits(keep):
     m, n = keep.shape
     w = (2 ** torch.arange(8, device=keep.device, dtype=torch.int32))
     return (keep.view(m, n // 8, 8).int() * w).sum(-1).to(torch.uint8)
+
+
+# ---------------------------------------------------------------------------------- BatchNorm and pooling references
+NUM_SMS = 132
+BN_Y_TAU = 4 * EPS32         # y = relu(fmaf(x, g r, b - m g r) + res): g r, m g r, the fma and the residual add
+BN_DX_TAU = 8 * EPS32        # dx = g r (dy - db / M - xhat dg / M): 1/M, two quotients, xhat (2), the product, 2 subtractions
+# criterion 2 end to end needs this many rows per channel: over fewer, the yardstick (the RMS of rounding the exact
+# result to bf16) depends on whether those few values happen to sit near the bf16 grid
+E2E_MIN_ROWS = 64
+
+
+def bn_reduce_plan(path, m, c):
+    """(chain, tree, partials) of the BatchNorm kernels' per-channel fp32 reductions over ``m`` rows: the longest
+    chain of additions one thread makes, the depth of the in-block tree over the threads that share a channel, and the
+    number of per-block partials added by atomics.  ``path``: "regs" (bn.cu, grid of ``bn_grid(M, C, 4 * 132)``),
+    "stream" (bn_stream.cu ``reduce_grid``: 16 KB chunks, two 8-channel vectors per consumer thread and chunk) or
+    "fused" (bn_fused.cu ``plan``)."""
+    cv = c // 8
+    if path == "regs":
+        tx = 1 << (min(cv, 32).bit_length() - 1)
+        ty = 256 // tx
+        gx = -(-cv // tx)
+        gy = max(1, min(4 * NUM_SMS // gx, -(-m // (4 * ty))))
+        return -(-m // (gy * ty)), int(math.log2(ty)), gy
+    n = -(-m * c // 8192)
+    tree = int(math.log2(512 // cv))
+    if path == "stream":
+        grid = max(1, min(-(-n // 4), NUM_SMS))
+        return 2 * -(-n // grid), tree, grid
+    if path == "fused":
+        k = -(-n // min(n, NUM_SMS))
+        return 2 * k, tree, -(-n // k)
+    raise ValueError(path)
+
+
+def bn_reduce_tau(path, m, c):
+    """fp32 rounding bound of those reductions relative to ``sum |terms|``: one rounding per addition on the deepest
+    path, and 3 for the per-term ``xhat`` and fma."""
+    chain, tree, parts = bn_reduce_plan(path, m, c)
+    return (chain + tree + parts + 3) * EPS32
+
+
+def f32(v):
+    """A Python number rounded to fp32, as a float64 scalar (the kernels' ``(float)`` casts)."""
+    return float(torch.tensor(v, dtype=torch.float64).float())
+
+
+def f32_div(a, b):
+    """fp32 ``a / b`` correctly rounded (the kernels' ``1.f / (float)M``)."""
+    return float(torch.tensor([float(a)], dtype=torch.float32) / torch.tensor([float(b)], dtype=torch.float32))
+
+
+def _rstd_interval(var, dvar, eps):
+    """``rsqrtf(var + eps)`` for a variance within ``var +- dvar``: the add rounds once and rsqrtf is within 2 ulp."""
+    lo = torch.rsqrt((var + dvar).clamp_min(0) + eps) * (1 - 3 * EPS32)
+    hi = torch.rsqrt((var - dvar).clamp_min(0) + eps) * (1 + 3 * EPS32)
+    return lo, hi
+
+
+def check_interval(got, lo, hi, what=""):
+    """Per-channel ``lo <= got <= hi``; returns the worst distance from the middle over the half-width."""
+    g, lo, hi = got.double(), lo.double().to(got.device), hi.double().to(got.device)
+    mid, half = (lo + hi) / 2, (hi - lo) / 2
+    ratio = ((g - mid).abs() / half.clamp_min(1e-300)).nan_to_num(float("inf"))
+    c1 = float(ratio.max()) if g.numel() else 0.0
+    _log(what, c1, None)
+    bad = ~((g >= lo) & (g <= hi))
+    if bad.any():
+        idx = torch.argsort(ratio, descending=True)[:4].tolist()
+        raise AssertionError("%s: %d of %d channels out of bounds, worst %s" % (
+            what, int(bad.sum()), bad.numel(), ", ".join("[%d] got %r allowed [%r, %r]" % (
+                i, float(g[i]), float(lo[i]), float(hi[i])) for i in idx)))
+    return c1
+
+
+def check_bn_saved_stats(sums, mean, rstd, m, eps, what="", running=None):
+    """The saved ``mean``/``rstd`` (and, with ``running = (rm0, rv0, rm, rv, momentum)``, the running statistics before
+    and after) against float64 formulas on the kernel's own fp32 ``sums`` [sum, sum of squares]: ``mean = s fl(1/M)``,
+    ``var = max(q fl(1/M) - mean^2, 0)`` with the saved mean (within 2 ulps of ``q/M + mean^2``),
+    ``rstd = rsqrt(var + eps)``, running statistics updated with the unbiased ``var M / (M - 1)``.  A wrong formula
+    (biased running variance, eps outside the square root, momentum on the wrong side) fails."""
+    c = mean.numel()
+    inv = f32_div(1, m)
+    s, q = sums[:c].double(), sums[c:].double()
+    mref = s * inv
+    check_interval(mean, mref - EPS32 * mref.abs(), mref + EPS32 * mref.abs(), what=what + " mean")
+    m64 = mean.double()
+    var = q * inv - m64 * m64
+    dvar = 2 * EPS32 * (q * inv + m64 * m64)
+    lo, hi = _rstd_interval(var, dvar, f32(eps))
+    check_interval(rstd, lo, hi, what=what + " rstd")
+    if running is not None:
+        rm0, rv0, rm, rv, momentum = running
+        mom = f32(momentum)
+        one_m = f32(1.0 - mom)
+        ratio = f32_div(m, m - 1) if m > 1 else 1.0
+        a, b = one_m * rm0.double(), mom * m64
+        ref, slack = a + b, 3 * EPS32 * (a.abs() + b.abs())
+        check_interval(rm, ref - slack, ref + slack, what=what + " running mean")
+        a, b = one_m * rv0.double(), mom * ratio * var.clamp_min(0)
+        ref, slack = a + b, 3 * EPS32 * (a.abs() + b.abs()) + mom * ratio * dvar
+        check_interval(rv, ref - slack, ref + slack, what=what + " running var")
+
+
+def bn_exact_stats(x):
+    """Exact float64 batch statistics of a bf16 [M, C] (or NCHW-shaped) input: (mean, var, mean |x|, mean x^2)."""
+    x64 = rows(x).double()
+    mean = x64.mean(0)
+    return mean, (x64 - mean).square().mean(0), x64.abs().mean(0), x64.square().mean(0)
+
+
+def check_bn_stats_e2e(x, mean, rstd, eps, tau_s, what=""):
+    """The saved statistics against the exact statistics of ``x``, through the bound propagated from the reduction's
+    ``tau_s`` (``bn_reduce_tau``):  d_mean <= tau_s mean|x| + u |mean|,
+    d_var <= tau_s mean(x^2) + 2 |mean| d_mean + d_mean^2 + 3 u (mean(x^2) + mean^2),  rstd = rsqrt(var + eps) within
+    the resulting interval (``1/2 d_var / (var + eps) + 2 u`` to first order).  The fp32 ``sum x^2 / M - mean^2`` loses
+    accuracy as |mean| / std grows, and so does this bound.  Returns the ratios (mean, rstd)."""
+    mu, var, a, q = bn_exact_stats(x)
+    dmu = tau_s * a + EPS32 * mu.abs()
+    dvar = tau_s * q + 2 * mu.abs() * dmu + dmu * dmu + 3 * EPS32 * (q + mu * mu)
+    r1 = check_interval(mean, mu - dmu, mu + dmu, what=what + " mean vs exact")
+    lo, hi = _rstd_interval(var, dvar, f32(eps))
+    r2 = check_interval(rstd, lo, hi, what=what + " rstd vs exact")
+    return r1, r2
+
+
+def bn_y_ref(x, mean, rstd, gamma, beta, res=None, relu=False):
+    """(ref, mag) of the BatchNorm apply from the saved statistics: ``relu(x g r + (b - m g r) + res)``; tau
+    ``BN_Y_TAU``."""
+    x64, m64 = rows(x).double(), mean.double()
+    sc = gamma.double() * rstd.double()
+    a, ms = x64 * sc, m64 * sc
+    ref = a + (beta.double() - ms)
+    mag = a.abs() + beta.double().abs() + ms.abs()
+    if res is not None:
+        ref, mag = ref + rows(res).double(), mag + rows(res).double().abs()
+    return (ref.relu() if relu else ref), mag
+
+
+def scale_shift_ref(x, scale, shift, res=None, relu=False):
+    """(ref, mag) of ``scale_shift_act``: one fmaf, then the residual add (tau 2 EPS32)."""
+    a = rows(x).double() * scale.double()
+    ref, mag = a + shift.double(), a.abs() + shift.double().abs()
+    if res is not None:
+        ref, mag = ref + rows(res).double(), mag + rows(res).double().abs()
+    return (ref.relu() if relu else ref), mag
+
+
+def bn_dx_ref(d, x, mean, rstd, gamma, dsums, m, keep=None, dsums_err=None):
+    """(ref, mag) of the BatchNorm input gradient from the kernel's own ``dsums``:
+    ``g r (dy_m - db / M - xhat dg / M)`` with ``dy_m = d * keep`` (the ReLU mask of the STORED output; None: no ReLU or
+    a gradient stored already masked); tau ``BN_DX_TAU``.  ``dsums_err``: when ``dsums`` is the float64 reference
+    rather than the kernel's (which a caller cannot read), its error bound ``tau_s * mag`` from ``bn_dsums_ref``; the
+    effect on dx, ``|g r| (e_db + |xhat| e_dg) / M``, is added to ``mag`` in units of ``BN_DX_TAU``."""
+    c = mean.numel()
+    g = rows(d).double()
+    if keep is not None:
+        g = g * keep
+    xhat = (rows(x).double() - mean.double()) * rstd.double()
+    k1, k2 = dsums[:c].double() / m, dsums[c:].double() / m
+    sc = gamma.double() * rstd.double()
+    mag = sc.abs() * (g.abs() + k1.abs() + (xhat * k2).abs())
+    if dsums_err is not None:
+        e = dsums_err.double().to(mag.device)
+        mag = mag + sc.abs() * (e[:c] + xhat.abs() * e[c:]) / m / BN_DX_TAU
+    return sc * (g - k1 - xhat * k2), mag
+
+
+def bn_exact(x, gamma, beta, eps, res=None, relu=False, y=None, dy=None):
+    """End-to-end float64 BatchNorm (+ residual) (+ ReLU) of the bf16 inputs with their exact batch statistics: a dict
+    of (ref, mag) pairs ``y``, and with ``dy`` also ``dx``, ``dres``, ``dgamma``, ``dbeta``.  The ReLU mask of the
+    backward is that of the STORED output ``y`` (the kernels' rule).  Equal to float64 ``F.batch_norm`` and its
+    autograd (tests/test_bn_pool_bounds_cpu.py)."""
+    x64 = rows(x).double()
+    m = x64.shape[0]
+    mu, var, _, _ = bn_exact_stats(x)
+    rstd = torch.rsqrt(var + f32(eps))
+    xhat = (x64 - mu) * rstd
+    g64, b64 = gamma.double(), beta.double()
+    yref = xhat * g64 + b64 + (rows(res).double() if res is not None else 0)
+    out = {"y": (yref.relu() if relu else yref, bn_y_ref(x, mu, rstd, gamma, beta, res)[1])}
+    if dy is not None:
+        gm = rows(dy).double()
+        if relu:
+            gm = gm * (rows(y).double() > 0)
+        db, dg = gm.sum(0), (gm * xhat).sum(0)
+        sc = g64 * rstd
+        out["dx"] = (sc * (gm - db / m - xhat * dg / m),
+                     sc.abs() * (gm.abs() + (db / m).abs() + (xhat * dg / m).abs()))
+        out["dres"] = (gm, gm.abs())
+        out["dgamma"], out["dbeta"] = (dg, (gm * xhat).abs().sum(0)), (db, gm.abs().sum(0))
+    return out
+
+
+def maxpool_ref(x):
+    """float64 3x3 / stride 2 / pad 1 max pool of the bf16 NCHW ``x`` and the flat (h W + w) index of the maximum.
+    Torch takes the first maximum in (kh, kw) scan order and pads with -inf, which is the kernel's rule.  (NaN is out of
+    scope: the kernel's ``>`` drops it, torch propagates it.)"""
+    return F.max_pool2d(x.double(), 3, 2, 1, return_indices=True)
+
+
+def check_exact(got, want, what=""):
+    """Exact equality (outputs that involve no rounding: masked gradients, mask bits, parameter-gradient sinks, max-pool
+    values and slots; +0 and -0 are equal, NaN is not); the message names the first differing element."""
+    g, w = got.reshape(-1), want.to(got.device, got.dtype).reshape(-1)
+    bad = g != w
+    if bad.any():
+        i = int(bad.nonzero()[0])
+        raise AssertionError("%s: %d of %d elements differ, first at flat index %d (%s): got %r, want %r" % (
+            what, int(bad.sum()), bad.numel(), i, [int(t) for t in torch.unravel_index(torch.tensor(i), got.shape)],
+            g[i].item(), w[i].item()))
+
+
+def check_maxpool(y, slots, x, what=""):
+    """Max-pool output [N, C, Ho, Wo] and the kernel's arg-max slots against ``maxpool_ref``: both exact.  Returns the
+    flat indices of the maxima for the backward reference."""
+    ref, idx = maxpool_ref(x)
+    check_exact(y.double(), ref.to(y.device), what=what + " y")
+    check_exact(slots.long(), maxpool_slots(idx, x.shape[3]).to(slots.device), what=what + " arg-max slot")
+    return idx
+
+
+def maxpool_slots(idx, w):
+    """The kernel's window slot ``kh * 3 + kw`` of each flat maximum index [N, C, Ho, Wo]."""
+    ho, wo = idx.shape[2], idx.shape[3]
+    oh = torch.arange(ho, device=idx.device).view(1, 1, ho, 1)
+    ow = torch.arange(wo, device=idx.device).view(1, 1, 1, wo)
+    return (idx // w - (2 * oh - 1)) * 3 + (idx % w - (2 * ow - 1))
+
+
+def maxpool_bwd_ref(dy, idx, x_shape):
+    """(ref, mag) of the max-pool input gradient: ``dy`` routed to the maxima in float64.  A pixel is in at most 4
+    windows: tau 3 EPS32."""
+    n, c, h, w = x_shape
+    flat = idx.reshape(n, c, -1)
+    d64 = dy.double().reshape(n, c, -1)
+    ref = torch.zeros(n, c, h * w, dtype=torch.float64, device=dy.device).scatter_add_(2, flat, d64)
+    mag = torch.zeros_like(ref).scatter_add_(2, flat, d64.abs())
+    return ref.view(n, c, h, w), mag.view(n, c, h, w)
+
+
+def avgpool_ref(x):
+    """(ref, mag) of the 2x2 / stride 2 average pool (ceil mode, exclusive): at most 4 terms and a power-of-two scale,
+    tau 3 EPS32."""
+    x64 = x.double()
+    return tuple(F.avg_pool2d(t, 2, 2, 0, ceil_mode=True, count_include_pad=False) for t in (x64, x64.abs()))
+
+
+def avgpool_bwd_ref(dy, x_shape):
+    """(ref, mag) of its input gradient (each pixel in one window; the power-of-two scale is exact: tau EPS32)."""
+    outs = []
+    for d in (dy.double(), dy.double().abs()):
+        z = torch.zeros(x_shape, dtype=torch.float64, device=dy.device, requires_grad=True)
+        F.avg_pool2d(z, 2, 2, 0, ceil_mode=True, count_include_pad=False).backward(d)
+        outs.append(z.grad)
+    return tuple(outs)
+
+
+def gap_tau(hw):
+    """Global average pool forward: a chain of ceil(HW / 8) additions per thread, 8 partials, and ``fl(1 / HW)``
+    (inexact for HW = 49) times the sum."""
+    return (math.ceil(hw / 8) + 8 + 2) * EPS32
+
+
+def gap_ref(x):
+    """(ref, mag) [N, C] of the global average pool of NCHW-shaped ``x`` (tau ``gap_tau(H W)``)."""
+    x64 = x.double()
+    return x64.mean((2, 3)), x64.abs().mean((2, 3))
+
+
+def gap_bwd_ref(dy, x_shape):
+    """(ref, mag) of its input gradient ``dy / HW`` on every pixel: ``fl(1 / HW)`` and the product, tau 2 EPS32."""
+    n, c, h, w = x_shape
+    ref = (dy.double() / (h * w)).view(n, c, 1, 1).expand(n, c, h, w)
+    return ref, ref.abs()
+
+
+def dilate2_ref(x):
+    """Zero insertion: out[:, :, 2 h, 2 w] = x[:, :, h, w], every other element 0 (exact)."""
+    n, c, h, w = x.shape
+    out = torch.zeros(n, c, 2 * h, 2 * w, dtype=x.dtype, device=x.device)
+    out[:, :, ::2, ::2] = x
+    return out
 
 
 # ----------------------------------------------------------------------------------------------- guarded windows

@@ -1,8 +1,10 @@
-"""Numerics of every hand-written sm_90a kernel against a plain PyTorch fp32 reference."""
+"""Numerics of every hand-written sm_90a kernel against a plain PyTorch reference (float64 element-wise bounds of
+tests/f64_bounds.py for BatchNorm and pooling)."""
 import pytest
 import torch
 import torch.nn.functional as F
 
+import f64_bounds as fb
 from edl_b200 import ops
 from edl_b200.ops import bn as bnmod
 
@@ -36,33 +38,46 @@ def test_bn_fwd_bwd(shape, relu, res, path):
 def _bn_fwd_bwd(shape, relu, res):
     torch.manual_seed(0)
     n, c, h, w = shape
+    m = n * h * w
     x = _cl((torch.randn(shape, device=DEV) * 2 + 0.5).bfloat16()).requires_grad_(True)
     r = _cl(torch.randn(shape, device=DEV).bfloat16()).requires_grad_(True) if res else None
     gamma = (torch.rand(c, device=DEV) + 0.5).requires_grad_(True)
     beta = (torch.randn(c, device=DEV) * 0.1).requires_grad_(True)
     rm, rv = torch.zeros(c, device=DEV), torch.ones(c, device=DEV)
     y = ops.batch_norm_act(x, gamma, beta, rm, rv, residual=r, relu=relu, training=True)
+    _, _, _, mean, rstd, _ = y.grad_fn.saved_tensors      # the saved statistics, read before backward frees them
     dy = _cl(torch.randn(shape, device=DEV).bfloat16())
     y.backward(dy)
-    # fp32 reference
-    xr = x.detach().float().requires_grad_(True)
-    rr = r.detach().float().requires_grad_(True) if res else None
-    gr, br = gamma.detach().clone().requires_grad_(True), beta.detach().clone().requires_grad_(True)
-    rm2, rv2 = torch.zeros(c, device=DEV), torch.ones(c, device=DEV)
-    yr = F.batch_norm(xr, rm2, rv2, gr, br, True, 0.1, 1e-5)
+    # float64 BatchNorm with the exact statistics of the bf16 input; the ReLU mask of the stored output, like the kernels
+    ex = fb.bn_exact(x.detach(), gamma.detach(), beta.detach(), 1e-5, r.detach() if res else None, relu,
+                     y=y.detach(), dy=dy)
+    what = "bn %s relu %d res %d" % (shape, relu, res)
+    # the saved statistics: within the bound propagated from the reductions' rounding of any of the three paths
+    tau_s = max(fb.bn_reduce_tau(p, m, c) for p in ("regs", "stream", "fused"))
+    fb.check_bn_stats_e2e(x.detach(), mean, rstd, 1e-5, tau_s, what=what)
+    if m >= fb.E2E_MIN_ROWS:
+        fb.check_bf16(y.detach(), *ex["y"], criteria=(2,), what=what + " y")
+        fb.check_bf16(x.grad, *ex["dx"], criteria=(2,), what=what + " dx")
+    else:
+        # too few rows per channel for criterion 2: criterion 1 from the saved statistics, with the float64 dsums
+        # standing in for the kernel's (their error bound folded into dx's slack)
+        xd, yd = fb.rows(x.detach()), fb.rows(y.detach())
+        keep = yd > 0 if relu else None
+        fb.check_bf16(y.detach(), *fb.bn_y_ref(xd, mean, rstd, gamma.detach(), beta.detach(),
+                                               fb.rows(r.detach()) if res else None, relu),
+                      tau=fb.BN_Y_TAU, criteria=(1,), what=what + " y")
+        ds, ds_mag, _ = fb.bn_dsums_ref(fb.rows(dy), xd, mean, rstd, gamma, beta, relu, y=yd if relu else None)
+        fb.check_bf16(x.grad, *fb.bn_dx_ref(fb.rows(dy), xd, mean, rstd, gamma.detach(), ds, m, keep,
+                                           dsums_err=tau_s * ds_mag), tau=fb.BN_DX_TAU, criteria=(1,), what=what + " dx")
+    for name, got in (("dgamma", gamma.grad), ("dbeta", beta.grad)):
+        # the exact statistics differ from the kernel's by their fp32 rounding, far below 2^-12 of the sum of |terms|
+        fb.check_sums(got, *ex[name], m, tau_s=2 ** -12, what=what + " " + name)
     if res:
-        yr = yr + rr
-    if relu:
-        yr = torch.relu(yr)
-    # use the kernel's own (bf16-rounded) output to build the ReLU mask, like the kernel does
-    yr.backward(dy.float())
-    assert _rel(y, yr) < 1e-2
-    assert _rel(x.grad, xr.grad) < 2e-2
-    assert _rel(gamma.grad, gr.grad) < 2e-2
-    assert _rel(beta.grad, br.grad) < 2e-2
-    if res:
-        assert _rel(r.grad, rr.grad) < 2e-2
-    assert _rel(rm, rm2) < 1e-3 and _rel(rv, rv2) < 1e-3
+        fb.check_exact(r.grad, fb.rows(ex["dres"][0]).reshape(n, h, w, c).permute(0, 3, 1, 2), what=what + " dres")
+    mu, var, _, _ = fb.bn_exact_stats(x.detach())
+    rm_ref, rv_ref = 0.1 * mu, 0.9 + 0.1 * var * (m / (m - 1))
+    fb.check_sums(rm, rm_ref, rm_ref.abs(), m, tau_s=2 ** -12, what=what + " running mean")
+    fb.check_sums(rv, rv_ref, rv_ref.abs(), m, tau_s=2 ** -12, what=what + " running var")
 
 
 def test_bn_sinks_and_eval():
@@ -133,11 +148,9 @@ def test_maxpool(shape):
     y = ops.max_pool_3x3_s2(x)
     dy = _cl(torch.randn_like(y))
     y.backward(dy)
-    xr = x.detach().float().requires_grad_(True)
-    yr = F.max_pool2d(xr, 3, 2, 1)
-    yr.backward(dy.float())
-    assert torch.equal(y.float(), yr)
-    assert _rel(x.grad, xr.grad) < 1e-2
+    ref, idx = fb.maxpool_ref(x.detach())
+    fb.check_exact(y.detach().double(), ref, what="maxpool y")
+    fb.check_bf16(x.grad, *fb.maxpool_bwd_ref(dy, idx, shape), tau=3 * fb.EPS32, what="maxpool dx")
 
 
 @pytest.mark.parametrize("shape", [(2, 256, 56, 56), (2, 64, 7, 9)])
@@ -147,18 +160,14 @@ def test_avgpool_gap(shape):
     y = ops.avg_pool_2x2(x)
     dy = _cl(torch.randn_like(y))
     y.backward(dy)
-    xr = x.detach().float().requires_grad_(True)
-    yr = F.avg_pool2d(xr, 2, 2, 0, ceil_mode=True, count_include_pad=False)
-    yr.backward(dy.float())
-    assert _rel(y, yr) < 1e-2 and _rel(x.grad, xr.grad) < 1e-2
+    fb.check_bf16(y.detach(), *fb.avgpool_ref(x.detach()), tau=3 * fb.EPS32, what="avgpool y")
+    fb.check_bf16(x.grad, *fb.avgpool_bwd_ref(dy, shape), tau=fb.EPS32, what="avgpool dx")
     x2 = _cl(torch.randn(shape, device=DEV).bfloat16()).requires_grad_(True)
     g = ops.global_avg_pool(x2)
     dg = torch.randn_like(g)
     g.backward(dg)
-    x2r = x2.detach().float().requires_grad_(True)
-    gr = x2r.mean((2, 3))
-    gr.backward(dg.float())
-    assert _rel(g, gr) < 1e-2 and _rel(x2.grad, x2r.grad) < 1e-2
+    fb.check_bf16(g.detach(), *fb.gap_ref(x2.detach()), tau=fb.gap_tau(shape[2] * shape[3]), what="gap y")
+    fb.check_bf16(x2.grad, *fb.gap_bwd_ref(dg, shape), tau=2 * fb.EPS32, what="gap dx")
 
 
 def test_fused_sgd_matches_reference():
