@@ -107,6 +107,17 @@ EDL_DEVICE void store_bf16x4(__nv_bfloat16* dst, float4 v, bool accumulate) {
   *reinterpret_cast<uint2*>(dst) = packed;
 }
 
+// The first min(n, 4) elements of v into dst (+= when accumulating) with 2-byte stores: the last columns of a row, or
+// rows that are not 8-byte aligned.
+EDL_DEVICE void store_bf16_tail(__nv_bfloat16* dst, float4 v, int n, bool accumulate) {
+  const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    if (i >= n) break;
+    dst[i] = __float2bfloat16_rn(accumulate ? e[i] + __bfloat162float(dst[i]) : e[i]);
+  }
+}
+
 EDL_DEVICE float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));

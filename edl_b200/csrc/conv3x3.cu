@@ -318,6 +318,7 @@ const char* conv3x3_bf16(const Conv3x3Args& a, cudaStream_t stream) {
   if (!conv3x3_supported(a.N, a.H, a.W, a.Cin, a.Cout, a.dgrad, a.groups)) return "conv3x3: unsupported shape";
   if (!persistent_gemm_enabled() && (a.groups > 1 || a.col_scale != nullptr || a.col_shift != nullptr || a.relu))
     return "conv3x3: groups / inference epilogue need the persistent kernel";
+  if (a.ksize != 3) return "conv3x3: a 1x1 / stride 2 convolution goes through conv1x1_s2_bf16";
   if (a.stride != 1 && (a.stride != 2 || a.dgrad || !persistent_gemm_enabled()))
     return "conv3x3: stride 2 is implemented for fprop on the persistent kernel only";
   if (a.device >= 0) {
@@ -345,6 +346,25 @@ const char* conv3x3_dgrad_s2_bf16(const Conv3x3Args& a, cudaStream_t stream) {
   }
   const Geometry geo = plan(a.N, a.H, a.W);
   return conv3x3_dgrad_s2_persistent(a, geo.BH, geo.BN, geo.tiles_h, geo.tiles_img, stream);
+}
+
+bool conv1x1_s2_supported(int N, int Ho, int Wo, int Cin, int Cout, bool dgrad) {
+  // the strided input map spans 2 Wo columns and 2 BH rows of the input: TMA boxes stop at 256 elements
+  if (!persistent_gemm_enabled() || Wo < 1 || Ho < 1 || 2 * Wo > 256) return false;
+  if (!conv3x3_supported(N, Ho, Wo, Cin, Cout, dgrad, 1)) return false;
+  return 2 * plan(N, Ho, Wo).BH <= 256;
+}
+
+const char* conv1x1_s2_bf16(const Conv3x3Args& a, cudaStream_t stream) {
+  if (a.ksize != 1 || a.stride != 2 || a.groups != 1) return "conv1x1_s2: ksize 1, stride 2, groups 1";
+  if (!conv1x1_s2_supported(a.N, a.H, a.W, a.Cin, a.Cout, a.dgrad)) return "conv1x1_s2: unsupported shape";
+  if (a.device >= 0) {
+    cudaError_t e = cudaSetDevice(a.device);   // tensor-map encoding needs a bound context (see gemm.cu)
+    if (e != cudaSuccess) return cudaGetErrorString(e);
+  }
+  const Geometry geo = plan(a.N, a.H, a.W);
+  if (a.dgrad) return conv1x1_dgrad_s2_persistent(a, geo.BH, geo.BN, geo.tiles_h, geo.tiles_img, stream);
+  return conv3x3_bf16_persistent(a, geo.BH, geo.BN, geo.tiles_h, geo.tiles_img, stream);
 }
 
 }  // namespace edl

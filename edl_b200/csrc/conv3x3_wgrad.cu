@@ -50,12 +50,17 @@ struct WgradParams {
   __nv_bfloat16* out;        // bf16 [Cout][9*Cin] (KRSC)
   int accumulate;
   int stride;                // 1, or 2: X rows 2*h + r - 1 (the columns are subsampled by the tensor map)
-  float* part;               // split-K partial tiles [split][ctas][128 x 192] (gridDim.z > 1)
+  float* part;               // split-K partial tiles [split][ctas][128 x TAPS*64] (gridDim.z > 1)
 };
 
+// TAPS = filter taps per CTA: 3 (one filter row of the 3x3 convolution; out is KRSC [Cout][9*Cin]), or 1 (the 1x1 / pad 0 /
+// stride 2 convolution: X pixel (2h, 2w) only, one accumulator, out is [Cout][Cin]).
+template <int TAPS>
 __global__ void __launch_bounds__(kThreads, 1)
 conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX,
                      const WgradParams p) {
+  static_assert(TAPS == 3 || TAPS == 1, "a filter row of the 3x3, or the 1x1 centre tap");
+  constexpr int kRows = TAPS == 3 ? 3 : 1;      // filter rows, one CTA each
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -64,9 +69,9 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // blockIdx.x = (tile * 3 + r); tile = mt * tiles_n + nt
-  const int r = blockIdx.x % 3;
-  const int tile = blockIdx.x / 3;
+  // blockIdx.x = (tile * kRows + r); tile = mt * tiles_n + nt
+  const int r = blockIdx.x % kRows;
+  const int tile = blockIdx.x / kRows;
   const int m0 = (tile / p.tiles_n) * kBlockM;
   const int n0 = (tile % p.tiles_n) * kBlockN;
   const int kb_begin = blockIdx.z * p.kb_per_split;
@@ -101,12 +106,13 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
         const int h0 = (kb % p.HB) * p.BH;
         const int img0 = (kb / p.HB) * p.NB;
         if (ptx::elect_one()) {
-          ptx::mbar_arrive_expect_tx(&full_bar[st], chunk_tx * (two_chunks ? 5u : 4u));
+          ptx::mbar_arrive_expect_tx(&full_bar[st], chunk_tx * (two_chunks ? 2u + TAPS : 1u + TAPS));
           ptx::tma_load_4d(sa, &tmDy, &full_bar[st], m0, 0, h0, img0);
           if (two_chunks) ptx::tma_load_4d(sa + kChunkBytes, &tmDy, &full_bar[st], m0 + 64, 0, h0, img0);
 #pragma unroll
-          for (int s = 0; s < 3; ++s)
-            ptx::tma_load_4d(sb + s * kChunkBytes, &tmX, &full_bar[st], n0, s - 1, h0 * p.stride + r - 1, img0);
+          for (int s = 0; s < TAPS; ++s)
+            ptx::tma_load_4d(sb + s * kChunkBytes, &tmX, &full_bar[st], n0, TAPS == 3 ? s - 1 : 0,
+                             h0 * p.stride + (TAPS == 3 ? r - 1 : 0), img0);
         }
         __syncwarp();
       }
@@ -116,7 +122,7 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
       const int et = threadIdx.x - 128;
       const int row = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // first accumulator row of this thread (second: + 8)
       const int cq = (lane & 3) * 2;
-      float acc[3][kBlockN / 2];
+      float acc[TAPS][kBlockN / 2];
       using Mma = ptx::WgmmaBf16<kBlockN, 1, 1>;
       const int ksteps = p.KB / kMmaK;
       for (int i = 0; i < num_kb; ++i) {
@@ -131,7 +137,7 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
         ptx::wgmma_fence();
         for (int k = 0; k < ksteps; ++k) {
 #pragma unroll
-          for (int s = 0; s < 3; ++s)
+          for (int s = 0; s < TAPS; ++s)
             Mma::mma(acc[s], da0 + (uint64_t)(k * 128), db0 + (uint64_t)(s * (kChunkBytes >> 4) + k * 128),
                      (i | k) != 0 ? 1u : 0u);
         }
@@ -143,17 +149,17 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
       uint8_t* sf = smem;                        // the ring is drained: fp32 staging tile
       int rows_valid = p.Cout - m0;
       if (rows_valid > kBlockM) rows_valid = kBlockM;
-      const int64_t ldw = (int64_t)9 * p.Cin;
+      const int64_t ldw = (int64_t)(TAPS * TAPS) * p.Cin;
       const bool direct = gridDim.z == 1;
 #pragma unroll
-      for (int s = 0; s < 3; ++s) {
+      for (int s = 0; s < TAPS; ++s) {
 #pragma unroll
         for (int j = 0; j < kBlockN / 8; ++j) {
           *reinterpret_cast<float2*>(sf + row * kPitch + (j * 8 + cq) * 4) = make_float2(acc[s][4 * j], acc[s][4 * j + 1]);
           *reinterpret_cast<float2*>(sf + (row + 8) * kPitch + (j * 8 + cq) * 4) = make_float2(acc[s][4 * j + 2], acc[s][4 * j + 3]);
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");
-        const int64_t col0 = (int64_t)(r * 3 + s) * p.Cin + n0;
+        const int64_t col0 = TAPS == 3 ? (int64_t)(r * 3 + s) * p.Cin + n0 : (int64_t)n0;
 #pragma unroll 1   // one 16-byte piece per iteration, as in version 2 below
         for (int f = et; f < rows_valid * kVecPerRow; f += kEpiThreads) {
           const int rr = f / kVecPerRow, c4 = (f % kVecPerRow) * 4;
@@ -162,8 +168,8 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
             // this CTA saw every pixel: bf16 (+= bucket) straight from the staged tile
             store_bf16x4(p.out + (int64_t)(m0 + rr) * ldw + col0 + c4, t, p.accumulate);
           } else {
-            *reinterpret_cast<float4*>(p.part + ((int64_t)blockIdx.z * gridDim.x + blockIdx.x) * (kBlockM * 3 * kBlockN) +
-                                       rr * (3 * kBlockN) + s * kBlockN + c4) = t;
+            *reinterpret_cast<float4*>(p.part + ((int64_t)blockIdx.z * gridDim.x + blockIdx.x) * (kBlockM * TAPS * kBlockN) +
+                                       rr * (TAPS * kBlockN) + s * kBlockN + c4) = t;
           }
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");   // staging tile is reused by the next tap
@@ -459,39 +465,11 @@ WgradGeometry plan_wgrad(int N, int H, int W) {
   return best;
 }
 
-}  // namespace
-
-bool conv3x3_wgrad_supported(int N, int H, int W, int Cin, int Cout) {
-  if (Cin % 64 != 0 || Cout % 64 != 0) return false;
-  return g_wgrad3_version == 2 ? plan_wgrad2(N, H, W).ok : plan_wgrad(N, H, W).ok;
-}
-
-void set_wgrad3_version(int version, int base_offset_mode) {
-  g_wgrad3_version = version == 1 ? 1 : 2;
-  g_wgrad3_bo = base_offset_mode ? 1 : 0;
-}
-int get_wgrad3_version() { return g_wgrad3_version; }
-
-bool conv3x3_wgrad_s2_supported(int N, int Ho, int Wo, int Cin, int Cout) {
-  if (Cin % 64 != 0 || Cout % 64 != 0 || 2 * Wo > 256) return false;
-  const WgradGeometry g = plan_wgrad(N, Ho, Wo);
-  return g.ok && 2 * g.BH <= 256;
-}
-
-const char* conv3x3_wgrad_bf16(const Conv3x3WgradArgs& a, cudaStream_t stream) {
+// version 1: TAPS filter taps per CTA (3: one row of the 3x3 convolution, 1: the 1x1 / stride-2 centre tap)
+template <int TAPS>
+const char* launch_wgrad1(const Conv3x3WgradArgs& a, cudaStream_t stream) {
+  constexpr int kRows = TAPS == 3 ? 3 : 1;
   const bool s2 = a.stride == 2;
-  if (s2 ? !conv3x3_wgrad_s2_supported(a.N, a.H, a.W, a.Cin, a.Cout)
-         : !conv3x3_wgrad_supported(a.N, a.H, a.W, a.Cin, a.Cout))
-    return "conv3x3_wgrad: unsupported shape";
-  if (a.dW == nullptr) return "conv3x3_wgrad: missing output";
-  if (a.device >= 0) {
-    cudaError_t e = cudaSetDevice(a.device);   // tensor-map encoding needs a bound context (see gemm.cu)
-    if (e != cudaSuccess) return cudaGetErrorString(e);
-  }
-  if (g_wgrad3_version == 2 && !s2) {
-    const Wgrad2Geometry g2 = plan_wgrad2(a.N, a.H, a.W);
-    return a.Cin % 128 == 0 ? launch_wgrad2<128>(a, g2, stream) : launch_wgrad2<64>(a, g2, stream);
-  }
   const WgradGeometry geo = plan_wgrad(a.N, a.H, a.W);
   alignas(64) CUtensorMap tmDy, tmX;
   {
@@ -515,11 +493,12 @@ const char* conv3x3_wgrad_bf16(const Conv3x3WgradArgs& a, cudaStream_t stream) {
     const uint32_t es[4] = {1, 2, 2, 1};
     if (const char* e = encode_tmap_strided(&tmX, a.X, 4, dims, st, box, es, 2)) return e;
   }
+  auto kern = conv3x3_wgrad_kernel<TAPS>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
     if (e != cudaSuccess) return cudaGetErrorString(e);
-    apply_carveout((const void*)conv3x3_wgrad_kernel);
+    apply_carveout((const void*)kern);
     attr_set = true;
   }
   WgradParams p;
@@ -536,18 +515,57 @@ const char* conv3x3_wgrad_bf16(const Conv3x3WgradArgs& a, cudaStream_t stream) {
   p.out = reinterpret_cast<__nv_bfloat16*>(a.dW);
   p.accumulate = a.accumulate ? 1 : 0;
   p.stride = s2 ? 2 : 1;
-  dim3 grid(tiles_m * p.tiles_n * 3, 1, split);
-  if (const char* e = check_partials(a, split, (int64_t)grid.x * kBlockM * 3 * kBlockN)) return e;
+  dim3 grid(tiles_m * p.tiles_n * kRows, 1, split);
+  if (const char* e = check_partials(a, split, (int64_t)grid.x * kBlockM * TAPS * kBlockN)) return e;
   p.part = a.partials;
-  conv3x3_wgrad_kernel<<<grid, kThreads, kSmemTotal, stream>>>(tmDy, tmX, p);
+  kern<<<grid, kThreads, kSmemTotal, stream>>>(tmDy, tmX, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cudaGetErrorString(e);
   if (split > 1) {
-    splitk_reduce(a.partials, split, (int)grid.x, p.tiles_n, kBlockM, 3 * kBlockN, 3, a.Cin, a.Cout, 9 * a.Cin, a.dW,
-                  (int64_t)9 * a.Cin, a.accumulate, stream);
+    const int ld = TAPS * TAPS * a.Cin;
+    splitk_reduce(a.partials, split, (int)grid.x, p.tiles_n, kBlockM, TAPS * kBlockN, TAPS, a.Cin, a.Cout, ld, a.dW,
+                  (int64_t)ld, a.accumulate, stream);
     e = cudaGetLastError();
   }
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
+}  // namespace
+
+bool conv3x3_wgrad_supported(int N, int H, int W, int Cin, int Cout) {
+  if (Cin % 64 != 0 || Cout % 64 != 0) return false;
+  return g_wgrad3_version == 2 ? plan_wgrad2(N, H, W).ok : plan_wgrad(N, H, W).ok;
+}
+
+void set_wgrad3_version(int version, int base_offset_mode) {
+  g_wgrad3_version = version == 1 ? 1 : 2;
+  g_wgrad3_bo = base_offset_mode ? 1 : 0;
+}
+int get_wgrad3_version() { return g_wgrad3_version; }
+
+bool conv3x3_wgrad_s2_supported(int N, int Ho, int Wo, int Cin, int Cout) {
+  if (Cin % 64 != 0 || Cout % 64 != 0 || 2 * Wo > 256) return false;
+  const WgradGeometry g = plan_wgrad(N, Ho, Wo);
+  return g.ok && 2 * g.BH <= 256;
+}
+
+const char* conv3x3_wgrad_bf16(const Conv3x3WgradArgs& a, cudaStream_t stream) {
+  const bool s2 = a.stride == 2;
+  const bool k1 = a.ksize == 1;
+  if (k1 && !s2) return "conv3x3_wgrad: the 1x1 weight gradient here is the stride-2 one";
+  if (s2 ? !conv3x3_wgrad_s2_supported(a.N, a.H, a.W, a.Cin, a.Cout)
+         : !conv3x3_wgrad_supported(a.N, a.H, a.W, a.Cin, a.Cout))
+    return "conv3x3_wgrad: unsupported shape";
+  if (a.dW == nullptr) return "conv3x3_wgrad: missing output";
+  if (a.device >= 0) {
+    cudaError_t e = cudaSetDevice(a.device);   // tensor-map encoding needs a bound context (see gemm.cu)
+    if (e != cudaSuccess) return cudaGetErrorString(e);
+  }
+  if (g_wgrad3_version == 2 && !s2) {
+    const Wgrad2Geometry g2 = plan_wgrad2(a.N, a.H, a.W);
+    return a.Cin % 128 == 0 ? launch_wgrad2<128>(a, g2, stream) : launch_wgrad2<64>(a, g2, stream);
+  }
+  return k1 ? launch_wgrad1<1>(a, stream) : launch_wgrad1<3>(a, stream);
 }
 
 // upper bound over both kernel versions, in CTAs of 64 Cin columns (sizes the partial-tile buffer)

@@ -40,8 +40,9 @@ struct GemmParams {
   const float* col_shift;
   int relu;
   float* col_stats;  // [2N]
-  __nv_bfloat16* out_bf16;   // EPI 1: bf16 [M, N], row pitch ldo (+= when accumulate)
+  __nv_bfloat16* out_bf16;   // EPI 1: bf16 [M, n_out], row pitch ldo (+= when accumulate)
   long long ldo;
+  int n_out;                 // EPI 1: columns stored (<= N; the rest of B's width is padding)
   int accumulate;
   float* part;       // EPI 1 with a K split: partial tiles [split][tiles][BLOCK_M x BLOCK_N]
   // GEMM -> peer ship (see gemm.h)
@@ -255,13 +256,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (gridDim.z == 1) {
           int rows_valid = p.M - m0;
           if (rows_valid > BLOCK_M) rows_valid = BLOCK_M;
-          int cols_valid = p.N - n0;
+          int cols_valid = p.n_out - n0;
           if (cols_valid > BLOCK_N) cols_valid = BLOCK_N;
+          // 8-byte stores need 4-column aligned rows; an output narrower than B (n_out % 4 != 0) is stored per element
+          const bool vec = (p.ldo & 3) == 0 && (reinterpret_cast<uintptr_t>(p.out_bf16) & 7) == 0;
           for (int f = et; f < rows_valid * kVecPerRow; f += kEpiThreads) {
             const int rr = f / kVecPerRow, c4 = (f % kVecPerRow) * 4;
-            if (c4 + 3 >= cols_valid) continue;
-            store_bf16x4(p.out_bf16 + (int64_t)(m0 + rr) * p.ldo + n0 + c4,
-                         *reinterpret_cast<const float4*>(sf + rr * kPitch + c4 * 4), p.accumulate);
+            if (c4 >= cols_valid) continue;
+            const float4 t = *reinterpret_cast<const float4*>(sf + rr * kPitch + c4 * 4);
+            __nv_bfloat16* dst = p.out_bf16 + (int64_t)(m0 + rr) * p.ldo + n0 + c4;
+            if (vec && c4 + 3 < cols_valid) store_bf16x4(dst, t, p.accumulate);
+            else store_bf16_tail(dst, t, cols_valid - c4, p.accumulate);
           }
         } else {
           float* dst = p.part + ((int64_t)blockIdx.z * gridDim.x + tile) * (BLOCK_M * BLOCK_N);
@@ -396,6 +401,7 @@ const char* launch_variant(const GemmArgs& g, cudaStream_t stream) {
   p.col_stats = g.col_stats;
   p.out_bf16 = reinterpret_cast<__nv_bfloat16*>(g.D);
   p.ldo = g.ldd;
+  p.n_out = (EPI == 1 && g.n_out > 0 && g.n_out < g.N) ? g.n_out : g.N;
   p.accumulate = g.accumulate ? 1 : 0;
   p.part = split > 1 ? g.partials : nullptr;
   p.ship_flag = EPI == 0 ? reinterpret_cast<uint32_t*>(g.ship_flag) : nullptr;
@@ -411,8 +417,8 @@ const char* launch_variant(const GemmArgs& g, cudaStream_t stream) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cudaGetErrorString(e);
   if (split > 1) {
-    splitk_reduce(g.partials, split, (int)grid.x, tiles_n, BLOCK_M, BLOCK_N, 1, 0, g.M, g.N, g.D, g.ldd, g.accumulate,
-                  stream);
+    splitk_reduce(g.partials, split, (int)grid.x, tiles_n, BLOCK_M, BLOCK_N, 1, 0, g.M, p.n_out, g.D, g.ldd,
+                  g.accumulate, stream);
     e = cudaGetLastError();
   }
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
@@ -454,7 +460,7 @@ splitk_reduce_kernel(const float* __restrict__ part, int split, int ctas, int ti
         n = (r * 3 + s) * cin + (tile % tiles_n) * bn + cc;
         ok = (tile % tiles_n) * bn + cc + 3 < cin;
       }
-      ok = ok && m < M && n + 3 < N;
+      ok = ok && m < M && n < N;
       if (ok) {
         const float* src = part + (int64_t)t * tile_elems + (int64_t)rr * cols + c4;
         int z = q;
@@ -480,7 +486,10 @@ splitk_reduce_kernel(const float* __restrict__ part, int split, int ctas, int ti
         const float4 o = sm[k][vl];
         acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w;
       }
-      store_bf16x4(out + (int64_t)m * ldo + n, acc, accumulate);
+      // 8-byte stores need 4-column aligned rows; a row pitch or width that is not a multiple of 4 is stored per element
+      const bool vec = (ldo & 3) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0 && n + 3 < N;
+      if (vec) store_bf16x4(out + (int64_t)m * ldo + n, acc, accumulate);
+      else store_bf16_tail(out + (int64_t)m * ldo + n, acc, N - n, accumulate);
     }
     __syncthreads();
   }

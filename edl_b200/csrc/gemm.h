@@ -41,6 +41,10 @@ struct GemmArgs {
   bool accumulate = false;
   float* partials = nullptr;
   int64_t partials_elems = 0;
+  // weight-gradient form: columns of D that are stored (0: all N).  With n_out < N the last N - n_out columns of the
+  // product (zero padding of the B operand, e.g. the 7x7 stem's 147 -> 160 im2col width) never reach memory; D then
+  // needs no alignment beyond its element size
+  int n_out = 0;
   int device = -1;                    // CUDA device ordinal of the operands (binds the context)
   // D = A*B + add_src (bf16 [M, N], row pitch ld_add): fuses the gradient accumulation of a tensor with two
   // consumers (residual branch + 1x1 conv) into the dgrad epilogue.  Persistent kernel only.
@@ -85,6 +89,7 @@ struct Conv3x3Args {
                                // [Cout, 3, 3, Cin/groups]
   int stride = 1;              // 1 or 2 (fprop on the persistent kernel only).  N, H, W are the OUTPUT geometry; with
                                // stride 2 the input X is [N, 2H, 2W, Cin] and is sampled by the TMA traversal stride
+  int ksize = 3;               // 3, or 1: the 1x1 / pad 0 / stride 2 convolution (conv1x1_s2_bf16), Wt is [Cout, Cin]
   int device = -1;
 };
 bool conv3x3_supported(int N, int H, int W, int Cin, int Cout, bool dgrad, int groups = 1);
@@ -92,6 +97,12 @@ const char* conv3x3_bf16(const Conv3x3Args& args, cudaStream_t stream);
 // input gradient of the stride-2 convolution: args.X = dY [N, H, W, Cout], args.Y = dX [N, 2H, 2W, Cin], N/H/W of dY
 bool conv3x3_dgrad_s2_supported(int N, int Ho, int Wo, int Cin, int Cout);
 const char* conv3x3_dgrad_s2_bf16(const Conv3x3Args& args, cudaStream_t stream);
+// 1x1 / pad 0 / stride 2 convolution = the centre tap of the 3x3 / pad 1 / stride 2 one: y[n, h, w] = x[n, 2h, 2w] * W^T.
+// fprop (args.dgrad == false): X = x [N, 2H, 2W, Cin], Y = y [N, H, W, Cout] (+ col_stats or the inference epilogue);
+// dgrad: X = dY [N, H, W, Cout], Y = dX [N, 2H, 2W, Cin], zero at the three pixel parities the convolution skips.
+// Wt is [Cout, Cin]; N, H, W are the output geometry.  Persistent kernel only.
+bool conv1x1_s2_supported(int N, int Ho, int Wo, int Cin, int Cout, bool dgrad);
+const char* conv1x1_s2_bf16(const Conv3x3Args& args, cudaStream_t stream);
 
 // Weight gradient of the same convolution (conv3x3_wgrad.cu): dW[Cout,3,3,Cin] (+)= sum_pixels dY x shifted X, pixel
 // reduction split over `split_k` CTAs through partial tiles like the 1x1 weight-gradient GEMM.
@@ -104,6 +115,7 @@ struct Conv3x3WgradArgs {
   bool accumulate = false;    // dW += result instead of dW = result
   int device = -1;
   int stride = 1;             // 2: X is [N, 2H, 2W, Cin], read through the TMA traversal stride (version-1 kernel)
+  int ksize = 3;              // 1: the 1x1 / pad 0 / stride 2 convolution, dW is [Cout, Cin] (version-1 kernel, one tap)
   // fp32 partial tiles [split][ctas][128 x 3*BLOCK_N], required when split_k > 1: split_k *
   // conv3x3_wgrad_tiles(Cin, Cout) * 128 * 192 elements cover both kernel versions
   float* partials = nullptr;
@@ -136,6 +148,8 @@ const char* conv3x3_dgrad_s2_persistent(const Conv3x3Args& args, int BH, int BN,
                                         cudaStream_t stream);
 const char* conv3x3_bf16_persistent(const Conv3x3Args& args, int BH, int BN, int tiles_h, int tiles_img,
                                     cudaStream_t stream);
+const char* conv1x1_dgrad_s2_persistent(const Conv3x3Args& args, int BH, int BN, int tiles_h, int tiles_img,
+                                        cudaStream_t stream);
 
 // internal: N-d bf16 tensor-map encoder shared by the TMA kernels (defined in gemm.cu)
 const char* encode_tmap_bf16(void* out, const void* ptr, int rank, const uint64_t* dims,

@@ -114,10 +114,15 @@ void set_partials(const c10::optional<Tensor>& partials, float** ptr, int64_t* e
 void gemm_wgrad_bf16(const Tensor& dy, const Tensor& x, Tensor& out, int64_t split_k, bool accumulate,
                      const c10::optional<Tensor>& partials) {
   edl::GemmArgs g = gemm_operands(dy, x, true, true);
-  TORCH_CHECK(out.scalar_type() == at::kBFloat16 && out.dim() == 2 && out.size(0) == g.M && out.size(1) == g.N &&
-              out.stride(1) == 1, "out must be bf16 [N1, N2] with a contiguous last dim");
-  TORCH_CHECK(g.N % 4 == 0 && out.stride(0) % 4 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 8 == 0,
-              "the weight-gradient stores need N2 % 4 == 0 and 8-byte aligned rows");
+  TORCH_CHECK(out.scalar_type() == at::kBFloat16 && out.dim() == 2 && out.size(0) == g.M && out.size(1) <= g.N &&
+              out.size(1) > 0 && out.stride(1) == 1, "out must be bf16 [N1, <= N2] with a contiguous last dim");
+  if (out.size(1) == g.N) {
+    TORCH_CHECK(g.N % 4 == 0 && out.stride(0) % 4 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 8 == 0,
+                "the weight-gradient stores need N2 % 4 == 0 and 8-byte aligned rows");
+  } else {
+    // a narrower output: only its columns are stored (x's last columns are padding, e.g. the 7x7 stem's im2col)
+    g.n_out = (int)out.size(1);
+  }
   g.D = out.data_ptr();
   g.ldd = out.stride(0);
   g.split_k = (int)split_k;
@@ -218,6 +223,80 @@ void conv3x3_dgrad_s2(const Tensor& dy, const Tensor& w, Tensor& dx) {
 }
 bool conv3x3_dgrad_s2_supported(int64_t n, int64_t ho, int64_t wo, int64_t cin, int64_t cout) {
   return edl::conv3x3_dgrad_s2_supported((int)n, (int)ho, (int)wo, (int)cin, (int)cout);
+}
+
+// 1x1 / pad 0 / stride 2 convolution (gemm.h conv1x1_s2_bf16) on the persistent kernel, w [Cout, Cin] (any [Cout, 1, 1, Cin]
+// view).  fprop: x [N, Cin, 2H, 2W] -> y [N, Cout, H, W] with col_stats (training) or col_scale / col_shift / relu
+// (inference).  dgrad: x is dY [N, Cout, H, W], y is dX [N, Cin, 2H, 2W] (zero-filled, then the even-even pixels).
+void conv1x1_s2(const Tensor& x, const Tensor& w, Tensor& y, bool dgrad, const c10::optional<Tensor>& col_stats,
+                const c10::optional<Tensor>& col_scale, const c10::optional<Tensor>& col_shift, bool relu) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 4 && y.dim() == 4);
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && y.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16);
+  TORCH_CHECK(x.is_contiguous(at::MemoryFormat::ChannelsLast) && y.is_contiguous(at::MemoryFormat::ChannelsLast),
+              "conv1x1_s2 needs channels_last activations");
+  TORCH_CHECK(w.is_contiguous() && w.numel() == w.size(0) * w.size(-1), "weight must be [Cout, Cin] (or [Cout, 1, 1, Cin])");
+  const Tensor& in = dgrad ? y : x;      // the convolution's input  [N, Cin, 2H, 2W]
+  const Tensor& out = dgrad ? x : y;     // the convolution's output [N, Cout, H, W]
+  edl::Conv3x3Args a;
+  a.X = x.data_ptr();
+  a.Wt = w.data_ptr();
+  a.Y = y.data_ptr();
+  a.N = out.size(0);
+  a.H = out.size(2);
+  a.W = out.size(3);
+  a.Cout = w.size(0);
+  a.Cin = w.size(-1);
+  a.dgrad = dgrad;
+  a.stride = 2;
+  a.ksize = 1;
+  TORCH_CHECK(in.size(0) == a.N && in.size(1) == a.Cin && out.size(1) == a.Cout && in.size(2) == 2 * a.H &&
+              in.size(3) == 2 * a.W, "conv1x1_s2: x / w / y shapes do not belong together (input 2H x 2W)");
+  TORCH_CHECK(!dgrad || (!col_stats.has_value() && !col_scale.has_value() && !col_shift.has_value() && !relu),
+              "conv1x1_s2: statistics / epilogue belong to the fprop launch");
+  a.col_stats = optp<float>(col_stats);
+  a.col_scale = optp<float>(col_scale);
+  a.col_shift = optp<float>(col_shift);
+  a.relu = relu;
+  a.device = x.device().index();
+  c10::cuda::CUDAGuard guard(x.device());
+  const char* err = edl::conv1x1_s2_bf16(a, at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl conv1x1_s2 failed: ", err);
+}
+bool conv1x1_s2_supported(int64_t n, int64_t ho, int64_t wo, int64_t cin, int64_t cout, bool dgrad) {
+  return edl::conv1x1_s2_supported((int)n, (int)ho, (int)wo, (int)cin, (int)cout, dgrad);
+}
+
+// dW [Cout, Cin] (+)= weight gradient of the 1x1 / pad 0 / stride 2 convolution: x [N, Cin, 2H, 2W], dy [N, Cout, H, W]
+// channels_last; the version-1 weight-gradient kernel with one tap (split_k > 1 needs `partials`: split_k *
+// conv3x3_wgrad_tiles(Cin, Cout) / 3 * 128 * 64 floats)
+void conv1x1_s2_wgrad(const Tensor& x, const Tensor& dy, Tensor& dw, int64_t split_k, bool accumulate,
+                      const c10::optional<Tensor>& partials) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 4 && dy.dim() == 4);
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && dy.scalar_type() == at::kBFloat16 && dw.scalar_type() == at::kBFloat16);
+  TORCH_CHECK(x.is_contiguous(at::MemoryFormat::ChannelsLast) && dy.is_contiguous(at::MemoryFormat::ChannelsLast),
+              "conv1x1_s2_wgrad needs channels_last activations");
+  TORCH_CHECK(dw.is_contiguous() && dw.numel() == dw.size(0) * dw.size(-1), "dw must be [Cout, Cin] (or [Cout, 1, 1, Cin])");
+  edl::Conv3x3WgradArgs a;
+  a.X = x.data_ptr();
+  a.dY = dy.data_ptr();
+  a.dW = dw.data_ptr();
+  a.N = x.size(0);
+  a.H = dy.size(2);
+  a.W = dy.size(3);
+  a.Cin = x.size(1);
+  a.Cout = dy.size(1);
+  a.stride = 2;
+  a.ksize = 1;
+  TORCH_CHECK(dy.size(0) == a.N && x.size(2) == 2 * a.H && x.size(3) == 2 * a.W && dw.size(0) == a.Cout &&
+              dw.size(-1) == a.Cin, "conv1x1_s2_wgrad: x / dy / dw shapes do not belong together");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(a.dW) % 8 == 0, "dw window must be 8-byte aligned");
+  a.split_k = (int)split_k;
+  a.accumulate = accumulate;
+  set_partials(partials, &a.partials, &a.partials_elems);
+  a.device = x.device().index();
+  c10::cuda::CUDAGuard guard(x.device());
+  const char* err = edl::conv3x3_wgrad_bf16(a, at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl conv1x1_s2_wgrad failed: ", err);
 }
 
 // D bf16 [M,N] = relu?((A8[M,K] * B8[N,K]^T) * col_scale + col_shift); A8/B8 are e4m3 bytes (uint8 / float8 tensors)
@@ -472,4 +551,7 @@ void register_gemm_bindings(pybind11::module_& m) {
   m.def("get_wgrad3_version", &edl::get_wgrad3_version);
   m.def("conv3x3_wgrad_plan", &conv3x3_wgrad_plan);
   m.def("conv3x3_s2", &conv3x3_s2);
+  m.def("conv1x1_s2", &conv1x1_s2);
+  m.def("conv1x1_s2_supported", &conv1x1_s2_supported);
+  m.def("conv1x1_s2_wgrad", &conv1x1_s2_wgrad);
 }

@@ -1006,6 +1006,10 @@ const char* conv3x3_bf16_persistent(const Conv3x3Args& a, int BH, int BN, int ti
   alignas(64) CUtensorMap tmX, tmW, tmY;
   const int sd = a.stride == 2 ? 2 : 1;
   if (sd == 2 && (dg || 2 * a.W > 256 || 2 * BH > 256)) return "conv3x3 stride 2: fprop only, output width <= 128";
+  // 1x1 / pad 0 / stride 2: the centre tap of the stride-2 3x3 -- the same strided input map, one tap at (0, 0)
+  const bool k1 = a.ksize == 1;
+  if (k1 && (sd != 2 || groups != 1)) return "conv1x1 stride 2: dense, stride 2 only";
+  const int taps = k1 ? 1 : 9;
   const bool halo = g_conv_halo && sd == 1 &&
                     halo_geometry(a.N, a.H, a.W, &BH, &BN, &tiles_h, &tiles_img);
   if (halo) {
@@ -1029,14 +1033,18 @@ const char* conv3x3_bf16_persistent(const Conv3x3Args& a, int BH, int BN, int ti
     if (const char* e = encode_tmap_bf16(&tmY, a.Y, 4, dims, st, box)) return e;
   }
   const int w_cin = a.Cin / a.groups;      // channel extent of the KRSC weight tensor
-  if (const char* e = tmap2d(&tmW, a.Wt, (uint64_t)9 * w_cin, a.Cout, (uint64_t)9 * w_cin, 64, dg ? kBlockK : bn))
+  if (const char* e = tmap2d(&tmW, a.Wt, (uint64_t)taps * w_cin, a.Cout, (uint64_t)taps * w_cin, 64, dg ? kBlockK : bn))
     return e;
   PersistParams p{};
-  p.M = tiles_img * tiles_h * kBlockM; p.N = cy; p.K = 9 * cx;
+  p.M = tiles_img * tiles_h * kBlockM; p.N = cy; p.K = taps * cx;
   p.tiles_m = tiles_img * tiles_h;
   p.tiles_n = (cy + bn - 1) / bn;
   p.kc_blocks = cin_g / kBlockK;
-  p.num_kb = (halo ? 3 : 9) * p.kc_blocks;
+  p.num_kb = (halo ? 3 : taps) * p.kc_blocks;
+  if (k1) {
+    p.ntaps = 1;
+    p.tap_dh[0] = p.tap_dw[0] = p.tap_w[0] = 0;
+  }
   p.Wb = halo ? a.W + 1 : a.W;
   p.b_res = (halo && n64 && p.kc_blocks == 1 && g_conv_bres) ? 1 : 0;
   p.col_stats = dg ? nullptr : a.col_stats;
@@ -1084,6 +1092,54 @@ void set_conv_halo(bool on) { g_conv_halo = on; }
 void set_conv_resident_weights(bool on) { g_conv_bres = on; }
 bool get_conv_halo() { return g_conv_halo; }
 
+namespace {
+// One parity class (ph, pw) of a stride-2 input gradient: a stride-1 dgrad-mode launch over dY with the taps of that class,
+// storing the pixels (2 i + ph, 2 j + pw) of dX through a tensor map with doubled pixel strides.  tmX / tmW are the dY
+// and weight maps, c_in_w the weight's channel extent per tap (Cin), taps {dh, dw, weight tap} of the class.
+const char* dgrad_s2_parity(const Conv3x3Args& a, int BH, int BN, int tiles_h, int tiles_img, const CUtensorMap& tmX,
+                            const CUtensorMap& tmW, int ph, int pw, int ntaps, const signed char (*taps)[3],
+                            cudaStream_t stream) {
+  const int cx = a.Cout, cy = a.Cin;
+  const bool n64 = cy <= 64;
+  const int bn = n64 ? 64 : 128;
+  const uint64_t W2 = 2ull * a.W, H2 = 2ull * a.H;
+  alignas(64) CUtensorMap tmY;
+  {
+    // the pixels (2 i + ph, 2 j + pw) of dX as a dense-looking [N, Ho, Wo, Cin] tensor with doubled pixel strides
+    const uint64_t dims[4] = {(uint64_t)cy, (uint64_t)a.W, (uint64_t)a.H, (uint64_t)a.N};
+    const uint64_t st[3] = {2ull * cy * 2, 2ull * W2 * cy * 2, H2 * W2 * cy * 2};
+    const uint32_t box[4] = {64, (uint32_t)a.W, (uint32_t)BH, (uint32_t)BN};
+    const char* base = reinterpret_cast<const char*>(a.Y) + ((uint64_t)ph * W2 + pw) * cy * 2;
+    if (const char* e = encode_tmap_bf16(&tmY, base, 4, dims, st, box)) return e;
+  }
+  PersistParams p{};
+  p.M = tiles_img * tiles_h * kBlockM; p.N = cy; p.K = ntaps * cx;
+  p.tiles_m = tiles_img * tiles_h;
+  p.tiles_n = (cy + bn - 1) / bn;
+  p.kc_blocks = cx / kBlockK;
+  p.cin_g = cx; p.cout_g = cy;
+  p.n_img = a.N; p.H = a.H; p.W = a.W; p.c_in_w = a.Cin; p.BH = BH; p.BN = BN; p.tiles_h = tiles_h;
+  p.stride = 1;
+  for (int t = 0; t < ntaps; ++t) {
+    p.tap_dh[t] = taps[t][0];
+    p.tap_dw[t] = taps[t][1];
+    p.tap_w[t] = taps[t][2];
+  }
+  p.ntaps = ntaps;
+  p.num_kb = ntaps * p.kc_blocks;
+  return n64 ? launch_p<64, 6, 3>(tmX, tmW, tmY, p, stream) : launch_p<128, 5, 3>(tmX, tmW, tmY, p, stream);
+}
+
+// dY [N, Ho, Wo, Cout] as the A operand of the dgrad mode
+const char* dgrad_s2_dy_map(const Conv3x3Args& a, int BH, int BN, CUtensorMap* tmX) {
+  const int cx = a.Cout;
+  const uint64_t dims[4] = {(uint64_t)cx, (uint64_t)a.W, (uint64_t)a.H, (uint64_t)a.N};
+  const uint64_t st[3] = {(uint64_t)cx * 2, (uint64_t)a.W * cx * 2, (uint64_t)a.H * a.W * cx * 2};
+  const uint32_t box[4] = {64, (uint32_t)a.W, (uint32_t)BH, (uint32_t)BN};
+  return encode_tmap_bf16(tmX, a.X, 4, dims, st, box);
+}
+}  // namespace
+
 // Input gradient of the 3x3 / pad 1 / STRIDE 2 convolution (round 2).  dX[n, h, w] = sum over the taps (r, s) with
 // h + 1 - r and w + 1 - s even of dY[n, (h + 1 - r) / 2, (w + 1 - s) / 2] * W[:, r, s, :]: for a fixed parity (h & 1, w & 1)
 // that is a stride-1 convolution of dY with 1, 2, 2 or 4 taps whose result lands on every second pixel of dX.  Four
@@ -1092,55 +1148,43 @@ bool get_conv_halo() { return g_conv_halo; }
 // a.X = dY [N, Ho, Wo, Cout], a.Y = dX [N, 2 Ho, 2 Wo, Cin], a.N / H / W = the dY geometry.
 const char* conv3x3_dgrad_s2_persistent(const Conv3x3Args& a, int BH, int BN, int tiles_h, int tiles_img,
                                         cudaStream_t stream) {
-  const int cx = a.Cout, cy = a.Cin;
-  const bool n64 = cy <= 64;
-  const int bn = n64 ? 64 : 128;
   alignas(64) CUtensorMap tmX, tmW;
-  {
-    const uint64_t dims[4] = {(uint64_t)cx, (uint64_t)a.W, (uint64_t)a.H, (uint64_t)a.N};
-    const uint64_t st[3] = {(uint64_t)cx * 2, (uint64_t)a.W * cx * 2, (uint64_t)a.H * a.W * cx * 2};
-    const uint32_t box[4] = {64, (uint32_t)a.W, (uint32_t)BH, (uint32_t)BN};
-    if (const char* e = encode_tmap_bf16(&tmX, a.X, 4, dims, st, box)) return e;
-  }
+  if (const char* e = dgrad_s2_dy_map(a, BH, BN, &tmX)) return e;
   if (const char* e = tmap2d(&tmW, a.Wt, (uint64_t)9 * a.Cin, a.Cout, (uint64_t)9 * a.Cin, 64, kBlockK)) return e;
-  const uint64_t W2 = 2ull * a.W, H2 = 2ull * a.H;
   for (int ph = 0; ph < 2; ++ph) {
     for (int pw = 0; pw < 2; ++pw) {
-      alignas(64) CUtensorMap tmY;
-      {
-        // the pixels (2 i + ph, 2 j + pw) of dX as a dense-looking [N, Ho, Wo, Cin] tensor with doubled pixel strides
-        const uint64_t dims[4] = {(uint64_t)cy, (uint64_t)a.W, (uint64_t)a.H, (uint64_t)a.N};
-        const uint64_t st[3] = {2ull * cy * 2, 2ull * W2 * cy * 2, H2 * W2 * cy * 2};
-        const uint32_t box[4] = {64, (uint32_t)a.W, (uint32_t)BH, (uint32_t)BN};
-        const char* base = reinterpret_cast<const char*>(a.Y) + ((uint64_t)ph * W2 + pw) * cy * 2;
-        if (const char* e = encode_tmap_bf16(&tmY, base, 4, dims, st, box)) return e;
-      }
-      PersistParams p{};
-      p.M = tiles_img * tiles_h * kBlockM; p.N = cy; p.K = 9 * cx;
-      p.tiles_m = tiles_img * tiles_h;
-      p.tiles_n = (cy + bn - 1) / bn;
-      p.kc_blocks = cx / kBlockK;
-      p.cin_g = cx; p.cout_g = cy;
-      p.n_img = a.N; p.H = a.H; p.W = a.W; p.c_in_w = a.Cin; p.BH = BH; p.BN = BN; p.tiles_h = tiles_h;
-      p.stride = 1;
+      signed char taps[4][3];
       int nt = 0;
       for (int r = 0; r < 3; ++r) {
         if (((ph + 1 - r) & 1) != 0) continue;
         for (int sft = 0; sft < 3; ++sft) {
           if (((pw + 1 - sft) & 1) != 0) continue;
-          p.tap_dh[nt] = (signed char)((ph + 1 - r) / 2);      // exact: the numerator is even (0 or 2)
-          p.tap_dw[nt] = (signed char)((pw + 1 - sft) / 2);
-          p.tap_w[nt] = (signed char)(r * 3 + sft);
+          taps[nt][0] = (signed char)((ph + 1 - r) / 2);      // exact: the numerator is even (0 or 2)
+          taps[nt][1] = (signed char)((pw + 1 - sft) / 2);
+          taps[nt][2] = (signed char)(r * 3 + sft);
           ++nt;
         }
       }
-      p.ntaps = nt;
-      p.num_kb = nt * p.kc_blocks;
-      const char* e = n64 ? launch_p<64, 6, 3>(tmX, tmW, tmY, p, stream) : launch_p<128, 5, 3>(tmX, tmW, tmY, p, stream);
-      if (e != nullptr) return e;
+      if (const char* e = dgrad_s2_parity(a, BH, BN, tiles_h, tiles_img, tmX, tmW, ph, pw, nt, taps, stream)) return e;
     }
   }
   return nullptr;
+}
+
+// Input gradient of the 1x1 / pad 0 / stride 2 convolution: dX[n, 2h, 2w] = dY[n, h, w] * W and zero elsewhere.  dX is
+// zero-filled (a memset node when captured in a graph), then ONE dgrad-mode launch with the single tap (0, 0) stores the
+// even-even pixels through the parity-(0, 0) map of the 3x3 path.  dX stays a dense tensor, so a consumer that adds it to
+// another gradient (the bottleneck's forked input) reads it like any other.  Weight [Cout, Cin], read MN-major.
+const char* conv1x1_dgrad_s2_persistent(const Conv3x3Args& a, int BH, int BN, int tiles_h, int tiles_img,
+                                        cudaStream_t stream) {
+  alignas(64) CUtensorMap tmX, tmW;
+  if (const char* e = dgrad_s2_dy_map(a, BH, BN, &tmX)) return e;
+  if (const char* e = tmap2d(&tmW, a.Wt, (uint64_t)a.Cin, a.Cout, (uint64_t)a.Cin, 64, kBlockK)) return e;
+  const size_t dx_bytes = (size_t)a.N * (2 * a.H) * (2 * a.W) * a.Cin * 2;
+  cudaError_t ce = cudaMemsetAsync(a.Y, 0, dx_bytes, stream);
+  if (ce != cudaSuccess) return cudaGetErrorString(ce);
+  const signed char centre[1][3] = {{0, 0, 0}};
+  return dgrad_s2_parity(a, BH, BN, tiles_h, tiles_img, tmX, tmW, 0, 0, 1, centre, stream);
 }
 
 }  // namespace edl

@@ -64,6 +64,14 @@ class ConvBNAct(nn.Module):
                 and ops.gemm.CONV3_S2 and ops.conv3x3_s2_supported(x, self.weight)):
             # experimental (EDL_CONV3_S2=1): stride-2 fprop on the wgmma kernel, statistics in its epilogue
             op = ops.conv3x3_s2
+        elif (self.k == 1 and self.stride == 2 and self.groups == 1 and self.impl != "cudnn"
+                and ops.conv1x1_s2_supported(x, self.weight)):
+            # plain ResNet's projection shortcuts: 1x1 / stride 2 on the persistent kernel (the stride-2 3x3's centre tap)
+            op = ops.conv1x1_s2 if (want_stats or torch.is_grad_enabled()) else ops.conv1x1_s2_infer
+        elif (self.k == 7 and self.stride == 2 and self.cin == 3 and self.impl != "cudnn"
+                and ops.stem7_supported(x, self.weight)):
+            # plain ResNet's 7x7 stem: im2col + persistent GEMM (statistics in its epilogue), split-K GEMM weight gradient
+            op = ops.stem7
         if op is not None:
             stats = None
             if want_stats:

@@ -88,7 +88,8 @@ from .bn import (batch_norm_act, BatchNormAct2d, scale_shift_act, bn_stats_into,
 from .loss import soft_cross_entropy, topk_accuracy  # noqa: E402
 from .pool import max_pool_3x3_s2, avg_pool_2x2, global_avg_pool  # noqa: E402
 from .optim import FlatSGDMomentum, FlatAdam, SparseAdam  # noqa: E402
-from .gemm import stem7_infer, stem7_supported  # noqa: E402
+from .gemm import stem7, stem7_infer, stem7_supported  # noqa: E402
+from .gemm import conv1x1_s2, conv1x1_s2_infer, conv1x1_s2_supported  # noqa: E402
 from .gemm import (gemm_bf16, linear_bf16, conv1x1, conv_lib, conv3x3, conv3x3_supported, conv3x3_infer,  # noqa: E402
                    conv3x3_infer_supported, conv3x3_wgrad, conv3x3_wgrad_supported, conv3x3_s2, conv3x3_s2_infer,
                    conv3x3_s2_supported, stem_conv, stem_conv_supported, conv3x3_pair, conv3x3_pair_supported)
@@ -103,6 +104,7 @@ __all__ = [
     "FlatSGDMomentum", "FlatAdam", "SparseAdam", "embedding_bag_mean_sparse", "embedding_bags_mean_sparse",
     "gemm_bf16", "linear_bf16", "conv1x1", "conv_lib", "conv3x3",
     "conv3x3_supported", "conv3x3_infer", "conv3x3_infer_supported", "stem7_infer", "stem7_supported",
+    "stem7", "conv1x1_s2", "conv1x1_s2_infer", "conv1x1_s2_supported",
     "conv3x3_wgrad", "conv3x3_wgrad_supported", "conv3x3_s2", "conv3x3_s2_infer", "conv3x3_s2_supported",
     "stem_conv", "stem_conv_supported", "conv3x3_pair", "conv3x3_pair_supported",
     "rope", "rope_tables", "embedding_bag_mean", "normalize_u8", "DynamicLossScaler", "set_fused_bn", "set_relu_mask",

@@ -639,6 +639,113 @@ def conv3x3_s2(x, weight_krsc, stats: Optional[torch.Tensor] = None):
     return _Conv3x3S2Fn.apply(x, weight_krsc, stats, *_grad_sink(weight_krsc))
 
 
+# ---------------------------------------------------------------------------------------------------------------
+# 1x1 / pad 0 / stride 2 convolutions (the projection shortcuts of plain ResNet): output pixel (h, w) reads input pixel
+# (2h, 2w), i.e. the centre tap of the stride-2 3x3 convolution above -- fprop on the persistent kernel through the same
+# strided input map, dgrad as one dgrad-mode launch storing the even-even pixels of a zero-filled dX, wgrad on the
+# version-1 weight-gradient kernel with one tap (csrc/gemm_persist.cu, csrc/conv3x3_wgrad.cu).
+
+def conv1x1_s2_supported(x, weight_krsc) -> bool:
+    from . import native
+
+    if not (x.is_cuda and x.dtype == torch.bfloat16 and weight_krsc.dtype == torch.bfloat16 and x.dim() == 4):
+        return False
+    n, c, h, w = x.shape
+    if weight_krsc.dim() == 4 and tuple(weight_krsc.shape[1:3]) != (1, 1):
+        return False
+    cout, cin = weight_krsc.shape[0], weight_krsc.shape[-1]
+    return (cin == c and c % 64 == 0 and h % 2 == 0 and w % 2 == 0 and w // 2 <= 128
+            and native().conv1x1_s2_supported(n, h // 2, w // 2, c, cout, False))
+
+
+def _conv1x1_s2_launch(x, weight, stats, scale, shift, relu):
+    from . import native, count_launch
+
+    x = _cl(x)
+    n, _, h, w = x.shape
+    y = torch.empty((n, weight.shape[0], h // 2, w // 2), device=x.device, dtype=x.dtype, memory_format=torch.channels_last)
+    native().conv1x1_s2(x, weight, y, False, stats, scale, shift, relu)
+    count_launch()
+    return y
+
+
+@torch.no_grad()
+def conv1x1_s2_infer(x, weight_krsc, scale=None, shift=None, relu=False):
+    """Inference 1x1 / stride 2 convolution with the folded-BN scale / shift and the ReLU in the epilogue."""
+    return _conv1x1_s2_launch(x, weight_krsc, None, scale, shift, relu)
+
+
+def conv1x1_s2_wgrad_split(n, ho, wo, cin, cout) -> int:
+    """Split-K factor of the 1x1 / stride-2 weight gradient: the rule of ``conv3x3_wgrad_split`` over its tiles (one CTA
+    per 128 x 64 tile instead of three)."""
+    from . import native
+
+    kblocks, ctas = native().conv3x3_wgrad_s2_kblocks(n, ho, wo), native().conv3x3_wgrad_tiles(cin, cout) // 3
+    return 1 if ctas >= 48 else max(1, min(max(1, _NUM_SMS // ctas), max(1, kblocks // 2)))
+
+
+def conv1x1_s2_wgrad(x, dy, weight_shape, sink=None, split_k: Optional[int] = None):
+    """dW [Cout, 1, 1, Cin] of the 1x1 / stride 2 convolution; with ``sink`` added into it (returns None)."""
+    from . import native, count_launch
+
+    x, dy = _cl(x), _cl(dy)
+    cout, cin = weight_shape[0], weight_shape[-1]
+    n, _, ho, wo = dy.shape
+    if split_k is None:
+        split_k = conv1x1_s2_wgrad_split(n, ho, wo, cin, cout)
+    if sink is not None:
+        out, acc = sink.view(weight_shape), True
+    else:
+        out, acc = torch.empty(tuple(weight_shape), device=x.device, dtype=torch.bfloat16), False
+    tiles = native().conv3x3_wgrad_tiles(cin, cout) // 3
+    partials = _splitk_partials(x.device, split_k * tiles * 128 * 64) if split_k > 1 else None
+    native().conv1x1_s2_wgrad(x, dy, out, int(split_k), acc, partials)
+    count_launch(2 if split_k > 1 else 1)
+    return None if sink is not None else out
+
+
+class _Conv1x1S2Fn(torch.autograd.Function):
+    """Training form of the 1x1 / stride 2 convolution (BN statistics in the fprop epilogue).  The input gradient is a
+    dense tensor, zero at the three pixel parities the convolution skips, so a forked input adds it like any other."""
+
+    @staticmethod
+    def forward(ctx, x, w, stats, sink, ready):
+        x = _cl(x)
+        y = _conv1x1_s2_launch(x, w, stats, None, None, False)
+        ctx.save_for_backward(x, w)
+        ctx.cfg = (2, 0, 1)
+        ctx.sink, ctx.ready = sink, ready
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        from . import native, count_launch
+
+        x, w = ctx.saved_tensors
+        dy = _cl(dy)
+        n, c, h, wd = x.shape
+        cout = w.shape[0]
+        dx = dw = None
+        if ctx.needs_input_grad[0]:
+            if native().conv1x1_s2_supported(n, h // 2, wd // 2, c, cout, True):
+                dx = torch.empty_like(x)
+                native().conv1x1_s2(dy, w, dx, True, None, None, None, False)
+                count_launch()
+            else:
+                dx = _lib_dgrad(dy, x, w, ctx.cfg)
+        if ctx.needs_input_grad[1]:
+            own = native().conv3x3_wgrad_s2_supported(n, h // 2, wd // 2, c, cout)
+            dw = _deliver_wgrad(dy, x, ctx.sink, ctx.ready, lambda sink: (
+                conv1x1_s2_wgrad(x, dy, w.shape, sink) if own else _lib_wgrad(dy, x, w, ctx.cfg, sink)))
+        return dx, dw, None, None, None
+
+
+def conv1x1_s2(x, weight_krsc, stats: Optional[torch.Tensor] = None):
+    """NHWC 1x1 / pad 0 / stride 2 convolution, weight [Cout, 1, 1, Cin]; ``stats`` (pre-zeroed fp32 [2*Cout]) receives
+    the per-channel sum / sum of squares of the output for the following train-mode BatchNorm."""
+    return _Conv1x1S2Fn.apply(x, weight_krsc, stats, *_grad_sink(weight_krsc))
+
+
 # The first stem convolution (3 -> 32 channels, 3x3 / stride 2) runs on the direct kernel of csrc/stem.cu with the
 # BatchNorm statistics fused in.  On by default (EDL_OWN_STEM1=0: library kernel).
 OWN_STEM1 = __import__("os").environ.get("EDL_OWN_STEM1", "1") == "1"
@@ -681,6 +788,78 @@ def stem7_infer(x, weight_krsc, scale=None, shift=None, relu=False):
     y = torch.empty((n, cout, ho, wo), device=x.device, dtype=x.dtype, memory_format=torch.channels_last)
     gemm_bf16(a, wp, out=y.permute(0, 2, 3, 1).reshape(-1, cout), col_scale=scale, col_shift=shift, relu=relu)
     return y
+
+
+def _stem7_padded(weight_krsc):
+    """The [Cout, 160] GEMM weight of a 7x7 stem, rebuilt from ``weight_krsc`` on EVERY call: one copy of the 147 real
+    columns into a buffer kept on the parameter (its 13 pad columns stay zero).  The copy is part of a captured graph, so
+    a replay reads the weight the optimizer last wrote -- a cache keyed on ``weight._version`` (``stem7_infer``) would not
+    see the in-place updates of a replayed optimizer step."""
+    cout = weight_krsc.shape[0]
+    buf = getattr(weight_krsc, "_edl_stem7_padded", None)
+    if buf is None or buf.device != weight_krsc.device or buf.shape[0] != cout:
+        buf = torch.zeros((cout, 160), device=weight_krsc.device, dtype=torch.bfloat16)
+        weight_krsc._edl_stem7_padded = buf
+    buf[:, :147].copy_(weight_krsc.detach().reshape(cout, 147))
+    return buf
+
+
+def stem7_wgrad(dy, a, weight_shape, sink=None, split_k: Optional[int] = None):
+    """dW [Cout, 7, 7, 3] of the 7x7 stem from its output gradient and saved im2col matrix ``a`` [M, 160]: the split-K
+    weight-gradient GEMM over the padded width, storing only the 147 real columns (KRSC order = [Cout, 147]); with
+    ``sink`` added into it (returns None)."""
+    from . import native, count_launch
+
+    dy = _cl(dy)
+    cout = weight_shape[0]
+    dy2 = dy.permute(0, 2, 3, 1).reshape(-1, cout)
+    split = split_k if split_k is not None else _split_k_for(cout, 160, dy2.shape[0])
+    out = sink.view(cout, 147) if sink is not None else torch.empty((cout, 147), device=dy.device, dtype=torch.bfloat16)
+    tiles = (cout + 127) // 128 * 2            # 128-column tiles over the 160 columns
+    partials = _splitk_partials(dy.device, split * tiles * 128 * 128) if split > 1 else None
+    native().gemm_wgrad_bf16(dy2, a, out, split, sink is not None, partials)
+    count_launch(2 if split > 1 else 1)
+    return None if sink is not None else out.view(weight_shape)
+
+
+class _Stem7Fn(torch.autograd.Function):
+    """Training form of the 7x7 / stride 2 / pad 3 stem: ``stem7_im2col`` + the persistent GEMM with the BN statistics
+    in its epilogue; the im2col matrix is kept for the weight gradient.  The input is the image: no dgrad."""
+
+    @staticmethod
+    def forward(ctx, x, w, stats, sink, ready):
+        from . import native, count_launch
+
+        x = _cl(x)
+        n, _, h, wd = x.shape
+        ho, wo = (h - 1) // 2 + 1, (wd - 1) // 2 + 1
+        cout = w.shape[0]
+        wp = _stem7_padded(w)
+        a = torch.empty((n * ho * wo, 160), device=x.device, dtype=torch.bfloat16)
+        native().stem7_im2col(x, a)
+        count_launch()
+        y = torch.empty((n, cout, ho, wo), device=x.device, dtype=x.dtype, memory_format=torch.channels_last)
+        gemm_bf16(a, wp, out=y.permute(0, 2, 3, 1).reshape(-1, cout), col_stats=stats)
+        ctx.save_for_backward(x, w, a)
+        ctx.sink, ctx.ready = sink, ready
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, a = ctx.saved_tensors
+        dx = dw = None
+        if ctx.needs_input_grad[0]:      # nobody asks for the gradient of the images; kept for completeness
+            dx = _lib_dgrad(_cl(dy), x, w, (2, 3, 1))
+        if ctx.needs_input_grad[1]:
+            dw = _deliver_wgrad(dy, a, ctx.sink, ctx.ready, lambda sink: stem7_wgrad(dy, a, w.shape, sink))
+        return dx, dw, None, None, None
+
+
+def stem7(x, weight_krsc, stats: Optional[torch.Tensor] = None):
+    """7x7 / stride 2 / pad 3 convolution of a 3-channel image (plain ResNet's stem), weight KRSC [Cout, 7, 7, 3];
+    ``stats`` (pre-zeroed fp32 [2*Cout]) receives the BN statistics of the output.  ``stem7_supported`` states what is
+    accepted."""
+    return _Stem7Fn.apply(x, weight_krsc, stats, *_grad_sink(weight_krsc))
 
 
 def stem_conv_supported(x, weight_krsc) -> bool:
