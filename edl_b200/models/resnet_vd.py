@@ -17,7 +17,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import ops
-from ..ops.bn import BatchNormAct2d
+from ..ops.bn import BatchNormAct2d, checkpoint_context
 
 
 class ConvBNAct(nn.Module):
@@ -222,7 +222,7 @@ class ResNetVd(nn.Module):
         if self.recompute and self.training and torch.is_grad_enabled():
             from torch.utils.checkpoint import checkpoint
             for blk in self.blocks:
-                x = checkpoint(blk, x, use_reentrant=False)
+                x = checkpoint(blk, x, use_reentrant=False, context_fn=checkpoint_context)
         else:
             x = self.blocks(x)
         x = ops.global_avg_pool(x)

@@ -6,6 +6,8 @@ tensors in ``channels_last`` memory format (i.e. NHWC in memory) or plain 2-D ``
 """
 from __future__ import annotations
 
+import contextlib
+
 import torch
 import torch.nn as nn
 
@@ -33,6 +35,27 @@ _RELU_MASK = _os.environ.get("EDL_RELU_MASK", "1") == "1"
 def set_relu_mask(enabled: bool) -> None:
     global _RELU_MASK
     _RELU_MASK = bool(enabled)
+
+
+# True while torch.utils.checkpoint re-runs a block's forward during backward: that forward must not update the running
+# statistics a second time.  A plain flag, not thread-local: the recompute runs on autograd's device threads.
+_RECOMPUTING = False
+
+
+@contextlib.contextmanager
+def _recomputing():
+    global _RECOMPUTING
+    prev, _RECOMPUTING = _RECOMPUTING, True
+    try:
+        yield
+    finally:
+        _RECOMPUTING = prev
+
+
+def checkpoint_context():
+    """``context_fn`` for ``torch.utils.checkpoint.checkpoint(use_reentrant=False)``: the first forward runs as usual,
+    the recomputed one leaves every ``BatchNormAct2d``'s running statistics alone."""
+    return contextlib.nullcontext(), _recomputing()
 
 
 def _mc(x: torch.Tensor) -> torch.Tensor:
@@ -327,7 +350,9 @@ class BatchNormAct2d(nn.Module):
         return sg, sb, (lambda: [c() for c in cbs]) if cbs else None
 
     def forward(self, x, residual=None, sums=None):
-        return batch_norm_act(x, self.weight, self.bias, self.running_mean, self.running_var,
+        # the kernels skip the running-statistics update when they get none (a recomputed forward)
+        rm, rv = (None, None) if _RECOMPUTING else (self.running_mean, self.running_var)
+        return batch_norm_act(x, self.weight, self.bias, rm, rv,
                               residual=residual, relu=self.relu, training=self.training,
                               momentum=self.momentum, eps=self.eps, sums=sums, ws=self.ws,
                               sinks=self._sinks())

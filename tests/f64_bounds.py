@@ -52,6 +52,16 @@ and over tests/test_bn_pool_bounds_gpu.py, test_kernels_gpu.py and test_relu_mas
     saved rstd, staged and vs exact                          c1 1.000 (the constant channel: rsqrtf(eps) at the
                                                              interval's end, since the variance cannot go below 0)
     scale_shift_act, max-pool dx, average pool, global pool  c1 1.000   c2 1.00
+and layer by layer inside whole training steps (tests/test_step_oracle_gpu.py: ResNet50_vd, ResNet18_vd and plain
+ResNet50, every BatchNorm mode, the trainer and its graph replays; NVIDIA H100 80GB HBM3, 700 W power limit):
+
+    conv fprop (all paths), BatchNorm y and dx, dgrad           c1 1.000   c2 1.00
+    activation gradients summed over consumers (``terms``)      c1 0.991   c2 1.03
+    weight gradients in .grad and bucket windows                c1 1.000   c2 1.06 (library layers, criterion 2 alone)
+    dgamma / dbeta (check_sums)                                 c1 0.06
+    saved statistics, staged / vs exact                         c1 0.50 / 0.10
+    running statistics, staged / vs exact                       c1 0.17 / 0.08
+    pools, global pool backward                                 c1 1.000   c2 1.00
 c1 sits at 1 because a correctly rounded element near a rounding midpoint has an error of half an ulp.
 
 Set ``EDL_F64_BOUNDS_LOG`` to a file name to append one JSON line per check with both ratios."""
@@ -485,6 +495,26 @@ def check_bn_stats_e2e(x, mean, rstd, eps, tau_s, what=""):
     r1 = check_interval(mean, mu - dmu, mu + dmu, what=what + " mean vs exact")
     lo, hi = _rstd_interval(var, dvar, f32(eps))
     r2 = check_interval(rstd, lo, hi, what=what + " rstd vs exact")
+    return r1, r2
+
+
+def check_bn_running_e2e(x, rm0, rv0, rm, rv, momentum, tau_s, what=""):
+    """The running statistics after ONE momentum update from ``(rm0, rv0)`` against the exact batch statistics of ``x``,
+    through the bound of ``check_bn_stats_e2e`` (for a path whose per-channel sums cannot be read).  A second update (a
+    recomputed forward that updates them again) or none at all fails.  Returns the ratios (mean, var)."""
+    mu, var, a, q = bn_exact_stats(x)
+    m = rows(x).shape[0]
+    dmu = tau_s * a + EPS32 * mu.abs()
+    dvar = tau_s * q + 2 * mu.abs() * dmu + dmu * dmu + 3 * EPS32 * (q + mu * mu)
+    mom = f32(momentum)
+    one_m = f32(1.0 - mom)
+    ratio = m / (m - 1) if m > 1 else 1.0
+    a0, b = one_m * rm0.double().to(mu.device), mom * mu
+    slack = 3 * EPS32 * (a0.abs() + b.abs()) + mom * dmu
+    r1 = check_interval(rm, a0 + b - slack, a0 + b + slack, what=what + " running mean vs exact")
+    a0, b = one_m * rv0.double().to(mu.device), mom * ratio * var
+    slack = 4 * EPS32 * (a0.abs() + b.abs()) + mom * ratio * dvar
+    r2 = check_interval(rv, a0 + b - slack, a0 + b + slack, what=what + " running var vs exact")
     return r1, r2
 
 
