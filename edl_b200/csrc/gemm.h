@@ -51,6 +51,9 @@ struct GemmArgs {
   const void* add_src = nullptr;
   int64_t ld_add = 0;
   BnBwdFuse bn;                        // bn.x != nullptr enables the fused BN-backward reduction (row pitch = ldd)
+  // D = gelu(A*B^T * col_scale + col_shift), erf form, fp32 (inference; B K-major, no addend / ReLU / statistics).
+  // Persistent kernel only.
+  bool gelu = false;
   // fused "GEMM -> peer ship" (EPI 0 only): D may be a PEER GPU's buffer (NVLink-mapped address);
   // every CTA TMA-stores its tile there, and the CTA that completes last publishes
   // *ship_flag (peer address) = seq with release/system semantics -- no separate copy kernel.

@@ -100,6 +100,23 @@ void gemm_bf16(const Tensor& A, const Tensor& B, const Tensor& D, bool a_mn_majo
   TORCH_CHECK(err == nullptr, "edl gemm_bf16 failed: ", err);
 }
 
+// D[M,N] = gelu(A * B^T * col_scale + col_shift) (erf form, fp32) on the persistent kernel's GELU epilogue; inference only.
+void gemm_bf16_gelu(const Tensor& A, const Tensor& B, const Tensor& D, const c10::optional<Tensor>& col_scale,
+                    const c10::optional<Tensor>& col_shift) {
+  edl::GemmArgs g = gemm_operands(A, B, false, false);
+  TORCH_CHECK(D.scalar_type() == at::kBFloat16);
+  TORCH_CHECK(D.dim() == 2 && D.size(0) == g.M && D.size(1) == g.N && D.stride(1) == 1);
+  g.D = D.data_ptr();
+  g.ldd = D.stride(0);
+  TORCH_CHECK(g.ldd % 8 == 0 && reinterpret_cast<uintptr_t>(g.D) % 16 == 0);
+  g.col_scale = optp<float>(col_scale);
+  g.col_shift = optp<float>(col_shift);
+  g.gelu = true;
+  c10::cuda::CUDAGuard guard(A.device());
+  const char* err = edl::gemm_bf16(g, at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl gemm_bf16_gelu failed: ", err);
+}
+
 // fp32 scratch for the partial tiles of a split reduction (optional: the kernels report it missing or too small)
 void set_partials(const c10::optional<Tensor>& partials, float** ptr, int64_t* elems) {
   if (!partials.has_value() || !partials->defined()) return;
@@ -510,6 +527,7 @@ void conv3x3_infer(const Tensor& x, const Tensor& w, Tensor& y, const c10::optio
 
 void register_gemm_bindings(pybind11::module_& m) {
   m.def("gemm_bf16", &gemm_bf16);
+  m.def("gemm_bf16_gelu", &gemm_bf16_gelu);
   m.def("gemm_wgrad_bf16", &gemm_wgrad_bf16);
   m.def("conv3x3", &conv3x3);
   m.def("set_persistent_gemm", &edl::set_persistent_gemm);

@@ -138,7 +138,9 @@ EDL_DEVICE void issue_bn_tiles(const PersistParams& p, int tm, int nn0, int rows
   __syncwarp();
 }
 
-template <int BLOCK_N, int STAGES, int MODE, int BNR, int ASTAGES, int EPIW>
+// GELU: inference epilogue y = gelu(acc * scale + shift) with the erf form 0.5 v (1 + erf(v / sqrt 2)) in fp32 (the
+// FFN1 GEMM of a Transformer encoder, bias in col_shift).  A compile-time switch: the other instantiations are unchanged.
+template <int BLOCK_N, int STAGES, int MODE, int BNR, int ASTAGES, int EPIW, bool GELU = false>
 __global__ void __launch_bounds__(128 + EPIW * 32, 1)
 gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmAdd,
@@ -571,6 +573,10 @@ gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 #pragma unroll
             for (int e = 0; e < 4; ++e) v[e] = fmaxf(v[e], 0.f);
           }
+          if constexpr (GELU) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) v[e] = 0.5f * v[e] * (1.f + erff(v[e] * 0.70710678118654752f));
+          }
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -868,14 +874,14 @@ bool g_epi16 = [] {
   return e != nullptr && e[0] == '1' && e[1] == '6';
 }();
 
-template <int BLOCK_N, int STAGES, int MODE, int BNR, int ASTAGES, int EPIW>
+template <int BLOCK_N, int STAGES, int MODE, int BNR, int ASTAGES, int EPIW, bool GELU>
 const char* launch_pe(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const PersistParams& p,
                      cudaStream_t stream, const CUtensorMap* tmAdd = nullptr, const CUtensorMap* tmBnX = nullptr,
                      const CUtensorMap* tmBnY = nullptr) {
   using L = PSmem<BLOCK_N, STAGES, BNR, ASTAGES>;
   static_assert(L::kTotal <= 227 * 1024, "shared memory budget");
   constexpr int kThreads = 128 + EPIW * 32;
-  auto kern = gemm_persist_kernel<BLOCK_N, STAGES, MODE, BNR, ASTAGES, EPIW>;
+  auto kern = gemm_persist_kernel<BLOCK_N, STAGES, MODE, BNR, ASTAGES, EPIW, GELU>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal);
@@ -893,14 +899,15 @@ const char* launch_pe(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUte
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
-template <int BLOCK_N, int STAGES, int MODE, int BNR = 0, int ASTAGES = 0>
+template <int BLOCK_N, int STAGES, int MODE, int BNR = 0, int ASTAGES = 0, bool GELU = false>
 const char* launch_p(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const PersistParams& p,
                      cudaStream_t stream, const CUtensorMap* tmAdd = nullptr, const CUtensorMap* tmBnX = nullptr,
                      const CUtensorMap* tmBnY = nullptr) {
   if constexpr (BLOCK_N >= 128) {
-    if (g_epi16) return launch_pe<BLOCK_N, STAGES, MODE, BNR, ASTAGES, 16>(tmA, tmB, tmD, p, stream, tmAdd, tmBnX, tmBnY);
+    if (g_epi16)
+      return launch_pe<BLOCK_N, STAGES, MODE, BNR, ASTAGES, 16, GELU>(tmA, tmB, tmD, p, stream, tmAdd, tmBnX, tmBnY);
   }
-  return launch_pe<BLOCK_N, STAGES, MODE, BNR, ASTAGES, 8>(tmA, tmB, tmD, p, stream, tmAdd, tmBnX, tmBnY);
+  return launch_pe<BLOCK_N, STAGES, MODE, BNR, ASTAGES, 8, GELU>(tmA, tmB, tmD, p, stream, tmAdd, tmBnX, tmBnY);
 }
 
 const char* tmap2d(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t outer, uint64_t pitch_elems,
@@ -936,7 +943,8 @@ const char* gemm_bf16_persistent(const GemmArgs& g, cudaStream_t stream) {
   // a 128 x 128 tile needs 32 KB of operands per 256 tensor-core cycles = 128 B / clk / SM, about twice what the
   // L2 -> SM path delivers when every SM pulls; with N = 256 the
   // A tile is reused twice as often and the requirement drops to 96 B / clk.
-  const bool wide = g_wide_tiles && !g.b_mn_major && g.bn.x == nullptr && g.col_stats == nullptr && g.N % 256 == 0 &&
+  // (not with the GELU epilogue: with the erf expansion the 256-column tile spills its accumulators)
+  const bool wide = g_wide_tiles && !g.gelu && !g.b_mn_major && g.bn.x == nullptr && g.col_stats == nullptr && g.N % 256 == 0 &&
                     g.K >= 256 &&
                     (int64_t)((g.M + kBlockM - 1) / kBlockM) * (g.N / 256) >= kNumSMs;
   const int bn = n64 ? 64 : (wide ? 256 : 128);
@@ -986,6 +994,11 @@ const char* gemm_bf16_persistent(const GemmArgs& g, cudaStream_t stream) {
     const CUtensorMap* pby = (has_y || has_mask) ? &tmBy : nullptr;
     return n64 ? launch_p<64, 4, 1, 2>(tmA, tmB, tmD, p, stream, padd, &tmBx, pby)
                : launch_p<128, 3, 1, 2>(tmA, tmB, tmD, p, stream, padd, &tmBx, pby);
+  }
+  if (g.gelu) {
+    if (g.b_mn_major || g.add_src != nullptr || g.col_stats != nullptr || g.relu)
+      return "gemm GELU epilogue: forward GEMM (B K-major) with an optional scale / shift only";
+    return n64 ? launch_p<64, 6, 0, 0, 0, true>(tmA, tmB, tmD, p, stream) : launch_p<128, 5, 0, 0, 0, true>(tmA, tmB, tmD, p, stream);
   }
   if (!g.b_mn_major) {
     if (wide) return launch_p<256, 3, 0>(tmA, tmB, tmD, p, stream, padd);

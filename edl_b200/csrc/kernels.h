@@ -206,4 +206,23 @@ void slot_ack(void* ack_peer, const void* seq_ptr, uint32_t seq_imm, cudaStream_
 void wait_flag_async(const void* flag, const void* seq_ptr, uint32_t seq_imm, double timeout_s, void* err,
                      cudaStream_t s);
 
+// ---- attention.cu / layernorm.cu: the Transformer encoder of the NLP teacher (inference) ----
+constexpr int kAttnMaxLen = 512;
+bool attention_supported(int B, int L, int H, int head_dim);
+// qkv bf16 [B * L, 3 * H * 64] (Q | K | V column blocks, 16-byte aligned), mask uint8 [B, L] (1 = attend; nullptr: all),
+// out bf16 [B * L, H * 64].  Returns nullptr or an error string.
+const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream);
+constexpr int kLnMaxC = 1024;
+bool layernorm_supported(int C);
+// y[r] = (x[r] - mean) * rsqrt(var + eps) * gamma + beta over the C columns of each row; x, y bf16 [rows, C] (row pitch
+// C), gamma / beta fp32 [C]; statistics in fp32
+void layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y, int64_t rows, int C, float eps,
+                   cudaStream_t s);
+// the same over x[r] = word[ids[r]] + pos[pos_ids[r]] + seg[seg_ids[r]] (bf16 tables [*, C], sum in fp32).  An id
+// outside its table reads nothing (the row sums the other tables) and sets *err to 1.
+void embedding_layernorm_fwd(const int64_t* ids, const int64_t* pos_ids, const int64_t* seg_ids, const void* word,
+                             int64_t n_word, const void* pos, int64_t n_pos, const void* seg, int64_t n_seg,
+                             const float* gamma, const float* beta, void* y, int64_t rows, int C, float eps, int* err,
+                             cudaStream_t s);
+
 }  // namespace edl

@@ -1,0 +1,82 @@
+// torch bindings for the Transformer encoder kernels (attention.cu, layernorm.cu).
+#include <ATen/cuda/CUDAContext.h>
+#include <c10/cuda/CUDAGuard.h>
+#include <torch/extension.h>
+
+#include "kernels.h"
+
+namespace {
+using torch::Tensor;
+
+void check_bf16_2d(const Tensor& t, const char* name) {
+  TORCH_CHECK(t.is_cuda() && t.dim() == 2 && t.scalar_type() == at::kBFloat16 && t.is_contiguous(), name,
+              " must be a contiguous 2-D bf16 CUDA tensor");
+}
+
+// qkv [B * L, 3 * H * 64], mask uint8 [B, L] or None, out [B * L, H * 64]
+void attention_fwd(const Tensor& qkv, const c10::optional<Tensor>& mask, Tensor& out, int64_t B, int64_t L, int64_t H) {
+  check_bf16_2d(qkv, "qkv");
+  check_bf16_2d(out, "out");
+  TORCH_CHECK(qkv.size(0) == B * L && qkv.size(1) == 3 * H * 64, "qkv must be [B * L, 3 * H * 64]");
+  TORCH_CHECK(out.size(0) == B * L && out.size(1) == H * 64, "out must be [B * L, H * 64]");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0);
+  const uint8_t* mp = nullptr;
+  if (mask.has_value() && mask->defined()) {
+    TORCH_CHECK(mask->is_cuda() && mask->scalar_type() == at::kByte && mask->is_contiguous() && mask->numel() == B * L,
+                "mask must be a contiguous uint8 [B, L] CUDA tensor");
+    mp = mask->data_ptr<uint8_t>();
+  }
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const char* err = edl::attention_fwd(qkv.data_ptr(), mp, out.data_ptr(), (int)B, (int)L, (int)H,
+                                       at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl attention_fwd failed: ", err);
+}
+
+void check_affine(const Tensor& g, const Tensor& b, int64_t C) {
+  TORCH_CHECK(g.is_cuda() && g.scalar_type() == at::kFloat && g.is_contiguous() && g.numel() == C, "gamma: fp32 [C]");
+  TORCH_CHECK(b.is_cuda() && b.scalar_type() == at::kFloat && b.is_contiguous() && b.numel() == C, "beta: fp32 [C]");
+}
+
+void layernorm_fwd(const Tensor& x, const Tensor& gamma, const Tensor& beta, Tensor& y, double eps) {
+  check_bf16_2d(x, "x");
+  check_bf16_2d(y, "y");
+  const int64_t C = x.size(1);
+  TORCH_CHECK(edl::layernorm_supported((int)C) && y.sizes() == x.sizes(), "layernorm: C % 8 == 0, 8 <= C <= 1024");
+  check_affine(gamma, beta, C);
+  c10::cuda::CUDAGuard guard(x.device());
+  edl::layernorm_fwd(x.data_ptr(), gamma.data_ptr<float>(), beta.data_ptr<float>(), y.data_ptr(), x.size(0), (int)C,
+                     (float)eps, at::cuda::getCurrentCUDAStream().stream());
+}
+
+void embedding_layernorm_fwd(const Tensor& ids, const Tensor& pos_ids, const Tensor& seg_ids, const Tensor& word,
+                             const Tensor& pos, const Tensor& seg, const Tensor& gamma, const Tensor& beta, Tensor& y,
+                             double eps, Tensor& err) {
+  const int64_t rows = ids.numel();
+  for (const Tensor* t : {&ids, &pos_ids, &seg_ids})
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kLong && t->is_contiguous() && t->numel() == rows,
+                "ids: contiguous int64 CUDA tensors of one size");
+  check_bf16_2d(word, "word");
+  check_bf16_2d(pos, "pos");
+  check_bf16_2d(seg, "seg");
+  check_bf16_2d(y, "y");
+  const int64_t C = word.size(1);
+  TORCH_CHECK(edl::layernorm_supported((int)C) && pos.size(1) == C && seg.size(1) == C && y.size(0) == rows &&
+              y.size(1) == C, "embedding_layernorm: tables and output of one width C, C % 8 == 0, 8 <= C <= 1024");
+  check_affine(gamma, beta, C);
+  TORCH_CHECK(err.is_cuda() && err.scalar_type() == at::kInt && err.numel() >= 1, "err: int32 CUDA flag");
+  c10::cuda::CUDAGuard guard(ids.device());
+  edl::embedding_layernorm_fwd(ids.data_ptr<int64_t>(), pos_ids.data_ptr<int64_t>(), seg_ids.data_ptr<int64_t>(),
+                               word.data_ptr(), word.size(0), pos.data_ptr(), pos.size(0), seg.data_ptr(), seg.size(0),
+                               gamma.data_ptr<float>(), beta.data_ptr<float>(), y.data_ptr(), rows, (int)C, (float)eps,
+                               err.data_ptr<int>(), at::cuda::getCurrentCUDAStream().stream());
+}
+
+}  // namespace
+
+void register_transformer_bindings(pybind11::module_& m) {
+  m.def("attention_fwd", &attention_fwd);
+  m.def("attention_supported", &edl::attention_supported);
+  m.def("layernorm_fwd", &layernorm_fwd);
+  m.def("layernorm_supported", &edl::layernorm_supported);
+  m.def("embedding_layernorm_fwd", &embedding_layernorm_fwd);
+}

@@ -156,7 +156,10 @@ def build_model(name):
 
 def main(argv=None):
     ap = argparse.ArgumentParser(description="EDL teacher inference server")
-    ap.add_argument("--model", required=True, help="teacher_zoo name, e.g. resnext101_32x16d / mnist_cnn")
+    ap.add_argument("--model", required=True, help="teacher_zoo name, e.g. resnext101_32x16d / mnist_cnn / ernie_base")
+    ap.add_argument("--weights", default=None,
+                    help="state dict to load (.safetensors or a torch file); sequence teachers take the BERT layout. "
+                         "Without it the weights are random")
     ap.add_argument("--port", type=int, default=9292)
     ap.add_argument("--gpu_ids", type=str, default="0")
     ap.add_argument("--thread", type=int, default=4)
@@ -170,6 +173,14 @@ def main(argv=None):
     logging.basicConfig(level=logging.INFO)
     dev = "cuda:%s" % args.gpu_ids.split(",")[0] if torch.cuda.is_available() else "cpu"
     model, feed_names, fetch_names, feed_shapes = build_model(args.model)
+    if args.weights:
+        net = getattr(model, "net", model)
+        if hasattr(net, "load_weights"):
+            unused = net.load_weights(args.weights)
+            logging.info("loaded %s (%d unused entries)", args.weights, len(unused))
+        else:
+            sd = torch.load(args.weights, map_location="cpu", weights_only=True)
+            net.load_state_dict(sd.get("state_dict", sd))
     dtype = torch.bfloat16 if dev.startswith("cuda") else torch.float32
     srv = TeacherServer(model, feed_names, fetch_names, feed_shapes, device=dev, dtype=dtype, port=args.port,
                         max_batch=args.max_batch, workers=max(4, args.thread))

@@ -1,0 +1,196 @@
+"""ERNIE 1.0 / BERT-style encoder for sequence classification, the NLP teacher of the ERNIE -> BOW distillation
+(the reference serves ERNIE 1.0 base with Paddle Serving; example/distill/nlp).
+
+Post-LN Transformer layers: QKV projection, masked multi-head attention, output projection + residual, LayerNorm,
+FFN1 with bias + erf-GELU, FFN2 + residual, LayerNorm; the [CLS] row goes through a tanh pooler and the classifier.
+Inference only.
+
+On CUDA every layer runs on the package's own kernels: the wgmma GEMM (bias in the epilogue, the residual as its fused
+addend, GELU as a compile-time epilogue variant), the attention kernel reading Q / K / V in place from the QKV output,
+the LayerNorm and the embedding-sum + LayerNorm kernels.  The weight matrices are cast to bf16 once, at the first CUDA
+forward after a load or a move; biases and LayerNorm parameters stay fp32.  On CPU the same forward runs in float32
+PyTorch math (the reference the GPU path is tested against)."""
+from __future__ import annotations
+
+import torch
+import torch.nn as nn
+import torch.nn.functional as F
+
+from .. import ops
+
+CLS_PAD = 8      # classifier rows after padding: a 2-class output row (4 bytes) is not a TMA-describable pitch
+
+
+class ErnieEncoder(nn.Module):
+    def __init__(self, vocab=18000, hidden=768, layers=12, heads=12, ffn=3072, max_pos=513, type_vocab=2,
+                 num_labels=2, eps=1e-12):
+        super().__init__()
+        if hidden % heads != 0:
+            raise ValueError("hidden %d is not a multiple of heads %d" % (hidden, heads))
+        self.hidden, self.heads, self.head_dim, self.num_labels, self.eps = hidden, heads, hidden // heads, num_labels, eps
+        self.num_layers = layers
+        std = 0.02
+
+        def mat(*shape):
+            return nn.Parameter(torch.randn(*shape) * std)
+
+        def vec(n, value=0.0):
+            return nn.Parameter(torch.full((n,), float(value)))
+
+        self.word_emb, self.pos_emb, self.seg_emb = mat(vocab, hidden), mat(max_pos, hidden), mat(type_vocab, hidden)
+        self.emb_ln_g, self.emb_ln_b = vec(hidden, 1.0), vec(hidden)
+        self.layers = nn.ModuleList()
+        for _ in range(layers):
+            lyr = nn.Module()
+            lyr.qkv_w, lyr.qkv_b = mat(3 * hidden, hidden), vec(3 * hidden)
+            lyr.out_w, lyr.out_b = mat(hidden, hidden), vec(hidden)
+            lyr.ln1_g, lyr.ln1_b = vec(hidden, 1.0), vec(hidden)
+            lyr.ffn1_w, lyr.ffn1_b = mat(ffn, hidden), vec(ffn)
+            lyr.ffn2_w, lyr.ffn2_b = mat(hidden, ffn), vec(hidden)
+            lyr.ln2_g, lyr.ln2_b = vec(hidden, 1.0), vec(hidden)
+            self.layers.append(lyr)
+        self.pool_w, self.pool_b = mat(hidden, hidden), vec(hidden)
+        self.cls_w, self.cls_b = mat(num_labels, hidden), vec(num_labels)
+        self.requires_grad_(False)
+        self._dev = None          # CUDA copies of the weights (bf16 matrices, fp32 vectors), built at first use
+
+    def _apply(self, fn, *args, **kwargs):
+        self._dev = None
+        return super()._apply(fn, *args, **kwargs)
+
+    # ------------------------------------------------------------------------------------------------- weights
+    def _device_weights(self):
+        if self._dev is None:
+            def m(t):
+                return t.detach().to(torch.bfloat16).contiguous()
+
+            def v(t):
+                return t.detach().float().contiguous()
+
+            n, c = self.num_labels, self.hidden
+            cls_w = torch.zeros(max(CLS_PAD, -(-n // CLS_PAD) * CLS_PAD), c, device=self.cls_w.device)
+            cls_w[:n] = self.cls_w.detach().float()
+            cls_b = torch.zeros(cls_w.shape[0], device=self.cls_w.device)
+            cls_b[:n] = self.cls_b.detach().float()
+            self._dev = {
+                "emb": (m(self.word_emb), m(self.pos_emb), m(self.seg_emb), v(self.emb_ln_g), v(self.emb_ln_b)),
+                "layers": [tuple(f(getattr(lyr, k)) for f, k in (
+                    (m, "qkv_w"), (v, "qkv_b"), (m, "out_w"), (v, "out_b"), (v, "ln1_g"), (v, "ln1_b"),
+                    (m, "ffn1_w"), (v, "ffn1_b"), (m, "ffn2_w"), (v, "ffn2_b"), (v, "ln2_g"), (v, "ln2_b")))
+                    for lyr in self.layers],
+                "head": (m(self.pool_w), v(self.pool_b), m(cls_w), v(cls_b)),
+            }
+        return self._dev
+
+    def load_bert_state_dict(self, sd, strict=True):
+        """Load a BERT-layout state dict (``[bert.]embeddings.*``, ``[bert.]encoder.layer.N.*``, ``[bert.]pooler.*``
+        and optionally ``classifier.*``; LayerNorm ``weight``/``bias`` or ``gamma``/``beta``).  Returns the names that
+        were not used.  ``strict``: every encoder tensor must be present with the model's shape."""
+        src = {}
+        for k, t in sd.items():
+            k = k[len("bert."):] if k.startswith("bert.") else k
+            src[k.replace("LayerNorm.gamma", "LayerNorm.weight").replace("LayerNorm.beta", "LayerNorm.bias")] = t
+        used = set()
+
+        def take(name):
+            if name not in src:
+                raise KeyError("BERT state dict has no %r" % name)
+            used.add(name)
+            return src[name]
+
+        def put(param, value):
+            value = torch.as_tensor(value)
+            if tuple(value.shape) != tuple(param.shape):
+                raise ValueError("shape mismatch: %s for a parameter of %s" % (tuple(value.shape), tuple(param.shape)))
+            param.data.copy_(value.to(param.dtype))
+
+        e = "embeddings."
+        put(self.word_emb, take(e + "word_embeddings.weight"))
+        put(self.pos_emb, take(e + "position_embeddings.weight"))
+        put(self.seg_emb, take(e + "token_type_embeddings.weight"))
+        put(self.emb_ln_g, take(e + "LayerNorm.weight"))
+        put(self.emb_ln_b, take(e + "LayerNorm.bias"))
+        for i, lyr in enumerate(self.layers):
+            p = "encoder.layer.%d." % i
+            a = p + "attention.self."
+            put(lyr.qkv_w, torch.cat([torch.as_tensor(take(a + n + ".weight")) for n in ("query", "key", "value")], 0))
+            put(lyr.qkv_b, torch.cat([torch.as_tensor(take(a + n + ".bias")) for n in ("query", "key", "value")], 0))
+            put(lyr.out_w, take(p + "attention.output.dense.weight"))
+            put(lyr.out_b, take(p + "attention.output.dense.bias"))
+            put(lyr.ln1_g, take(p + "attention.output.LayerNorm.weight"))
+            put(lyr.ln1_b, take(p + "attention.output.LayerNorm.bias"))
+            put(lyr.ffn1_w, take(p + "intermediate.dense.weight"))
+            put(lyr.ffn1_b, take(p + "intermediate.dense.bias"))
+            put(lyr.ffn2_w, take(p + "output.dense.weight"))
+            put(lyr.ffn2_b, take(p + "output.dense.bias"))
+            put(lyr.ln2_g, take(p + "output.LayerNorm.weight"))
+            put(lyr.ln2_b, take(p + "output.LayerNorm.bias"))
+        put(self.pool_w, take("pooler.dense.weight"))
+        put(self.pool_b, take("pooler.dense.bias"))
+        if "classifier.weight" in src:
+            put(self.cls_w, take("classifier.weight"))
+            put(self.cls_b, take("classifier.bias"))
+        if strict and "encoder.layer.%d.attention.self.query.weight" % self.num_layers in src:
+            raise ValueError("the state dict has more than %d encoder layers" % self.num_layers)
+        self._dev = None
+        return sorted(set(src) - used)
+
+    def load_weights(self, path, strict=True):
+        """``load_bert_state_dict`` from a ``.safetensors`` file or a torch-saved state dict."""
+        if str(path).endswith(".safetensors"):
+            from safetensors.torch import load_file
+
+            sd = load_file(str(path))
+        else:
+            sd = torch.load(str(path), map_location="cpu", weights_only=True)
+            sd = sd.get("state_dict", sd) if isinstance(sd, dict) else sd
+        return self.load_bert_state_dict(sd, strict=strict)
+
+    # ------------------------------------------------------------------------------------------------- forward
+    @torch.no_grad()
+    def forward(self, input_ids, position_ids, segment_ids, input_mask):
+        """ids int64 [B, L]; ``input_mask`` [B, L], nonzero = a real token.  Returns fp32 logits [B, num_labels]."""
+        b, l = input_ids.shape[0], input_ids.shape[1]
+        ids, pos, seg = (t.reshape(b, l).long() for t in (input_ids, position_ids, segment_ids))
+        keep = input_mask.reshape(b, l) != 0
+        if self.word_emb.is_cuda:
+            return self._forward_cuda(ids, pos, seg, keep.to(torch.uint8).contiguous(), b, l)
+        return self._forward_reference(ids, pos, seg, keep, b, l)
+
+    def _forward_cuda(self, ids, pos, seg, mask, b, l):
+        w = self._device_weights()
+        word, pemb, semb, g, beta = w["emb"]
+        x = ops.embedding_layernorm(ids, pos, seg, word, pemb, semb, g, beta, self.eps)
+        for qkv_w, qkv_b, out_w, out_b, ln1_g, ln1_b, f1_w, f1_b, f2_w, f2_b, ln2_g, ln2_b in w["layers"]:
+            qkv = ops.gemm_bf16(x, qkv_w, col_shift=qkv_b)
+            ctx = ops.attention(qkv, mask, b, l, self.heads, self.head_dim)
+            x = ops.layer_norm(ops.gemm_bf16(ctx, out_w, col_shift=out_b, add=x), ln1_g, ln1_b, self.eps)
+            f = ops.gemm_bf16(x, f1_w, col_shift=f1_b, gelu=True)
+            x = ops.layer_norm(ops.gemm_bf16(f, f2_w, col_shift=f2_b, add=x), ln2_g, ln2_b, self.eps)
+        pool_w, pool_b, cls_w, cls_b = w["head"]
+        cls_rows = x.view(b, l, self.hidden)[:, 0]                  # [B, C], row pitch L * C
+        pooled = torch.tanh(ops.linear_bf16(cls_rows, pool_w, pool_b))
+        return ops.gemm_bf16(pooled, cls_w, col_shift=cls_b)[:, :self.num_labels].float()
+
+    def _forward_reference(self, ids, pos, seg, keep, b, l):
+        f32 = torch.float32
+        x = ops.embedding_layernorm(ids, pos, seg, self.word_emb.to(f32), self.pos_emb.to(f32), self.seg_emb.to(f32),
+                                    self.emb_ln_g, self.emb_ln_b, self.eps)
+        for lyr in self.layers:
+            qkv = F.linear(x, lyr.qkv_w.to(f32), lyr.qkv_b.to(f32))
+            ctx = ops.attention(qkv, keep, b, l, self.heads, self.head_dim)
+            x = ops.layer_norm(F.linear(ctx, lyr.out_w.to(f32), lyr.out_b.to(f32)) + x, lyr.ln1_g, lyr.ln1_b, self.eps)
+            f = F.gelu(F.linear(x, lyr.ffn1_w.to(f32), lyr.ffn1_b.to(f32)))
+            x = ops.layer_norm(F.linear(f, lyr.ffn2_w.to(f32), lyr.ffn2_b.to(f32)) + x, lyr.ln2_g, lyr.ln2_b, self.eps)
+        pooled = torch.tanh(F.linear(x.view(b, l, self.hidden)[:, 0], self.pool_w.to(f32), self.pool_b.to(f32)))
+        return F.linear(pooled, self.cls_w.to(f32), self.cls_b.to(f32))
+
+
+def ernie_base(num_labels=2):
+    """ERNIE 1.0 base: vocabulary 18000, hidden 768, 12 layers, 12 heads, FFN 3072, 513 positions, 2 segment types."""
+    return ErnieEncoder(18000, 768, 12, 12, 3072, 513, 2, num_labels)
+
+
+def ernie_tiny(num_labels=2):
+    """A 2-layer, 128-wide configuration with the same structure (tests, examples)."""
+    return ErnieEncoder(1000, 128, 2, 2, 512, 513, 2, num_labels)

@@ -15,7 +15,7 @@ _NUM_SMS = 132
 
 
 def gemm_bf16(a, b, out=None, a_mn_major=False, b_mn_major=False, col_scale=None, col_shift=None,
-              relu=False, col_stats=None, add=None, bn=None):
+              relu=False, col_stats=None, add=None, bn=None, gelu=False):
     """D = op(A) @ op(B): see csrc/gemm.h for the operand conventions.  The weight-gradient form (both operands
     MN-major) is ``_wgrad_impl``.
 
@@ -24,9 +24,17 @@ def gemm_bf16(a, b, out=None, a_mn_major=False, b_mn_major=False, col_scale=None
     a_mn_major     : A [K, M]            -> D = A^T @ op(B)
     add given      : D = result + add (bf16 [M, N]) in the epilogue (gradient accumulation fused into dgrad).
     bn given       : a ``BNBackwardHook`` (ops/bn.py): D is the gradient of that BatchNorm's output and the
-                     epilogue accumulates its backward reduction (sum dy, sum dy * xhat) into hook.dsums."""
+                     epilogue accumulates its backward reduction (sum dy, sum dy * xhat) into hook.dsums.
+    gelu           : D = gelu(A @ B^T * col_scale + col_shift) with the erf form in fp32 (inference; both operands
+                     K-major, no addend / ReLU / statistics)."""
     from . import native, count_launch
 
+    if gelu and (a_mn_major or b_mn_major or add is not None or relu or col_stats is not None or bn is not None):
+        raise ValueError("gemm_bf16: the GELU epilogue is a forward GEMM with an optional scale / shift only")
+    if gelu and a.is_cuda and _tma_compatible(a, b, out, b.shape[0]) and not native().persistent_gemm_enabled():
+        from . import count_fallback
+        count_fallback("gemm_bf16: the GELU epilogue needs the persistent GEMM (disabled): fp32 matmul on the library")
+        return _gemm_reference(a, b, out, False, False, col_scale, col_shift, False, None, None, True)
     m = a.shape[1] if a_mn_major else a.shape[0]
     n = b.shape[1] if b_mn_major else b.shape[0]
     if not a.is_cuda or not _tma_compatible(a, b, out, n):
@@ -36,27 +44,13 @@ def gemm_bf16(a, b, out=None, a_mn_major=False, b_mn_major=False, col_scale=None
             from . import count_fallback
             count_fallback("gemm_bf16: operand not TMA-describable (pitch / base not 16-byte aligned or not bf16): "
                            "fp32 matmul on the library, %s x %s" % (tuple(a.shape), tuple(b.shape)))
-        af = a.float().t() if a_mn_major else a.float()
-        bf = b.float() if b_mn_major else b.float().t()
-        d = af @ bf
-        if add is not None:
-            d = d + add.float()
-        if col_scale is not None:
-            d = d * col_scale.float()
-        if col_shift is not None:
-            d = d + col_shift.float()
-        if relu:
-            d = torch.relu(d)
-        d = d.to(torch.bfloat16)
-        if col_stats is not None:
-            col_stats[:n] += d.float().sum(0)
-            col_stats[n:] += (d.float() ** 2).sum(0)
-        if out is not None:
-            out.copy_(d)
-            return out
-        return d
+        return _gemm_reference(a, b, out, a_mn_major, b_mn_major, col_scale, col_shift, relu, col_stats, add, gelu)
     if out is None:
         out = torch.empty((m, n), device=a.device, dtype=torch.bfloat16)
+    if gelu:
+        native().gemm_bf16_gelu(a, b, out, col_scale, col_shift)
+        count_launch()
+        return out
     if add is not None and not (native().persistent_gemm_enabled() and n % 8 == 0 and add.stride(-1) == 1
                                 and add.stride(0) % 8 == 0 and add.data_ptr() % 16 == 0):
         # the fused addend lives in the persistent kernel's epilogue; otherwise one extra elementwise pass, which is
@@ -74,6 +68,32 @@ def gemm_bf16(a, b, out=None, a_mn_major=False, b_mn_major=False, col_scale=None
     if bn is not None:
         bn.done = True
     return out
+
+
+def _gemm_reference(a, b, out, a_mn_major, b_mn_major, col_scale, col_shift, relu, col_stats, add, gelu):
+    """gemm_bf16's semantics in fp32 PyTorch math (CPU tensors, shapes TMA cannot describe)."""
+    n = b.shape[1] if b_mn_major else b.shape[0]
+    af = a.float().t() if a_mn_major else a.float()
+    bf = b.float() if b_mn_major else b.float().t()
+    d = af @ bf
+    if add is not None:
+        d = d + add.float()
+    if col_scale is not None:
+        d = d * col_scale.float()
+    if col_shift is not None:
+        d = d + col_shift.float()
+    if relu:
+        d = torch.relu(d)
+    if gelu:
+        d = torch.nn.functional.gelu(d)
+    d = d.to(torch.bfloat16)
+    if col_stats is not None:
+        col_stats[:n] += d.float().sum(0)
+        col_stats[n:] += (d.float() ** 2).sum(0)
+    if out is not None:
+        out.copy_(d)
+        return out
+    return d
 
 
 def _tma_compatible(a, b, out, n):
@@ -338,9 +358,14 @@ class _LinearFn(torch.autograd.Function):
         return dx, dw, db, None, None, None, None, None
 
 
-def linear_bf16(x, weight, bias=None, relu=False):
+def linear_bf16(x, weight, bias=None, relu=False, gelu=False):
     """y = act(x @ weight^T + bias) on the wgmma GEMM (bias/activation fused in the epilogue).
-    x [M, K] bf16, weight [N, K] bf16, bias [N] (any float dtype)."""
+    x [M, K] bf16, weight [N, K] bf16, bias [N] (any float dtype).  ``gelu``: the erf-form GELU epilogue, inference only
+    (raises when a gradient would be required)."""
+    if gelu:
+        if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, weight, bias)):
+            raise RuntimeError("linear_bf16(gelu=True) is inference only: no backward; run it under torch.no_grad()")
+        return gemm_bf16(x.contiguous(), weight, col_shift=bias.float() if bias is not None else None, gelu=True)
     return _LinearFn.apply(x, weight, bias, relu, *_grad_sink(weight), *_grad_sink(bias))
 
 
