@@ -16,7 +16,16 @@
 // Rows and keys at or past L are zero-filled by the TMA loads, masked as keys and clipped by the TMA store.  A row
 // sum is taken over the bf16-ROUNDED probabilities that enter P V, so O is a convex combination of V rows up to fp32
 // accumulation; a query row without any valid key stores 0.
+//
+// Variable-length batches (attention_varlen_fwd): sequences packed back to back, qkv [T, 3 * H * 64], sequence b in rows
+// [cu_seqlens[b], cu_seqlens[b + 1]).  The rows after a sequence are the next sequence's tokens, so one map over the
+// whole buffer would neither zero-fill nor clip at its end.  A prologue kernel therefore writes each sequence its own
+// pair of maps (tensormap.replace of the global address and the row count of a template map, published with
+// tensormap.cp_fenceproxy); the attention kernel acquires them and runs the same body with L = len_b.  A sequence's
+// output thus depends on its own rows only, whatever the others hold (NaN included), and nothing is stored outside it.
 #include <cuda.h>
+
+#include <type_traits>
 
 #include "gemm.h"
 #include "kernels.h"
@@ -48,9 +57,22 @@ EDL_DEVICE void tma_store_4d(const CUtensorMap* m, const void* smem_src, int c0,
       : "memory");
 }
 
+EDL_DEVICE void acquire_tmap(const CUtensorMap* m) {
+  asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
+}
+
+// Sequence layout of a packed batch: offsets [B + 1] and the per-sequence maps [B][Q/K/V, O] of the prologue.
+struct Varlen {
+  const int* cu_seqlens;
+  const CUtensorMap* maps;
+};
+
+// Seq = int: the padded layout, seq = L for every sequence (tmQKV / tmO span the whole batch).  Seq = Varlen: packed.
+template <typename Seq>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO,
-                     const uint8_t* __restrict__ mask, int L, int H) {
+                     const uint8_t* __restrict__ mask, Seq seq, int H) {
+  constexpr bool kVarlen = std::is_same<Seq, Varlen>::value;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -61,13 +83,33 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
   uint64_t* empty_bar = full_bar + kAttnStages;
 
   const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
+  int L, bc;                                                     // sequence length, batch coordinate in the maps
+  int64_t start;                                                 // first row of a packed sequence
+  const CUtensorMap* mQKV = &tmQKV;
+  const CUtensorMap* mO = &tmO;
+  if constexpr (kVarlen) {
+    start = seq.cu_seqlens[b];
+    L = seq.cu_seqlens[b + 1] - seq.cu_seqlens[b];
+    if (q0 >= L) return;                                         // the grid spans the longest sequence
+    mQKV = seq.maps + 2 * b;
+    mO = mQKV + 1;
+    bc = 0;
+  } else {
+    L = seq;
+    start = 0;                                                   // (b * L, formed at its use)
+    bc = b;
+  }
   const int groups = L - q0 > 64 ? 2 : 1;                       // consumer groups with at least one query row < L
   const int n_kt = (L + 63) / 64;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    ptx::prefetch_tmap(&tmQKV);
-    ptx::prefetch_tmap(&tmO);
+    if constexpr (kVarlen) {
+      acquire_tmap(mQKV);
+      acquire_tmap(mO);
+    }
+    ptx::prefetch_tmap(mQKV);
+    ptx::prefetch_tmap(mO);
     ptx::mbar_init(q_bar, 1);
     for (int s = 0; s < kAttnStages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
@@ -77,14 +119,14 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
   }
   // key validity of the whole row, padded to whole key tiles: keys at or past L are never attended
   for (int j = threadIdx.x; j < n_kt * 64; j += kAttnThreads)
-    smask[j] = (j < L && (mask == nullptr || mask[(int64_t)b * L + j] != 0)) ? 1 : 0;
+    smask[j] = (j < L && (mask == nullptr || mask[kVarlen ? start + j : (int64_t)b * L + j] != 0)) ? 1 : 0;
   __syncthreads();
 
   if (warp == 0) {
     // ------------------------------------------------------------ TMA producer (whole warp loops, one lane issues)
     if (ptx::elect_one()) {
       ptx::mbar_arrive_expect_tx(q_bar, groups * kHalfBytes);
-      for (int g = 0; g < groups; ++g) ptx::tma_load_4d(sq + g * kHalfBytes, &tmQKV, q_bar, 0, h, q0 + g * 64, b);
+      for (int g = 0; g < groups; ++g) ptx::tma_load_4d(sq + g * kHalfBytes, mQKV, q_bar, 0, h, q0 + g * 64, bc);
     }
     __syncwarp();
     for (int kt = 0; kt < n_kt; ++kt) {
@@ -93,8 +135,8 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
       uint8_t* sk = smem + kQBytes + s * kKVBytes;
       if (ptx::elect_one()) {
         ptx::mbar_arrive_expect_tx(&full_bar[s], kKVBytes);
-        ptx::tma_load_4d(sk, &tmQKV, &full_bar[s], 0, H + h, kt * 64, b);
-        ptx::tma_load_4d(sk + kHalfBytes, &tmQKV, &full_bar[s], 0, 2 * H + h, kt * 64, b);
+        ptx::tma_load_4d(sk, mQKV, &full_bar[s], 0, H + h, kt * 64, bc);
+        ptx::tma_load_4d(sk + kHalfBytes, mQKV, &full_bar[s], 0, 2 * H + h, kt * 64, bc);
       }
       __syncwarp();
     }
@@ -193,11 +235,72 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
     ptx::fence_proxy_async_smem();
     asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
     if ((threadIdx.x & 127) == 0) {
-      tma_store_4d(&tmO, st, 0, h, q0 + cw * 64, b);
+      if constexpr (kVarlen) acquire_tmap(mO);
+      tma_store_4d(mO, st, 0, h, q0 + cw * 64, bc);
       ptx::tma_store_commit();
       ptx::tma_store_wait_read0();
     }
   }
+}
+
+// One warp per sequence: copy the template maps to shared memory, point them at the sequence's first row, set their
+// row count to its length, and publish them to maps[2 b], maps[2 b + 1] for the tensor-map proxy.
+__global__ void __launch_bounds__(128)
+attention_varlen_maps_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO,
+                             const void* qkv, void* out, const int* __restrict__ cu_seqlens, CUtensorMap* maps, int B,
+                             int H) {
+  __shared__ alignas(128) CUtensorMap sm[4][2];
+  const int w = threadIdx.x >> 5, b = blockIdx.x * 4 + w;
+  if (b >= B) return;                                           // whole warps
+  CUtensorMap* s = sm[w];
+  if ((threadIdx.x & 31) == 0) {
+    const int start = cu_seqlens[b];
+    const int len = max(cu_seqlens[b + 1] - start, 1);          // a sequence with len < 1 launches no work
+    s[0] = tmQKV;
+    s[1] = tmO;
+    const uint64_t a0 = reinterpret_cast<uint64_t>(qkv) + (uint64_t)start * 3 * H * 128;
+    const uint64_t a1 = reinterpret_cast<uint64_t>(out) + (uint64_t)start * H * 128;
+    asm volatile("tensormap.replace.tile.global_address.shared::cta.b1024.b64 [%0], %1;" ::"r"(ptx::smem_u32(s)),
+                 "l"(a0) : "memory");
+    asm volatile("tensormap.replace.tile.global_address.shared::cta.b1024.b64 [%0], %1;" ::"r"(ptx::smem_u32(s + 1)),
+                 "l"(a1) : "memory");
+    asm volatile("tensormap.replace.tile.global_dim.shared::cta.b1024.b32 [%0], 2, %1;" ::"r"(ptx::smem_u32(s)),
+                 "r"(len) : "memory");
+    asm volatile("tensormap.replace.tile.global_dim.shared::cta.b1024.b32 [%0], 2, %1;" ::"r"(ptx::smem_u32(s + 1)),
+                 "r"(len) : "memory");
+  }
+  __syncwarp();
+  for (int i = 0; i < 2; ++i)
+    asm volatile("tensormap.cp_fenceproxy.global.shared::cta.tensormap::generic.release.gpu.sync.aligned [%0], [%1], 128;"
+                 ::"l"(reinterpret_cast<uint64_t>(maps + 2 * b + i)), "r"(ptx::smem_u32(s + i)) : "memory");
+}
+
+template <typename Seq>
+const char* launch_attention(const CUtensorMap& tmQKV, const CUtensorMap& tmO, const uint8_t* mask, Seq seq, int H,
+                             dim3 grid, cudaStream_t stream) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(attention_fwd_kernel<Seq>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
+    if (e != cudaSuccess) return cudaGetErrorString(e);
+    attr_set = true;
+  }
+  attention_fwd_kernel<Seq><<<grid, kAttnThreads, kAttnSmem, stream>>>(tmQKV, tmO, mask, seq, H);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
+// Q / K / V and O maps {64, 3H | H, rows, batch} of a [batch * rows, 3 * H * 64] / [batch * rows, H * 64] layout
+const char* encode_attention_maps(CUtensorMap* tmQKV, CUtensorMap* tmO, const void* qkv, void* out, int rows, int batch,
+                                  int H) {
+  const uint32_t box[4] = {64, 1, 64, 1};
+  {
+    const uint64_t dims[4] = {64, (uint64_t)3 * H, (uint64_t)rows, (uint64_t)batch};
+    const uint64_t st[3] = {128, (uint64_t)3 * H * 128, (uint64_t)rows * 3 * H * 128};
+    if (const char* e = encode_tmap_bf16(tmQKV, qkv, 4, dims, st, box)) return e;
+  }
+  const uint64_t dims[4] = {64, (uint64_t)H, (uint64_t)rows, (uint64_t)batch};
+  const uint64_t st[3] = {128, (uint64_t)H * 128, (uint64_t)rows * H * 128};
+  return encode_tmap_bf16(tmO, out, 4, dims, st, box);
 }
 
 }  // namespace
@@ -209,26 +312,26 @@ bool attention_supported(int B, int L, int H, int head_dim) {
 const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream) {
   if (!attention_supported(B, L, H, 64)) return "attention_fwd: unsupported shape (head dim 64, 1 <= L <= 512)";
   alignas(64) CUtensorMap tmQKV, tmO;
-  const uint32_t box[4] = {64, 1, 64, 1};
-  {
-    const uint64_t dims[4] = {64, (uint64_t)3 * H, (uint64_t)L, (uint64_t)B};
-    const uint64_t st[3] = {128, (uint64_t)3 * H * 128, (uint64_t)L * 3 * H * 128};
-    if (const char* e = encode_tmap_bf16(&tmQKV, qkv, 4, dims, st, box)) return e;
-  }
-  {
-    const uint64_t dims[4] = {64, (uint64_t)H, (uint64_t)L, (uint64_t)B};
-    const uint64_t st[3] = {128, (uint64_t)H * 128, (uint64_t)L * H * 128};
-    if (const char* e = encode_tmap_bf16(&tmO, out, 4, dims, st, box)) return e;
-  }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attention_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
-    if (e != cudaSuccess) return cudaGetErrorString(e);
-    attr_set = true;
-  }
-  attention_fwd_kernel<<<dim3((L + 127) / 128, H, B), kAttnThreads, kAttnSmem, stream>>>(tmQKV, tmO, mask, L, H);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+  if (const char* e = encode_attention_maps(&tmQKV, &tmO, qkv, out, L, B, H)) return e;
+  return launch_attention<int>(tmQKV, tmO, mask, L, H, dim3((L + 127) / 128, H, B), stream);
+}
+
+bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim) {
+  return T >= 1 && attention_supported(B, max_len, H, head_dim);
+}
+
+const char* attention_varlen_fwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, void* out, void* maps,
+                                 int T, int B, int max_len, int H, cudaStream_t stream) {
+  if (!attention_varlen_supported(T, B, max_len, H, 64))
+    return "attention_varlen_fwd: unsupported shape (head dim 64, T >= 1, 1 <= max_len <= 512)";
+  // templates over the whole buffer; the prologue replaces the address and the row count per sequence
+  alignas(64) CUtensorMap tmQKV, tmO;
+  if (const char* e = encode_attention_maps(&tmQKV, &tmO, qkv, out, T, 1, H)) return e;
+  CUtensorMap* m = static_cast<CUtensorMap*>(maps);
+  attention_varlen_maps_kernel<<<(B + 3) / 4, 128, 0, stream>>>(tmQKV, tmO, qkv, out, cu_seqlens, m, B, H);
+  if (cudaError_t e = cudaGetLastError(); e != cudaSuccess) return cudaGetErrorString(e);
+  return launch_attention<Varlen>(tmQKV, tmO, key_mask, Varlen{cu_seqlens, m}, H, dim3((max_len + 127) / 128, H, B),
+                                  stream);
 }
 
 }  // namespace edl

@@ -212,6 +212,12 @@ bool attention_supported(int B, int L, int H, int head_dim);
 // qkv bf16 [B * L, 3 * H * 64] (Q | K | V column blocks, 16-byte aligned), mask uint8 [B, L] (1 = attend; nullptr: all),
 // out bf16 [B * L, H * 64].  Returns nullptr or an error string.
 const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream);
+bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim);
+// Packed sequences: qkv bf16 [T, 3 * H * 64], sequence b in rows [cu_seqlens[b], cu_seqlens[b + 1]) (int32 device
+// offsets, 1 <= length <= max_len <= 512), key_mask uint8 [T] (1 = attend; nullptr: all), out bf16 [T, H * 64];
+// maps: device workspace of 2 * B CUtensorMaps (64-byte aligned).  A sequence's output depends on its own rows only.
+const char* attention_varlen_fwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, void* out, void* maps,
+                                 int T, int B, int max_len, int H, cudaStream_t stream);
 constexpr int kLnMaxC = 1024;
 bool layernorm_supported(int C);
 // y[r] = (x[r] - mean) * rsqrt(var + eps) * gamma + beta over the C columns of each row; x, y bf16 [rows, C] (row pitch

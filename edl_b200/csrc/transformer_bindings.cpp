@@ -32,6 +32,33 @@ void attention_fwd(const Tensor& qkv, const c10::optional<Tensor>& mask, Tensor&
   TORCH_CHECK(err == nullptr, "edl attention_fwd failed: ", err);
 }
 
+// qkv [T, 3 * H * 64], cu_seqlens int32 [B + 1], key_mask uint8 [T] or None, out [T, H * 64], maps uint8 [B * 256]
+void attention_varlen_fwd(const Tensor& qkv, const Tensor& cu_seqlens, const c10::optional<Tensor>& key_mask,
+                          Tensor& out, Tensor& maps, int64_t max_len, int64_t H) {
+  check_bf16_2d(qkv, "qkv");
+  check_bf16_2d(out, "out");
+  const int64_t T = qkv.size(0), B = cu_seqlens.numel() - 1;
+  TORCH_CHECK(qkv.size(1) == 3 * H * 64, "qkv must be [T, 3 * H * 64]");
+  TORCH_CHECK(out.size(0) == T && out.size(1) == H * 64, "out must be [T, H * 64]");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0);
+  TORCH_CHECK(cu_seqlens.is_cuda() && cu_seqlens.scalar_type() == at::kInt && cu_seqlens.dim() == 1 &&
+              cu_seqlens.is_contiguous() && B >= 1, "cu_seqlens must be a contiguous int32 [B + 1] CUDA tensor");
+  TORCH_CHECK(maps.is_cuda() && maps.scalar_type() == at::kByte && maps.is_contiguous() && maps.numel() >= B * 256 &&
+              reinterpret_cast<uintptr_t>(maps.data_ptr()) % 64 == 0, "maps: 64-byte aligned uint8 [B * 256] workspace");
+  TORCH_CHECK(T < (int64_t{1} << 31) && B <= 65535, "attention_varlen_fwd: T < 2^31 rows, B <= 65535 sequences");
+  const uint8_t* mp = nullptr;
+  if (key_mask.has_value() && key_mask->defined()) {
+    TORCH_CHECK(key_mask->is_cuda() && key_mask->scalar_type() == at::kByte && key_mask->is_contiguous() &&
+                key_mask->numel() == T, "key_mask must be a contiguous uint8 [T] CUDA tensor");
+    mp = key_mask->data_ptr<uint8_t>();
+  }
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const char* err = edl::attention_varlen_fwd(qkv.data_ptr(), cu_seqlens.data_ptr<int>(), mp, out.data_ptr(),
+                                              maps.data_ptr(), (int)T, (int)B, (int)max_len, (int)H,
+                                              at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl attention_varlen_fwd failed: ", err);
+}
+
 void check_affine(const Tensor& g, const Tensor& b, int64_t C) {
   TORCH_CHECK(g.is_cuda() && g.scalar_type() == at::kFloat && g.is_contiguous() && g.numel() == C, "gamma: fp32 [C]");
   TORCH_CHECK(b.is_cuda() && b.scalar_type() == at::kFloat && b.is_contiguous() && b.numel() == C, "beta: fp32 [C]");
@@ -76,6 +103,8 @@ void embedding_layernorm_fwd(const Tensor& ids, const Tensor& pos_ids, const Ten
 void register_transformer_bindings(pybind11::module_& m) {
   m.def("attention_fwd", &attention_fwd);
   m.def("attention_supported", &edl::attention_supported);
+  m.def("attention_varlen_fwd", &attention_varlen_fwd);
+  m.def("attention_varlen_supported", &edl::attention_varlen_supported);
   m.def("layernorm_fwd", &layernorm_fwd);
   m.def("layernorm_supported", &edl::layernorm_supported);
   m.def("embedding_layernorm_fwd", &embedding_layernorm_fwd);

@@ -69,16 +69,20 @@ class TeacherServer:
     @torch.no_grad()
     def _run_batch(self, slots):
         sizes = [len(next(iter(s["feeds"].values()))) for s in slots]
-        feeds = []
-        for name in self.feed_names:
-            arr = np.concatenate([s["feeds"][name] for s in slots], 0)
-            t = torch.from_numpy(np.ascontiguousarray(arr)).to(self.device)
-            if t.is_floating_point():
-                t = t.to(self.dtype)
-                if t.dim() == 4 and self.device.type == "cuda":
-                    t = t.contiguous(memory_format=torch.channels_last)
-            feeds.append(t)
-        out = self.model(*feeds)
+        if hasattr(self.model, "forward_requests"):
+            # the model collates itself (sequence teachers pack requests of different lengths)
+            out = self.model.forward_requests([[s["feeds"][name] for name in self.feed_names] for s in slots])
+        else:
+            feeds = []
+            for name in self.feed_names:
+                arr = np.concatenate([s["feeds"][name] for s in slots], 0)
+                t = torch.from_numpy(np.ascontiguousarray(arr)).to(self.device)
+                if t.is_floating_point():
+                    t = t.to(self.dtype)
+                    if t.dim() == 4 and self.device.type == "cuda":
+                        t = t.contiguous(memory_format=torch.channels_last)
+                feeds.append(t)
+            out = self.model(*feeds)
         if self.postprocess is not None:
             out = self.postprocess(out)
         if isinstance(out, dict):

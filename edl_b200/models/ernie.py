@@ -9,9 +9,13 @@ On CUDA every layer runs on the package's own kernels: the wgmma GEMM (bias in t
 addend, GELU as a compile-time epilogue variant), the attention kernel reading Q / K / V in place from the QKV output,
 the LayerNorm and the embedding-sum + LayerNorm kernels.  The weight matrices are cast to bf16 once, at the first CUDA
 forward after a load or a move; biases and LayerNorm parameters stay fp32.  On CPU the same forward runs in float32
-PyTorch math (the reference the GPU path is tested against)."""
+PyTorch math (the reference the GPU path is tested against).
+
+``forward_packed`` runs the same layers on a batch packed to its real tokens (``pack_sequences``) with the
+variable-length attention kernel; ``forward_requests`` packs requests of different lengths for the teacher server."""
 from __future__ import annotations
 
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -19,6 +23,40 @@ import torch.nn.functional as F
 from .. import ops
 
 CLS_PAD = 8      # classifier rows after padding: a 2-class output row (4 bytes) is not a TMA-describable pitch
+
+
+MAX_SEQ_LEN = 512  # the attention kernels' longest sequence
+
+
+def pack_sequences(input_ids, position_ids, segment_ids, input_mask, max_positions=None):
+    """Pack a padded batch ([B, L] or [B, L, 1] numpy arrays or CPU tensors) into its real tokens, for
+    ``ErnieEncoder.forward_packed``.
+
+    Keeps every token whose mask is nonzero and always token 0 of each sample (the [CLS] row the pooler reads), in
+    order.  Returns int64 CPU tensors ``ids, pos, seg`` [T], int32 ``cu_seqlens`` [B + 1], the host int ``max_len`` and
+    ``key_mask``: uint8 [T] when some sample's token 0 is masked (it is kept as a query but is not a key), else None.
+    The packed forward is then the padded forward for any mask, an empty one included.  Raises ValueError for a sample
+    of more than 512 kept tokens, or more than ``max_positions`` (the position table) when given."""
+    def arr(t):
+        return t.detach().cpu().numpy() if torch.is_tensor(t) else np.asarray(t)
+
+    mask = arr(input_mask)
+    b = mask.shape[0]
+    mask = mask.reshape(b, -1) != 0
+    if b == 0 or mask.shape[1] == 0:
+        raise ValueError("pack_sequences: empty batch %s" % (mask.shape,))
+    keep = mask.copy()
+    keep[:, 0] = True
+    lens = keep.sum(1)
+    limit = MAX_SEQ_LEN if max_positions is None else min(MAX_SEQ_LEN, int(max_positions))
+    if int(lens.max()) > limit:
+        raise ValueError("pack_sequences: a sample has %d tokens; at most %d are supported" % (int(lens.max()), limit))
+    cu = np.zeros(b + 1, np.int32)
+    np.cumsum(lens, out=cu[1:])
+    ids, pos, seg = (torch.from_numpy(np.ascontiguousarray(arr(t).reshape(mask.shape)[keep], dtype=np.int64))
+                     for t in (input_ids, position_ids, segment_ids))
+    key_mask = None if mask[:, 0].all() else torch.from_numpy(mask[keep].astype(np.uint8))
+    return ids, pos, seg, torch.from_numpy(cu), int(lens.max()), key_mask
 
 
 class ErnieEncoder(nn.Module):
@@ -154,35 +192,65 @@ class ErnieEncoder(nn.Module):
         ids, pos, seg = (t.reshape(b, l).long() for t in (input_ids, position_ids, segment_ids))
         keep = input_mask.reshape(b, l) != 0
         if self.word_emb.is_cuda:
-            return self._forward_cuda(ids, pos, seg, keep.to(torch.uint8).contiguous(), b, l)
-        return self._forward_reference(ids, pos, seg, keep, b, l)
+            mask, fwd = keep.to(torch.uint8).contiguous(), self._forward_cuda
+        else:
+            mask, fwd = keep, self._forward_reference
+        return fwd(ids, pos, seg, lambda qkv: ops.attention(qkv, mask, b, l, self.heads, self.head_dim),
+                   lambda x: x.view(b, l, self.hidden)[:, 0])                   # [B, C], row pitch L * C
 
-    def _forward_cuda(self, ids, pos, seg, mask, b, l):
+    @torch.no_grad()
+    def forward_packed(self, ids, pos, seg, cu_seqlens, max_len, key_mask=None):
+        """The forward over packed sequences (``pack_sequences``): ids / pos / seg int64 [T], ``cu_seqlens`` int32
+        [B + 1], ``max_len`` the longest length, ``key_mask`` uint8 [T] or None.  Every row-wise layer runs on the T real
+        tokens only.  Returns fp32 logits [B, num_labels].  On CUDA the inputs are expected on the model's device; the
+        path makes no host synchronisation under CUDA-graph capture, so it can be captured for fixed shapes."""
+        dev = self.word_emb.device
+        ids, pos, seg, cu_seqlens = (t.to(dev) for t in (ids, pos, seg, cu_seqlens))
+        key_mask = None if key_mask is None else key_mask.to(dev)
+        first = cu_seqlens[:-1].long()
+        fwd = self._forward_cuda if self.word_emb.is_cuda else self._forward_reference
+        return fwd(ids, pos, seg, lambda qkv: ops.attention_varlen(qkv, cu_seqlens, max_len, self.heads, key_mask),
+                   lambda x: x.index_select(0, first))
+
+    def forward_requests(self, requests):
+        """Serve a batch of requests whose sequence lengths may differ: each request is the forward's four feeds
+        ([n, L] or [n, L, 1], L per request).  Packs all samples on the host, copies the real tokens to the device and
+        runs ``forward_packed``.  Returns fp32 logits [sum n, num_labels] in request order."""
+        packs = [pack_sequences(*r, max_positions=self.pos_emb.shape[0]) for r in requests]
+        ids, pos, seg = (torch.cat([p[i] for p in packs]) for i in range(3))
+        lens = torch.cat([p[3].diff() for p in packs])
+        cu = torch.zeros(len(lens) + 1, dtype=torch.int32)
+        torch.cumsum(lens, 0, out=cu[1:])
+        key_mask = None
+        if any(p[5] is not None for p in packs):
+            key_mask = torch.cat([p[5] if p[5] is not None else torch.ones(len(p[0]), dtype=torch.uint8) for p in packs])
+        return self.forward_packed(ids, pos, seg, cu, max(p[4] for p in packs), key_mask)
+
+    def _forward_cuda(self, ids, pos, seg, attend, cls_rows):
         w = self._device_weights()
         word, pemb, semb, g, beta = w["emb"]
         x = ops.embedding_layernorm(ids, pos, seg, word, pemb, semb, g, beta, self.eps)
         for qkv_w, qkv_b, out_w, out_b, ln1_g, ln1_b, f1_w, f1_b, f2_w, f2_b, ln2_g, ln2_b in w["layers"]:
             qkv = ops.gemm_bf16(x, qkv_w, col_shift=qkv_b)
-            ctx = ops.attention(qkv, mask, b, l, self.heads, self.head_dim)
+            ctx = attend(qkv)
             x = ops.layer_norm(ops.gemm_bf16(ctx, out_w, col_shift=out_b, add=x), ln1_g, ln1_b, self.eps)
             f = ops.gemm_bf16(x, f1_w, col_shift=f1_b, gelu=True)
             x = ops.layer_norm(ops.gemm_bf16(f, f2_w, col_shift=f2_b, add=x), ln2_g, ln2_b, self.eps)
         pool_w, pool_b, cls_w, cls_b = w["head"]
-        cls_rows = x.view(b, l, self.hidden)[:, 0]                  # [B, C], row pitch L * C
-        pooled = torch.tanh(ops.linear_bf16(cls_rows, pool_w, pool_b))
+        pooled = torch.tanh(ops.linear_bf16(cls_rows(x), pool_w, pool_b))
         return ops.gemm_bf16(pooled, cls_w, col_shift=cls_b)[:, :self.num_labels].float()
 
-    def _forward_reference(self, ids, pos, seg, keep, b, l):
+    def _forward_reference(self, ids, pos, seg, attend, cls_rows):
         f32 = torch.float32
         x = ops.embedding_layernorm(ids, pos, seg, self.word_emb.to(f32), self.pos_emb.to(f32), self.seg_emb.to(f32),
                                     self.emb_ln_g, self.emb_ln_b, self.eps)
         for lyr in self.layers:
             qkv = F.linear(x, lyr.qkv_w.to(f32), lyr.qkv_b.to(f32))
-            ctx = ops.attention(qkv, keep, b, l, self.heads, self.head_dim)
+            ctx = attend(qkv)
             x = ops.layer_norm(F.linear(ctx, lyr.out_w.to(f32), lyr.out_b.to(f32)) + x, lyr.ln1_g, lyr.ln1_b, self.eps)
             f = F.gelu(F.linear(x, lyr.ffn1_w.to(f32), lyr.ffn1_b.to(f32)))
             x = ops.layer_norm(F.linear(f, lyr.ffn2_w.to(f32), lyr.ffn2_b.to(f32)) + x, lyr.ln2_g, lyr.ln2_b, self.eps)
-        pooled = torch.tanh(F.linear(x.view(b, l, self.hidden)[:, 0], self.pool_w.to(f32), self.pool_b.to(f32)))
+        pooled = torch.tanh(F.linear(cls_rows(x), self.pool_w.to(f32), self.pool_b.to(f32)))
         return F.linear(pooled, self.cls_w.to(f32), self.cls_b.to(f32))
 
 

@@ -62,6 +62,62 @@ def attention(qkv, mask, batch, seq_len, heads, head_dim=64, out=None):
     return out
 
 
+# ----------------------------------------------------------------------------------------- variable-length attention
+def attention_varlen_reference(qkv, cu_seqlens, max_len, heads, key_mask=None):
+    """Float32 math of ``attention_varlen``: ``attention_reference`` on each packed sequence.  Rows outside every
+    sequence are 0 (the kernel does not write them)."""
+    d = qkv.shape[1] // (3 * heads)
+    cu = [int(v) for v in cu_seqlens.tolist()]
+    out = torch.zeros((qkv.shape[0], heads * d), device=qkv.device, dtype=qkv.dtype)
+    for s, e in zip(cu[:-1], cu[1:]):
+        if e > s:
+            m = None if key_mask is None else key_mask[s:e].view(1, e - s)
+            out[s:e] = attention_reference(qkv[s:e], m, 1, e - s, heads, d)
+    return out
+
+
+def attention_varlen_supported(qkv, cu_seqlens, max_len, heads) -> bool:
+    from . import native
+
+    return (qkv.is_cuda and qkv.dtype == torch.bfloat16 and qkv.dim() == 2 and qkv.is_contiguous()
+            and qkv.data_ptr() % 16 == 0 and qkv.shape[1] % (3 * heads) == 0
+            and cu_seqlens.is_cuda and cu_seqlens.dim() == 1 and cu_seqlens.numel() >= 2
+            and native().attention_varlen_supported(qkv.shape[0], cu_seqlens.numel() - 1, int(max_len), heads,
+                                                    qkv.shape[1] // (3 * heads)))
+
+
+def attention_varlen(qkv, cu_seqlens, max_len, heads, key_mask=None, out=None):
+    """Masked multi-head self-attention over sequences packed back to back (inference).  ``qkv`` [T, 3 * H * 64] is the
+    QKV projection's output on the packed tokens; sequence b is rows [cu_seqlens[b], cu_seqlens[b + 1]) (int32 [B + 1],
+    offset 0, non-decreasing, lengths 1..512); ``max_len`` (host int) is at least the longest length; ``key_mask``
+    [T] (nonzero = attend) or None.  Returns O [T, H * 64].  Per sequence this is ``attention`` with L = its length,
+    and its output depends on its own rows only.
+
+    ``cu_seqlens`` is not read back to the host, so the call can be captured in a CUDA graph; ``pack_sequences``
+    (models/ernie.py) validates the offsets where they are made."""
+    from . import native, count_launch
+
+    if not qkv.is_cuda:
+        return attention_varlen_reference(qkv, cu_seqlens, max_len, heads, key_mask)
+    if not attention_varlen_supported(qkv, cu_seqlens, max_len, heads):
+        _count("attention_varlen: no kernel for T %d, B %d, max_len %d, H %d, width %d (%s): float32 math on the "
+               "library" % (qkv.shape[0], cu_seqlens.numel() - 1, max_len, heads, qkv.shape[-1], qkv.dtype))
+        return attention_varlen_reference(qkv, cu_seqlens, max_len, heads, key_mask)
+    b = cu_seqlens.numel() - 1
+    if out is None:
+        out = torch.empty((qkv.shape[0], qkv.shape[1] // 3), device=qkv.device, dtype=torch.bfloat16)
+    cu = cu_seqlens if (cu_seqlens.dtype == torch.int32 and cu_seqlens.is_contiguous()) else \
+        cu_seqlens.to(torch.int32).contiguous()
+    km = None
+    if key_mask is not None:
+        km = key_mask if (key_mask.dtype == torch.uint8 and key_mask.is_contiguous()) else \
+            (key_mask != 0).to(torch.uint8).contiguous()
+    maps = torch.empty(b * 256, device=qkv.device, dtype=torch.uint8)        # two 128-byte tensor maps per sequence
+    native().attention_varlen_fwd(qkv, cu, km, out, maps, int(max_len), heads)
+    count_launch(2)
+    return out
+
+
 # ---------------------------------------------------------------------------------------------------------- LayerNorm
 def layer_norm_reference(x, gamma, beta, eps):
     xf = x.float()

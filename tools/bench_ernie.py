@@ -3,12 +3,16 @@
     python tools/bench_ernie.py                      # B = 16, L = 128 and 256, one JSON line per length
     python tools/bench_ernie.py --profile DIR        # separately: a torch.profiler per-kernel table (no timing)
 
-Workload: ``ernie_base`` with random weights, batch 16, right-padded masks whose lengths come from a fixed seed.  "ours"
-is a CUDA-graph replay of ``ErnieEncoder.forward`` on the wgmma GEMM (bias / residual / GELU epilogues), the attention,
-LayerNorm and embedding-LayerNorm kernels; "torch" is a CUDA-graph replay of the same forward in bf16 on cuBLAS linear,
-``F.scaled_dot_product_attention`` and ``F.layer_norm``.  The two alternate in timed windows of device-timed replays.
-FLOPs are counted from shapes (GEMMs, Q K^T and P V over the full padded length); the share of peak is against the
-H100 SXM data-sheet dense bf16 rate (989 TFLOP/s at 700 W), so it is an end-to-end figure, not a kernel's."""
+Workload: ``ernie_base`` with random weights, batch 16, right-padded masks whose lengths come from a fixed seed (in
+[L/4, L], the spread of a batch padded to its longest sample).  "ours" is a CUDA-graph replay of
+``ErnieEncoder.forward`` on the wgmma GEMM (bias / residual / GELU epilogues), the attention, LayerNorm and
+embedding-LayerNorm kernels; "packed" is a CUDA-graph replay of ``forward_packed`` on the same samples packed to their
+real tokens (the varlen attention kernel, every other layer on T rows instead of B * L); "torch" is a CUDA-graph replay
+of the padded forward in bf16 on cuBLAS linear, ``F.scaled_dot_product_attention`` and ``F.layer_norm``.  The three
+alternate in timed windows of device-timed replays.  FLOPs are counted from shapes: ``gflop`` over the full padded
+length (what the padded forwards compute), ``gflop_real`` over the real tokens only (GEMM rows T, attention len_b^2 per
+sequence), the work every arm has to do; the shares of peak are against the H100 SXM data-sheet dense bf16 rate
+(989 TFLOP/s at 700 W), so they are end-to-end figures, not a kernel's."""
 import argparse
 import json
 import os
@@ -70,11 +74,13 @@ def torch_forward(model):
     return fwd
 
 
-def flops(model, b, l):
+def flops(model, b, l, lens=None):
+    """(GEMM, attention) FLOPs of a batch of b sequences padded to l, or of the sequences of lengths ``lens`` alone."""
     c, f, n = model.hidden, model.layers[0].ffn1_w.shape[0], model.num_layers
-    m = b * l
+    lens = [l] * b if lens is None else lens
+    m = sum(lens)
     gemm = 2 * m * c * (3 * c + c + 2 * f) * n + 2 * b * c * (c + model.num_labels)
-    attn = 4 * b * model.heads * l * l * model.head_dim * n
+    attn = 4 * model.heads * sum(x * x for x in lens) * model.head_dim * n
     return gemm, attn
 
 
@@ -119,15 +125,23 @@ def main():
         ops.reset_fallbacks()
         g_ours, out_ours = capture(model, feed)
         g_ref, out_ref = capture(torch.no_grad()(torch_forward(model)), feed)
+        packed = ernie.pack_sequences(*(t.cpu() for t in feed))
+        lens = packed[3].diff().tolist()
+        packed = [p.cuda() if torch.is_tensor(p) else p for p in packed]
+        g_pack, out_pack = capture(model.forward_packed, packed)
         g_ours.replay()
         g_ref.replay()
+        g_pack.replay()
         torch.cuda.synchronize()
-        cos = F.cosine_similarity(out_ours.flatten()[None].double(), out_ref.flatten()[None].double()).item()
+
+        def cosine(a, b):
+            return F.cosine_similarity(a.flatten()[None].double(), b.flatten()[None].double()).item()
+        cos = cosine(out_ours, out_ref)
         if args.profile:
             from torch.profiler import ProfilerActivity, profile
 
             os.makedirs(args.profile, exist_ok=True)
-            for name, g in (("ours", g_ours), ("torch", g_ref)):
+            for name, g in (("ours", g_ours), ("packed", g_pack), ("torch", g_ref)):
                 with profile(activities=[ProfilerActivity.CUDA]) as prof:
                     for _ in range(5):
                         g.replay()
@@ -137,26 +151,39 @@ def main():
                     fh.write(table)
                 print("== L %d %s (5 replays) ==\n%s" % (l, name, table))
             continue
-        for g in (g_ours, g_ref):
+        for g in (g_ours, g_pack, g_ref):
             timed(g, 5)
-        t_ours, t_ref = [], []
+        t_ours, t_pack, t_ref = [], [], []
         for _ in range(args.windows):
             t_ours.append(timed(g_ours, args.reps))
+            t_pack.append(timed(g_pack, args.reps))
             t_ref.append(timed(g_ref, args.reps))
         gemm, attn = flops(model, args.batch, l)
-        best_o, best_r = min(t_ours), min(t_ref)
-        med_o, med_r = sorted(t_ours)[len(t_ours) // 2], sorted(t_ref)[len(t_ref) // 2]
+        real = sum(flops(model, args.batch, l, lens))
+        best_o, best_p, best_r = min(t_ours), min(t_pack), min(t_ref)
+        med_o, med_p, med_r = (sorted(t)[len(t) // 2] for t in (t_ours, t_pack, t_ref))
         print(json.dumps({
             "workload": "ernie_base forward, B %d, L %d, padded masks" % (args.batch, l),
             "card": info, "fallbacks": ops.fallbacks(), "logits_cosine_vs_torch": round(cos, 6),
-            "ours_seq_per_s": round(args.batch / med_o, 1), "torch_seq_per_s": round(args.batch / med_r, 1),
-            "ours_ms_median": round(med_o * 1e3, 4), "torch_ms_median": round(med_r * 1e3, 4),
-            "ours_ms_best": round(best_o * 1e3, 4), "torch_ms_best": round(best_r * 1e3, 4),
-            "speedup_median": round(med_r / med_o, 3),
+            "real_tokens": sum(lens), "real_token_share": round(sum(lens) / (args.batch * l), 4),
+            "packed_logits_cosine_vs_padded": round(cosine(out_pack, out_ours), 6),
+            "packed_logits_max_abs_diff_vs_padded": float((out_pack - out_ours).abs().max()),
+            "packed_logits_bitwise_equal_padded": bool(torch.equal(out_pack, out_ours)),
+            "ours_seq_per_s": round(args.batch / med_o, 1), "packed_seq_per_s": round(args.batch / med_p, 1),
+            "torch_seq_per_s": round(args.batch / med_r, 1),
+            "ours_ms_median": round(med_o * 1e3, 4), "packed_ms_median": round(med_p * 1e3, 4),
+            "torch_ms_median": round(med_r * 1e3, 4),
+            "ours_ms_best": round(best_o * 1e3, 4), "packed_ms_best": round(best_p * 1e3, 4),
+            "torch_ms_best": round(best_r * 1e3, 4),
+            "speedup_median": round(med_r / med_o, 3), "packed_speedup_vs_padded_median": round(med_o / med_p, 3),
+            "packed_speedup_vs_torch_median": round(med_r / med_p, 3),
             "gflop": round((gemm + attn) / 1e9, 2), "gemm_flop_share": round(gemm / (gemm + attn), 4),
+            "gflop_real": round(real / 1e9, 2),
             "ours_tflops": round((gemm + attn) / med_o / 1e12, 1),
             "ours_share_of_bf16_peak": round((gemm + attn) / med_o / PEAK_BF16, 3),
             "torch_share_of_bf16_peak": round((gemm + attn) / med_r / PEAK_BF16, 3),
+            "real_tflops": {k: round(real / t / 1e12, 1) for k, t in (("ours", med_o), ("packed", med_p),
+                                                                      ("torch", med_r))},
         }), flush=True)
 
 
