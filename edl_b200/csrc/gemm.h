@@ -178,11 +178,20 @@ struct GemmFp8Args {
   // gemm_fp8_blockscaled only: a_scales fp32 [ceil(K/128), M], b_scales fp32 [ceil(N/128), ceil(K/128)]
   const float* a_scales = nullptr;
   const float* b_scales = nullptr;
+  // gemm_fp8_blockscaled: optional bf16 addend [M, N] (row pitch ld_add elements), added after col_shift
+  const void* add = nullptr;
+  int64_t ld_add = 0;
+  // gemm_fp8_blockscaled_gelu_e4m3 only: the output's block scales, fp32 [ceil(N/128), M]
+  float* a_scales_out = nullptr;
 };
 const char* gemm_fp8(const GemmFp8Args& args, cudaStream_t stream);
-// D[M,N] bf16 = relu?((sum_b (A_b * B_b^T) * a_scales[b, m] * b_scales[n / 128, b]) * col_scale[n] + col_shift[n])
-// over the 128-element K blocks b; col_scale carries only the folded BN scale here.
+// D[M,N] bf16 = relu?((sum_b (A_b * B_b^T) * a_scales[b, m] * b_scales[n / 128, b]) * col_scale[n] + col_shift[n]
+// (+ add[m, n] when add is set)) over the 128-element K blocks b; col_scale carries only the folded BN scale here.
 const char* gemm_fp8_blockscaled(const GemmFp8Args& args, cudaStream_t stream);
+// FFN1 of the sequence teacher: g = bf16(gelu(sum_b (A_b * B_b^T) * a_scales[b, m] * b_scales[n / 128, b] + col_shift[n]))
+// (erf form), quantised per row and 128-column block as quantize_e4m3_blocks does: D holds e4m3 bytes [M, N] (row
+// pitch ldd bytes, N % 16 == 0) and a_scales_out[n / 128, m] their scales.  No col_scale, ReLU or addend.
+const char* gemm_fp8_blockscaled_gelu_e4m3(const GemmFp8Args& args, cudaStream_t stream);
 
 // bf16 -> e4m3 with a per-tensor scale (q = sat(x / scale)); amax_out (optional) receives max|x| for
 // calibration / delayed scaling.

@@ -371,17 +371,22 @@ void quantize_e4m3_blocks(const Tensor& x, Tensor& q, Tensor& sa) {
   TORCH_CHECK(err == nullptr, "edl quantize_e4m3_blocks failed: ", err);
 }
 
-// D bf16 [M,N] = relu?((sum_b (A8_b * B8_b^T) * sa[b, m] * sb[n / 128, b]) * col_scale + col_shift)
-void gemm_fp8_blockscaled(const Tensor& A, const Tensor& sa, const Tensor& B, const Tensor& sb, Tensor& D,
-                          const c10::optional<Tensor>& col_scale, const c10::optional<Tensor>& col_shift, bool relu) {
+// The checks and arguments shared by the block-scaled entries (D: bf16, or e4m3 bytes for the GELU epilogue)
+edl::GemmFp8Args blockscaled_args(const Tensor& A, const Tensor& sa, const Tensor& B, const Tensor& sb, const Tensor& D,
+                                  const c10::optional<Tensor>& col_scale, const c10::optional<Tensor>& col_shift,
+                                  bool relu, bool q_out) {
   TORCH_CHECK(A.is_cuda() && B.is_cuda() && D.is_cuda() && A.dim() == 2 && B.dim() == 2 && D.dim() == 2);
   TORCH_CHECK(A.element_size() == 1 && B.element_size() == 1, "A and B hold e4m3 bytes");
-  TORCH_CHECK(D.scalar_type() == at::kBFloat16, "D must be bf16");
+  if (q_out) {
+    TORCH_CHECK(D.element_size() == 1, "the GELU e4m3 epilogue writes e4m3 bytes");
+  } else {
+    TORCH_CHECK(D.scalar_type() == at::kBFloat16, "D must be bf16");
+  }
   TORCH_CHECK(A.stride(1) == 1 && B.stride(1) == 1 && D.stride(1) == 1, "operands need a contiguous last dim");
   TORCH_CHECK(A.size(1) == B.size(1), "K mismatch: ", A.size(1), " vs ", B.size(1));
   TORCH_CHECK(D.size(0) == A.size(0) && D.size(1) == B.size(0), "D must be [M, N]");
   const int64_t M = A.size(0), N = B.size(0), K = A.size(1), kb = (K + 127) / 128;
-  TORCH_CHECK(K % 16 == 0 && A.stride(0) % 16 == 0 && B.stride(0) % 16 == 0 && D.stride(0) % 8 == 0,
+  TORCH_CHECK(K % 16 == 0 && A.stride(0) % 16 == 0 && B.stride(0) % 16 == 0 && D.stride(0) % (q_out ? 16 : 8) == 0,
               "fp8 GEMM needs 16-byte aligned rows");
   TORCH_CHECK(reinterpret_cast<uintptr_t>(A.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(B.data_ptr()) % 16 == 0 &&
               reinterpret_cast<uintptr_t>(D.data_ptr()) % 16 == 0, "A, B and D must be 16-byte aligned");
@@ -409,9 +414,40 @@ void gemm_fp8_blockscaled(const Tensor& A, const Tensor& sa, const Tensor& B, co
   g.a_scales = sa.data_ptr<float>();
   g.b_scales = sb.data_ptr<float>();
   g.device = A.device().index();
+  return g;
+}
+
+// D bf16 [M,N] = relu?((sum_b (A8_b * B8_b^T) * sa[b, m] * sb[n / 128, b]) * col_scale + col_shift (+ add))
+void gemm_fp8_blockscaled(const Tensor& A, const Tensor& sa, const Tensor& B, const Tensor& sb, Tensor& D,
+                          const c10::optional<Tensor>& col_scale, const c10::optional<Tensor>& col_shift, bool relu,
+                          const c10::optional<Tensor>& add) {
+  edl::GemmFp8Args g = blockscaled_args(A, sa, B, sb, D, col_scale, col_shift, relu, false);
+  if (add.has_value() && add->defined()) {
+    TORCH_CHECK(add->is_cuda() && add->device() == D.device() && add->scalar_type() == at::kBFloat16 &&
+                add->dim() == 2 && add->size(0) == g.M && add->size(1) == g.N && add->stride(1) == 1,
+                "add must be a bf16 [M, N] CUDA tensor with a contiguous last dim");
+    TORCH_CHECK(g.N % 8 == 0 && add->stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(add->data_ptr()) % 16 == 0,
+                "add needs 16-byte aligned rows");
+    g.add = add->data_ptr();
+    g.ld_add = add->stride(0);
+  }
   c10::cuda::CUDAGuard guard(A.device());
   const char* err = edl::gemm_fp8_blockscaled(g, at::cuda::getCurrentCUDAStream().stream());
   TORCH_CHECK(err == nullptr, "edl gemm_fp8_blockscaled failed: ", err);
+}
+
+// Q e4m3 [M,N], sa_out fp32 [ceil(N/128), M]: block quantisation of bf16(gelu(sum_b (A8_b * B8_b^T) * sa * sb + bias))
+void gemm_fp8_blockscaled_gelu_e4m3(const Tensor& A, const Tensor& sa, const Tensor& B, const Tensor& sb, Tensor& Q,
+                                    Tensor& sa_out, const c10::optional<Tensor>& bias) {
+  edl::GemmFp8Args g = blockscaled_args(A, sa, B, sb, Q, c10::nullopt, bias, false, true);
+  TORCH_CHECK(g.N % 16 == 0, "the GELU e4m3 epilogue needs N % 16 == 0, got N = ", g.N);
+  TORCH_CHECK(sa_out.is_cuda() && sa_out.device() == Q.device() && sa_out.scalar_type() == at::kFloat &&
+              sa_out.is_contiguous() && sa_out.dim() == 2 && sa_out.size(0) == (g.N + 127) / 128 &&
+              sa_out.size(1) == g.M, "sa_out must be contiguous fp32 [ceil(N/128), M]");
+  g.a_scales_out = sa_out.data_ptr<float>();
+  c10::cuda::CUDAGuard guard(A.device());
+  const char* err = edl::gemm_fp8_blockscaled_gelu_e4m3(g, at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl gemm_fp8_blockscaled_gelu_e4m3 failed: ", err);
 }
 
 bool conv3x3_supported(int64_t n, int64_t h, int64_t w, int64_t cin, int64_t cout, bool dgrad, int64_t groups) {
@@ -535,7 +571,9 @@ void register_gemm_bindings(pybind11::module_& m) {
   m.def("persistent_gemm_enabled", &edl::persistent_gemm_enabled);
   m.def("gemm_fp8", &gemm_fp8);
   m.def("quantize_e4m3", &quantize_e4m3);
-  m.def("gemm_fp8_blockscaled", &gemm_fp8_blockscaled);
+  m.def("gemm_fp8_blockscaled", &gemm_fp8_blockscaled, pybind11::arg("A"), pybind11::arg("sa"), pybind11::arg("B"), pybind11::arg("sb"),
+        pybind11::arg("D"), pybind11::arg("col_scale"), pybind11::arg("col_shift"), pybind11::arg("relu"), pybind11::arg("add") = pybind11::none());
+  m.def("gemm_fp8_blockscaled_gelu_e4m3", &gemm_fp8_blockscaled_gelu_e4m3);
   m.def("quantize_e4m3_blocks", &quantize_e4m3_blocks);
   m.def("conv3x3_supported", &conv3x3_supported);
   m.def("conv3x3_infer", &conv3x3_infer);

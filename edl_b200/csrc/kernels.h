@@ -230,5 +230,14 @@ void embedding_layernorm_fwd(const int64_t* ids, const int64_t* pos_ids, const i
                              int64_t n_word, const void* pos, int64_t n_pos, const void* seg, int64_t n_seg,
                              const float* gamma, const float* beta, void* y, int64_t rows, int C, float eps, int* err,
                              cudaStream_t s);
+// Quantising variants: also q e4m3 [rows, C] (contiguous, 8-byte aligned) and sa fp32 [ceil(C/128), rows] of the stored
+// bf16 y, bit for bit what quantize_e4m3_blocks (gemm.h) makes of y: s = max|y| / 448 per row and 128-column block (1
+// for an all-zero block), q = sat(y / s).
+void layernorm_e4m3_fwd(const void* x, const float* gamma, const float* beta, void* y, void* q, float* sa, int64_t rows,
+                        int C, float eps, cudaStream_t s);
+void embedding_layernorm_e4m3_fwd(const int64_t* ids, const int64_t* pos_ids, const int64_t* seg_ids, const void* word,
+                                  int64_t n_word, const void* pos, int64_t n_pos, const void* seg, int64_t n_seg,
+                                  const float* gamma, const float* beta, void* y, void* q, float* sa, int64_t rows, int C,
+                                  float eps, int* err, cudaStream_t s);
 
 }  // namespace edl

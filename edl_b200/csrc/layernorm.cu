@@ -1,6 +1,12 @@
 // LayerNorm over the hidden dimension, and the embedding sum + LayerNorm of a BERT / ERNIE encoder's input (inference).
 // One warp per row: a lane holds up to four 16-byte chunks (8 bf16) of the row in registers, so the row is read once
 // and the variance is the two-pass sum of (x - mean)^2 over the registers.  C % 8 == 0, C <= 1024.
+//
+// The quantising variants (template argument Q) also write e4m3 bytes q [rows, C] and fp32 scales sa [ceil(C/128), rows]
+// of the stored bf16 y, for the block-scaled FP8 GEMM that reads it: a 128-element block is one half-warp's chunk c, so
+// its max|y| is the half-warp shuffle of quantize_e4m3_blocks (gemm_fp8.cu) and the bytes and scales are those it writes.
+#include <cuda_fp8.h>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -10,9 +16,18 @@ namespace {
 constexpr int kLnWarps = 8;
 constexpr int kLnChunks = kLnMaxC / 256;     // 16-byte chunks per lane
 
+// Q: where the quantised copy goes (q: this row's C bytes; sa: the row's first scale, one scale every `rows` floats)
+struct LnQuant {
+  uint8_t* q;
+  float* sa;
+  int64_t rows;
+};
+
 // x: this lane's chunks of the row (chunk c of the lane is columns (c * 32 + lane) * 8 ..), n8 = C / 8
+template <bool Q = false>
 EDL_DEVICE void ln_store(float (&x)[kLnChunks][8], int lane, int n8, int C, const float* __restrict__ gamma,
-                         const float* __restrict__ beta, float eps, __nv_bfloat16* __restrict__ yrow) {
+                         const float* __restrict__ beta, float eps, __nv_bfloat16* __restrict__ yrow,
+                         [[maybe_unused]] const LnQuant& qo = LnQuant{}) {
   float s = 0.f;
 #pragma unroll
   for (int c = 0; c < kLnChunks; ++c)
@@ -30,24 +45,64 @@ EDL_DEVICE void ln_store(float (&x)[kLnChunks][8], int lane, int n8, int C, cons
         q = fmaf(d, d, q);
       }
   const float rstd = rsqrtf(warp_sum(q) / (float)C + eps);
+  if constexpr (Q) {
+    // every lane of a live chunk takes part in the shuffles; lanes past C hold zeros (a short tail block)
 #pragma unroll
-  for (int c = 0; c < kLnChunks; ++c) {
-    const int k = c * 32 + lane;
-    if (k >= n8) continue;
-    const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma) + 2 * k), g1 = __ldg(reinterpret_cast<const float4*>(gamma) + 2 * k + 1);
-    const float4 b0 = __ldg(reinterpret_cast<const float4*>(beta) + 2 * k), b1 = __ldg(reinterpret_cast<const float4*>(beta) + 2 * k + 1);
-    const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-    float y[8];
+    for (int c = 0; c < kLnChunks; ++c) {
+      if (c * 32 >= n8) break;
+      const int k = c * 32 + lane;
+      const bool live = k < n8;
+      float y[8];
+      if (live) {
+        const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma) + 2 * k), g1 = __ldg(reinterpret_cast<const float4*>(gamma) + 2 * k + 1);
+        const float4 b0 = __ldg(reinterpret_cast<const float4*>(beta) + 2 * k), b1 = __ldg(reinterpret_cast<const float4*>(beta) + 2 * k + 1);
+        const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+        const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
-    for (int e = 0; e < 8; ++e) y[e] = fmaf((x[c][e] - mean) * rstd, g[e], bb[e]);
-    st_vec(yrow + k * 8, pack8(y));
+        for (int e = 0; e < 8; ++e) y[e] = fmaf((x[c][e] - mean) * rstd, g[e], bb[e]);
+        const bf16x8 pk = pack8(y);
+        st_vec(yrow + k * 8, pk);
+        unpack8(pk, y);                                      // quantise the stored bf16 values
+      } else {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) y[e] = 0.f;
+      }
+      float amax = 0.f;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) amax = fmaxf(amax, fabsf(y[e]));
+#pragma unroll
+      for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+      const float s = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+      const int b = k >> 4;                                   // = 2 c + lane / 16
+      if ((lane & 15) == 0 && b * 16 < n8) qo.sa[(int64_t)b * qo.rows] = s;
+      if (live) {
+        uint8_t o[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) o[e] = (uint8_t)__nv_cvt_float_to_fp8(__fdiv_rn(y[e], s), __NV_SATFINITE, __NV_E4M3);
+        *reinterpret_cast<uint2*>(qo.q + k * 8) = *reinterpret_cast<const uint2*>(o);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int c = 0; c < kLnChunks; ++c) {
+      const int k = c * 32 + lane;
+      if (k >= n8) continue;
+      const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma) + 2 * k), g1 = __ldg(reinterpret_cast<const float4*>(gamma) + 2 * k + 1);
+      const float4 b0 = __ldg(reinterpret_cast<const float4*>(beta) + 2 * k), b1 = __ldg(reinterpret_cast<const float4*>(beta) + 2 * k + 1);
+      const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+      const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+      float y[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) y[e] = fmaf((x[c][e] - mean) * rstd, g[e], bb[e]);
+      st_vec(yrow + k * 8, pack8(y));
+    }
   }
 }
 
+template <bool Q>
 __global__ void __launch_bounds__(kLnWarps * 32)
 layernorm_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                 __nv_bfloat16* __restrict__ y, int64_t rows, int C, float eps) {
+                 __nv_bfloat16* __restrict__ y, int64_t rows, int C, float eps, uint8_t* __restrict__ q, float* __restrict__ sa) {
   const int lane = threadIdx.x & 31;
   const int64_t r = (int64_t)blockIdx.x * kLnWarps + (threadIdx.x >> 5);
   if (r >= rows) return;
@@ -63,15 +118,17 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ 
       for (int e = 0; e < 8; ++e) v[c][e] = f[e];
     }
   }
-  ln_store(v, lane, n8, C, gamma, beta, eps, y + r * C);
+  ln_store<Q>(v, lane, n8, C, gamma, beta, eps, y + r * C, LnQuant{q + r * C, sa + r, rows});
 }
 
+template <bool Q>
 __global__ void __launch_bounds__(kLnWarps * 32)
 embedding_layernorm_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ pos_ids,
                            const int64_t* __restrict__ seg_ids, const __nv_bfloat16* __restrict__ word, int64_t n_word,
                            const __nv_bfloat16* __restrict__ pos, int64_t n_pos, const __nv_bfloat16* __restrict__ seg,
                            int64_t n_seg, const float* __restrict__ gamma, const float* __restrict__ beta,
-                           __nv_bfloat16* __restrict__ y, int64_t rows, int C, float eps, int* err) {
+                           __nv_bfloat16* __restrict__ y, int64_t rows, int C, float eps, int* err,
+                           uint8_t* __restrict__ q, float* __restrict__ sa) {
   const int lane = threadIdx.x & 31;
   const int64_t r = (int64_t)blockIdx.x * kLnWarps + (threadIdx.x >> 5);
   if (r >= rows) return;
@@ -104,7 +161,7 @@ embedding_layernorm_kernel(const int64_t* __restrict__ ids, const int64_t* __res
       }
     }
   }
-  ln_store(v, lane, n8, C, gamma, beta, eps, y + r * C);
+  ln_store<Q>(v, lane, n8, C, gamma, beta, eps, y + r * C, LnQuant{q + r * C, sa + r, rows});
 }
 
 }  // namespace
@@ -114,8 +171,17 @@ bool layernorm_supported(int C) { return C >= 8 && C <= kLnMaxC && C % 8 == 0; }
 void layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y, int64_t rows, int C, float eps,
                    cudaStream_t s) {
   if (rows <= 0) return;
-  layernorm_kernel<<<(unsigned)((rows + kLnWarps - 1) / kLnWarps), kLnWarps * 32, 0, s>>>(
-      reinterpret_cast<const __nv_bfloat16*>(x), gamma, beta, reinterpret_cast<__nv_bfloat16*>(y), rows, C, eps);
+  layernorm_kernel<false><<<(unsigned)((rows + kLnWarps - 1) / kLnWarps), kLnWarps * 32, 0, s>>>(
+      reinterpret_cast<const __nv_bfloat16*>(x), gamma, beta, reinterpret_cast<__nv_bfloat16*>(y), rows, C, eps, nullptr,
+      nullptr);
+}
+
+void layernorm_e4m3_fwd(const void* x, const float* gamma, const float* beta, void* y, void* q, float* sa, int64_t rows,
+                        int C, float eps, cudaStream_t s) {
+  if (rows <= 0) return;
+  layernorm_kernel<true><<<(unsigned)((rows + kLnWarps - 1) / kLnWarps), kLnWarps * 32, 0, s>>>(
+      reinterpret_cast<const __nv_bfloat16*>(x), gamma, beta, reinterpret_cast<__nv_bfloat16*>(y), rows, C, eps,
+      reinterpret_cast<uint8_t*>(q), sa);
 }
 
 void embedding_layernorm_fwd(const int64_t* ids, const int64_t* pos_ids, const int64_t* seg_ids, const void* word,
@@ -123,10 +189,21 @@ void embedding_layernorm_fwd(const int64_t* ids, const int64_t* pos_ids, const i
                              const float* gamma, const float* beta, void* y, int64_t rows, int C, float eps, int* err,
                              cudaStream_t s) {
   if (rows <= 0) return;
-  embedding_layernorm_kernel<<<(unsigned)((rows + kLnWarps - 1) / kLnWarps), kLnWarps * 32, 0, s>>>(
+  embedding_layernorm_kernel<false><<<(unsigned)((rows + kLnWarps - 1) / kLnWarps), kLnWarps * 32, 0, s>>>(
       ids, pos_ids, seg_ids, reinterpret_cast<const __nv_bfloat16*>(word), n_word,
       reinterpret_cast<const __nv_bfloat16*>(pos), n_pos, reinterpret_cast<const __nv_bfloat16*>(seg), n_seg, gamma,
-      beta, reinterpret_cast<__nv_bfloat16*>(y), rows, C, eps, err);
+      beta, reinterpret_cast<__nv_bfloat16*>(y), rows, C, eps, err, nullptr, nullptr);
+}
+
+void embedding_layernorm_e4m3_fwd(const int64_t* ids, const int64_t* pos_ids, const int64_t* seg_ids, const void* word,
+                                  int64_t n_word, const void* pos, int64_t n_pos, const void* seg, int64_t n_seg,
+                                  const float* gamma, const float* beta, void* y, void* q, float* sa, int64_t rows, int C,
+                                  float eps, int* err, cudaStream_t s) {
+  if (rows <= 0) return;
+  embedding_layernorm_kernel<true><<<(unsigned)((rows + kLnWarps - 1) / kLnWarps), kLnWarps * 32, 0, s>>>(
+      ids, pos_ids, seg_ids, reinterpret_cast<const __nv_bfloat16*>(word), n_word,
+      reinterpret_cast<const __nv_bfloat16*>(pos), n_pos, reinterpret_cast<const __nv_bfloat16*>(seg), n_seg, gamma,
+      beta, reinterpret_cast<__nv_bfloat16*>(y), rows, C, eps, err, reinterpret_cast<uint8_t*>(q), sa);
 }
 
 }  // namespace edl

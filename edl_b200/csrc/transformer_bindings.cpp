@@ -1,4 +1,4 @@
-// torch bindings for the Transformer encoder kernels (attention.cu, layernorm.cu).
+// torch bindings for the Transformer encoder kernels (attention.cu, layernorm.cu and its quantising variants).
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -98,6 +98,55 @@ void embedding_layernorm_fwd(const Tensor& ids, const Tensor& pos_ids, const Ten
                                err.data_ptr<int>(), at::cuda::getCurrentCUDAStream().stream());
 }
 
+// q uint8 [rows, C] (contiguous), sa fp32 [ceil(C/128), rows]: the block quantisation of the stored y
+void check_quant_out(const Tensor& y, const Tensor& q, const Tensor& sa) {
+  const int64_t rows = y.size(0), C = y.size(1);
+  TORCH_CHECK(q.is_cuda() && q.device() == y.device() && q.element_size() == 1 && q.is_contiguous() && q.dim() == 2 &&
+              q.size(0) == rows && q.size(1) == C && reinterpret_cast<uintptr_t>(q.data_ptr()) % 8 == 0,
+              "q must be a contiguous, 8-byte aligned 1-byte [rows, C] tensor");
+  TORCH_CHECK(sa.is_cuda() && sa.device() == y.device() && sa.scalar_type() == at::kFloat && sa.is_contiguous() &&
+              sa.dim() == 2 && sa.size(0) == (C + 127) / 128 && sa.size(1) == rows,
+              "sa must be contiguous fp32 [ceil(C/128), rows]");
+}
+
+void layernorm_e4m3_fwd(const Tensor& x, const Tensor& gamma, const Tensor& beta, Tensor& y, Tensor& q, Tensor& sa,
+                        double eps) {
+  check_bf16_2d(x, "x");
+  check_bf16_2d(y, "y");
+  const int64_t C = x.size(1);
+  TORCH_CHECK(edl::layernorm_supported((int)C) && y.sizes() == x.sizes(), "layernorm: C % 8 == 0, 8 <= C <= 1024");
+  check_affine(gamma, beta, C);
+  check_quant_out(y, q, sa);
+  c10::cuda::CUDAGuard guard(x.device());
+  edl::layernorm_e4m3_fwd(x.data_ptr(), gamma.data_ptr<float>(), beta.data_ptr<float>(), y.data_ptr(), q.data_ptr(),
+                          sa.data_ptr<float>(), x.size(0), (int)C, (float)eps, at::cuda::getCurrentCUDAStream().stream());
+}
+
+void embedding_layernorm_e4m3_fwd(const Tensor& ids, const Tensor& pos_ids, const Tensor& seg_ids, const Tensor& word,
+                                  const Tensor& pos, const Tensor& seg, const Tensor& gamma, const Tensor& beta,
+                                  Tensor& y, Tensor& q, Tensor& sa, double eps, Tensor& err) {
+  const int64_t rows = ids.numel();
+  for (const Tensor* t : {&ids, &pos_ids, &seg_ids})
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kLong && t->is_contiguous() && t->numel() == rows,
+                "ids: contiguous int64 CUDA tensors of one size");
+  check_bf16_2d(word, "word");
+  check_bf16_2d(pos, "pos");
+  check_bf16_2d(seg, "seg");
+  check_bf16_2d(y, "y");
+  const int64_t C = word.size(1);
+  TORCH_CHECK(edl::layernorm_supported((int)C) && pos.size(1) == C && seg.size(1) == C && y.size(0) == rows &&
+              y.size(1) == C, "embedding_layernorm: tables and output of one width C, C % 8 == 0, 8 <= C <= 1024");
+  check_affine(gamma, beta, C);
+  check_quant_out(y, q, sa);
+  TORCH_CHECK(err.is_cuda() && err.scalar_type() == at::kInt && err.numel() >= 1, "err: int32 CUDA flag");
+  c10::cuda::CUDAGuard guard(ids.device());
+  edl::embedding_layernorm_e4m3_fwd(ids.data_ptr<int64_t>(), pos_ids.data_ptr<int64_t>(), seg_ids.data_ptr<int64_t>(),
+                                    word.data_ptr(), word.size(0), pos.data_ptr(), pos.size(0), seg.data_ptr(),
+                                    seg.size(0), gamma.data_ptr<float>(), beta.data_ptr<float>(), y.data_ptr(),
+                                    q.data_ptr(), sa.data_ptr<float>(), rows, (int)C, (float)eps, err.data_ptr<int>(),
+                                    at::cuda::getCurrentCUDAStream().stream());
+}
+
 }  // namespace
 
 void register_transformer_bindings(pybind11::module_& m) {
@@ -108,4 +157,6 @@ void register_transformer_bindings(pybind11::module_& m) {
   m.def("layernorm_fwd", &layernorm_fwd);
   m.def("layernorm_supported", &edl::layernorm_supported);
   m.def("embedding_layernorm_fwd", &embedding_layernorm_fwd);
+  m.def("layernorm_e4m3_fwd", &layernorm_e4m3_fwd);
+  m.def("embedding_layernorm_e4m3_fwd", &embedding_layernorm_e4m3_fwd);
 }

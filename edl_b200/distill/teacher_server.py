@@ -158,6 +158,19 @@ def build_model(name):
     return teacher_zoo.build(name)
 
 
+def fp8_scaling(net, requested=None):
+    """The ``--fp8`` scaling for teacher network ``net``.  ``requested`` None picks the model's default: ``block`` for a
+    sequence teacher (one that serves ``forward_requests``), ``tensor`` for an image teacher.  A sequence teacher offers
+    block scaling only: it raises ValueError for any other request."""
+    sequence = hasattr(net, "forward_requests")
+    if requested is None:
+        return "block" if sequence else "tensor"
+    if sequence and requested != "block":
+        raise ValueError("--fp8_scaling %s is not available for a sequence teacher: use --fp8_scaling block "
+                         "(the default for it)" % requested)
+    return requested
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description="EDL teacher inference server")
     ap.add_argument("--model", required=True, help="teacher_zoo name, e.g. resnext101_32x16d / mnist_cnn / ernie_base")
@@ -169,14 +182,23 @@ def main(argv=None):
     ap.add_argument("--thread", type=int, default=4)
     ap.add_argument("--max_batch", type=int, default=64)
     ap.add_argument("--mem_optim", action="store_true", help="accepted for CLI parity; no-op")
-    ap.add_argument("--fp8", action="store_true", help="e4m3 wgmma GEMMs for the 1x1 convolutions")
-    ap.add_argument("--fp8_scaling", choices=("tensor", "block"), default="tensor",
+    ap.add_argument("--fp8", action="store_true",
+                    help="e4m3 wgmma GEMMs for the 1x1 convolutions of an image teacher, or the encoder's linear layers "
+                         "of a sequence teacher")
+    ap.add_argument("--fp8_scaling", choices=("tensor", "block"), default=None,
                     help="with --fp8: 'tensor' = one activation scale per layer, calibrated on random data; 'block' = "
-                         "per-row, per-128-channel activation scales computed as each layer runs (no calibration)")
+                         "per-row, per-128-channel activation scales computed as each layer runs (no calibration). "
+                         "Default: 'tensor' for image teachers, 'block' (the only choice) for sequence teachers")
     args = ap.parse_args(argv)
     logging.basicConfig(level=logging.INFO)
     dev = "cuda:%s" % args.gpu_ids.split(",")[0] if torch.cuda.is_available() else "cpu"
     model, feed_names, fetch_names, feed_shapes = build_model(args.model)
+    scaling = None
+    if args.fp8:
+        try:
+            scaling = fp8_scaling(getattr(model, "net", model), args.fp8_scaling)
+        except ValueError as e:
+            ap.error(str(e))
     if args.weights:
         net = getattr(model, "net", model)
         if hasattr(net, "load_weights"):
@@ -189,7 +211,7 @@ def main(argv=None):
     srv = TeacherServer(model, feed_names, fetch_names, feed_shapes, device=dev, dtype=dtype, port=args.port,
                         max_batch=args.max_batch, workers=max(4, args.thread))
     net = getattr(srv.model, "net", srv.model)
-    if args.fp8 and dev.startswith("cuda") and hasattr(net, "enable_fp8") and args.fp8_scaling == "block":
+    if args.fp8 and dev.startswith("cuda") and hasattr(net, "enable_fp8") and scaling == "block":
         logging.info("fp8 (block-scaled): converted %d layers", net.enable_fp8(scaling="block"))
     elif args.fp8 and dev.startswith("cuda") and hasattr(net, "enable_fp8"):
         shape = feed_shapes[feed_names[0]]

@@ -12,7 +12,13 @@ forward after a load or a move; biases and LayerNorm parameters stay fp32.  On C
 PyTorch math (the reference the GPU path is tested against).
 
 ``forward_packed`` runs the same layers on a batch packed to its real tokens (``pack_sequences``) with the
-variable-length attention kernel; ``forward_requests`` packs requests of different lengths for the teacher server."""
+variable-length attention kernel; ``forward_requests`` packs requests of different lengths for the teacher server.
+
+``enable_fp8()`` switches the four linear layers of every encoder layer to the block-scaled e4m3 GEMM (ops/fp8.py):
+the LayerNorms write the next GEMM's quantised operand themselves, FFN1's epilogue quantises its GELU output for FFN2,
+and the residual adds run in the out-projection's and FFN2's epilogues.  The attention output is quantised by
+``quantize_e4m3_blocks``.  Embeddings, attention, pooler and classifier stay bf16.  On CPU an enabled model emulates
+that pipeline through the float32 paths of the same ops, rounding to bf16 wherever the GPU stores bf16."""
 from __future__ import annotations
 
 import numpy as np
@@ -21,6 +27,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import ops
+from ..ops import fp8
 
 CLS_PAD = 8      # classifier rows after padding: a 2-class output row (4 bytes) is not a TMA-describable pitch
 
@@ -91,6 +98,18 @@ class ErnieEncoder(nn.Module):
         self.cls_w, self.cls_b = mat(num_labels, hidden), vec(num_labels)
         self.requires_grad_(False)
         self._dev = None          # CUDA copies of the weights (bf16 matrices, fp32 vectors), built at first use
+        self._fp8 = False         # enable_fp8: the encoder's linear layers run block-scaled e4m3
+
+    def enable_fp8(self, scaling="block"):
+        """Run QKV, out-projection, FFN1 and FFN2 of every layer as block-scaled e4m3 GEMMs: one scale per activation
+        row and 128-element K block, computed on the fly, and one per 128 x 128 weight block (no calibration, no host
+        synchronisation).  Returns the number of converted linear layers (4 per encoder layer).  Only ``"block"``
+        scaling is offered: a per-tensor activation scale needs a calibration pass."""
+        if scaling != "block":
+            raise ValueError("ErnieEncoder.enable_fp8: scaling %r is not supported; use 'block'" % (scaling,))
+        self._fp8 = True
+        self._dev = None
+        return 4 * self.num_layers
 
     def _apply(self, fn, *args, **kwargs):
         self._dev = None
@@ -105,6 +124,12 @@ class ErnieEncoder(nn.Module):
             def v(t):
                 return t.detach().float().contiguous()
 
+            if self._fp8:                         # (e4m3 bytes, block scales); no bf16 copy of these matrices
+                def m_lin(t):
+                    return fp8.quantize_weight_blocks(t.detach())
+            else:
+                m_lin = m
+
             n, c = self.num_labels, self.hidden
             cls_w = torch.zeros(max(CLS_PAD, -(-n // CLS_PAD) * CLS_PAD), c, device=self.cls_w.device)
             cls_w[:n] = self.cls_w.detach().float()
@@ -113,8 +138,8 @@ class ErnieEncoder(nn.Module):
             self._dev = {
                 "emb": (m(self.word_emb), m(self.pos_emb), m(self.seg_emb), v(self.emb_ln_g), v(self.emb_ln_b)),
                 "layers": [tuple(f(getattr(lyr, k)) for f, k in (
-                    (m, "qkv_w"), (v, "qkv_b"), (m, "out_w"), (v, "out_b"), (v, "ln1_g"), (v, "ln1_b"),
-                    (m, "ffn1_w"), (v, "ffn1_b"), (m, "ffn2_w"), (v, "ffn2_b"), (v, "ln2_g"), (v, "ln2_b")))
+                    (m_lin, "qkv_w"), (v, "qkv_b"), (m_lin, "out_w"), (v, "out_b"), (v, "ln1_g"), (v, "ln1_b"),
+                    (m_lin, "ffn1_w"), (v, "ffn1_b"), (m_lin, "ffn2_w"), (v, "ffn2_b"), (v, "ln2_g"), (v, "ln2_b")))
                     for lyr in self.layers],
                 "head": (m(self.pool_w), v(self.pool_b), m(cls_w), v(cls_b)),
             }
@@ -227,6 +252,8 @@ class ErnieEncoder(nn.Module):
         return self.forward_packed(ids, pos, seg, cu, max(p[4] for p in packs), key_mask)
 
     def _forward_cuda(self, ids, pos, seg, attend, cls_rows):
+        if self._fp8:
+            return self._forward_fp8(ids, pos, seg, attend, cls_rows)
         w = self._device_weights()
         word, pemb, semb, g, beta = w["emb"]
         x = ops.embedding_layernorm(ids, pos, seg, word, pemb, semb, g, beta, self.eps)
@@ -240,7 +267,35 @@ class ErnieEncoder(nn.Module):
         pooled = torch.tanh(ops.linear_bf16(cls_rows(x), pool_w, pool_b))
         return ops.gemm_bf16(pooled, cls_w, col_shift=cls_b)[:, :self.num_labels].float()
 
+    def _forward_fp8(self, ids, pos, seg, attend, cls_rows):
+        """The FP8 layer flow; on CPU every op takes its float32 reference path on bf16 activations, which makes this
+        the emulation the CUDA path is tested against."""
+        w = self._device_weights()
+        word, pemb, semb, g, beta = w["emb"]
+        x, q, sa = ops.embedding_layernorm_e4m3(ids, pos, seg, word, pemb, semb, g, beta, self.eps)
+        last = len(w["layers"]) - 1
+        for i, (qkv_w, qkv_b, out_w, out_b, ln1_g, ln1_b, f1_w, f1_b, f2_w, f2_b, ln2_g, ln2_b) in enumerate(w["layers"]):
+            qkv = fp8.gemm_fp8_blockscaled(q, sa, *qkv_w, col_shift=qkv_b)
+            q, sa = fp8.quantize_e4m3_blocks(attend(qkv))
+            x, q, sa = ops.layer_norm_e4m3(fp8.gemm_fp8_blockscaled(q, sa, *out_w, col_shift=out_b, add=x),
+                                           ln1_g, ln1_b, self.eps)
+            q, sa = fp8.gemm_fp8_gelu_e4m3(q, sa, *f1_w, bias=f1_b)
+            h = fp8.gemm_fp8_blockscaled(q, sa, *f2_w, col_shift=f2_b, add=x)
+            if i < last:
+                x, q, sa = ops.layer_norm_e4m3(h, ln2_g, ln2_b, self.eps)
+            else:                                  # the pooler reads bf16 x only
+                x = ops.layer_norm(h, ln2_g, ln2_b, self.eps)
+        pool_w, pool_b, cls_w, cls_b = w["head"]
+        if x.is_cuda:
+            pooled = torch.tanh(ops.linear_bf16(cls_rows(x), pool_w, pool_b))
+            return ops.gemm_bf16(pooled, cls_w, col_shift=cls_b)[:, :self.num_labels].float()
+        bf = torch.bfloat16
+        pooled = torch.tanh(F.linear(cls_rows(x).float(), pool_w.float(), pool_b).to(bf))
+        return F.linear(pooled.float(), cls_w.float(), cls_b).to(bf)[:, :self.num_labels].float()
+
     def _forward_reference(self, ids, pos, seg, attend, cls_rows):
+        if self._fp8:
+            return self._forward_fp8(ids, pos, seg, attend, cls_rows)
         f32 = torch.float32
         x = ops.embedding_layernorm(ids, pos, seg, self.word_emb.to(f32), self.pos_emb.to(f32), self.seg_emb.to(f32),
                                     self.emb_ln_g, self.emb_ln_b, self.eps)

@@ -97,7 +97,8 @@ from .misc import rope, rope_tables, embedding_bag_mean, normalize_u8, DynamicLo
 from .embedding import embedding_bag_mean_sparse, embedding_bags_mean_sparse  # noqa: E402
 from .transformer import (attention, attention_supported, layer_norm, layer_norm_supported,  # noqa: E402
                           embedding_layernorm, embedding_layernorm_supported, attention_varlen,
-                          attention_varlen_supported)
+                          attention_varlen_supported, layer_norm_e4m3, layer_norm_e4m3_supported,
+                          embedding_layernorm_e4m3, embedding_layernorm_e4m3_supported)
 
 __all__ = [
     "native", "native_available", "launches", "reset_launches", "count_fallback", "fallbacks", "reset_fallbacks",
@@ -112,5 +113,6 @@ __all__ = [
     "stem_conv", "stem_conv_supported", "conv3x3_pair", "conv3x3_pair_supported",
     "rope", "rope_tables", "embedding_bag_mean", "normalize_u8", "DynamicLossScaler", "set_fused_bn", "set_relu_mask",
     "drop_bn_hook", "attention", "attention_supported", "layer_norm", "layer_norm_supported", "embedding_layernorm",
-    "embedding_layernorm_supported", "attention_varlen", "attention_varlen_supported",
+    "embedding_layernorm_supported", "attention_varlen", "attention_varlen_supported", "layer_norm_e4m3",
+    "layer_norm_e4m3_supported", "embedding_layernorm_e4m3", "embedding_layernorm_e4m3_supported",
 ]

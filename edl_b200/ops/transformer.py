@@ -3,7 +3,10 @@ the inference path of the ERNIE / BERT sequence teacher (models/ernie.py).
 
 Dispatch rule of the package: CPU tensors run the small float32 reference implementations below; on CUDA a shape a
 kernel cannot take (head dim other than 64, sequences longer than 512, a hidden size above 1024 or not a multiple of 8)
-runs the same reference math on the library through ``count_fallback``."""
+runs the same reference math on the library through ``count_fallback``.
+
+``layer_norm_e4m3`` and ``embedding_layernorm_e4m3`` also return the block-scaled e4m3 copy of their bf16 output
+(``ops.fp8.quantize_e4m3_blocks``), written by the same kernel, for the FP8 teacher's next GEMM."""
 from __future__ import annotations
 
 import torch
@@ -197,3 +200,66 @@ def embedding_layernorm(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps=
         for t, tab, what in ((ids, word, "input id"), (pos_ids, pos, "position id"), (seg_ids, seg, "segment id")):
             _check_ids(t, tab.shape[0], what)
     return out
+
+
+# ------------------------------------------------------------------------------------- LayerNorm with e4m3 output
+def _quant_out(y):
+    from .fp8 import BLOCK
+
+    rows, c = y.shape
+    return (torch.empty((rows, c), dtype=torch.uint8, device=y.device),
+            torch.empty((-(-c // BLOCK), rows), dtype=torch.float32, device=y.device))
+
+
+def layer_norm_e4m3_supported(x) -> bool:
+    return layer_norm_supported(x)
+
+
+def layer_norm_e4m3(x, gamma, beta, eps=1e-12):
+    """``layer_norm`` that also quantises its output for a block-scaled FP8 GEMM: returns (y bf16 [rows, C],
+    q uint8 e4m3 [rows, C], sa fp32 [ceil(C/128), rows]) with (q, sa) bit for bit ``quantize_e4m3_blocks(y)``.
+    On CPU (and for a shape the kernel cannot take) it is exactly that composition of the references."""
+    from . import native, count_launch
+    from .fp8 import quantize_e4m3_blocks_reference
+
+    if x.is_cuda and layer_norm_e4m3_supported(x):
+        y = torch.empty_like(x)
+        q, sa = _quant_out(y)
+        native().layernorm_e4m3_fwd(x, gamma.float().contiguous(), beta.float().contiguous(), y, q, sa, float(eps))
+        count_launch()
+        return y, q, sa
+    if x.is_cuda:
+        _count("layer_norm_e4m3: no kernel for %s %s: float32 math on the library" % (tuple(x.shape), x.dtype))
+    y = layer_norm_reference(x, gamma, beta, eps)
+    return (y,) + quantize_e4m3_blocks_reference(y)
+
+
+def embedding_layernorm_e4m3_supported(word, pos, seg) -> bool:
+    return embedding_layernorm_supported(word, pos, seg)
+
+
+def embedding_layernorm_e4m3(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps=1e-12):
+    """``embedding_layernorm`` that also returns the block-scaled e4m3 copy of its output: (y, q, sa) as in
+    ``layer_norm_e4m3``.  Out-of-range ids are handled as in ``embedding_layernorm`` (checked after the launch except
+    under CUDA-graph capture)."""
+    from . import native, count_launch
+    from .fp8 import quantize_e4m3_blocks_reference
+
+    if word.is_cuda and embedding_layernorm_e4m3_supported(word, pos, seg):
+        rows = ids.numel()
+        y = torch.empty((rows, word.shape[1]), device=word.device, dtype=torch.bfloat16)
+        q, sa = _quant_out(y)
+        err = torch.zeros(1, dtype=torch.int32, device=word.device)
+        ids, pos_ids, seg_ids = (t.reshape(-1).to(word.device, torch.int64).contiguous() for t in (ids, pos_ids, seg_ids))
+        native().embedding_layernorm_e4m3_fwd(ids, pos_ids, seg_ids, word, pos, seg, gamma.float().contiguous(),
+                                              beta.float().contiguous(), y, q, sa, float(eps), err)
+        count_launch()
+        if not torch.cuda.is_current_stream_capturing() and int(err.item()) != 0:
+            for t, tab, what in ((ids, word, "input id"), (pos_ids, pos, "position id"), (seg_ids, seg, "segment id")):
+                _check_ids(t, tab.shape[0], what)
+        return y, q, sa
+    if word.is_cuda:
+        _count("embedding_layernorm_e4m3: no kernel for width %d %s: float32 math on the library"
+               % (word.shape[1], word.dtype))
+    y = embedding_layernorm_reference(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps)
+    return (y,) + quantize_e4m3_blocks_reference(y)

@@ -8,12 +8,15 @@ Workload: ``ernie_base`` with random weights, batch 16, right-padded masks whose
 ``ErnieEncoder.forward`` on the wgmma GEMM (bias / residual / GELU epilogues), the attention, LayerNorm and
 embedding-LayerNorm kernels; "packed" is a CUDA-graph replay of ``forward_packed`` on the same samples packed to their
 real tokens (the varlen attention kernel, every other layer on T rows instead of B * L); "torch" is a CUDA-graph replay
-of the padded forward in bf16 on cuBLAS linear, ``F.scaled_dot_product_attention`` and ``F.layer_norm``.  The three
-alternate in timed windows of device-timed replays.  FLOPs are counted from shapes: ``gflop`` over the full padded
+of the padded forward in bf16 on cuBLAS linear, ``F.scaled_dot_product_attention`` and ``F.layer_norm``; "fp8" is a
+CUDA-graph replay of ``forward_packed`` on a copy of the model after ``enable_fp8()`` (block-scaled e4m3 linear layers),
+reported with its logits cosine and top-1 agreement against the bf16 packed arm (the classifier weights are scaled by 20
+so that the random model's top-1 is decisive).  The four alternate in timed windows of device-timed replays.  FLOPs are counted from shapes: ``gflop`` over the full padded
 length (what the padded forwards compute), ``gflop_real`` over the real tokens only (GEMM rows T, attention len_b^2 per
 sequence), the work every arm has to do; the shares of peak are against the H100 SXM data-sheet dense bf16 rate
 (989 TFLOP/s at 700 W), so they are end-to-end figures, not a kernel's."""
 import argparse
+import copy
 import json
 import os
 import subprocess
@@ -84,6 +87,28 @@ def flops(model, b, l, lens=None):
     return gemm, attn
 
 
+def split(avgs):
+    """Device time (ms over the profiled replays) per kernel group of a profiler ``key_averages()``."""
+    groups = (("fp8 GEMM, GELU -> e4m3 epilogue (FFN1)", ("gemm_fp8_wgmma_kernel", "Fp8BlockQParams")),
+              ("fp8 GEMM, residual epilogue (out-proj, FFN2)", ("gemm_fp8_wgmma_kernel", ", 1>")),
+              ("fp8 GEMM, bias epilogue (QKV)", ("gemm_fp8_wgmma_kernel",)),
+              ("ctx quantiser", ("quantize_e4m3_blocks_kernel",)),
+              ("LayerNorm (with e4m3 output)", ("layernorm_kernel<true>",)),
+              ("LayerNorm", ("layernorm_kernel",)),
+              ("bf16 GEMM", ("gemm",)),
+              ("attention", ("attention",)))
+    out = {}
+    for e in avgs:
+        t = getattr(e, "device_time_total", None)
+        t = e.cuda_time_total if t is None else t
+        if t <= 0:
+            continue
+        name = next((g for g, keys in groups if all(k in e.key for k in keys)), "other")
+        out[name] = out.get(name, 0.0) + t / 1e3
+    total = sum(out.values())
+    return {k: {"ms": round(v, 4), "share": round(v / total, 4)} for k, v in sorted(out.items(), key=lambda kv: -kv[1])}
+
+
 def capture(fn, args):
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -119,6 +144,10 @@ def main():
         raise SystemExit("bench_ernie.py measures on a GPU; none found")
     torch.manual_seed(0)
     model = ernie.ernie_base().cuda().eval()
+    with torch.no_grad():
+        model.cls_w.mul_(20)                  # decisive logits for the FP8 arm's top-1 agreement
+    model8 = copy.deepcopy(model)
+    model8.enable_fp8()
     info = card()
     for l in args.lens:
         feed = inputs(args.batch, l, l)
@@ -129,9 +158,11 @@ def main():
         lens = packed[3].diff().tolist()
         packed = [p.cuda() if torch.is_tensor(p) else p for p in packed]
         g_pack, out_pack = capture(model.forward_packed, packed)
+        g_fp8, out_fp8 = capture(model8.forward_packed, packed)
         g_ours.replay()
         g_ref.replay()
         g_pack.replay()
+        g_fp8.replay()
         torch.cuda.synchronize()
 
         def cosine(a, b):
@@ -141,27 +172,30 @@ def main():
             from torch.profiler import ProfilerActivity, profile
 
             os.makedirs(args.profile, exist_ok=True)
-            for name, g in (("ours", g_ours), ("packed", g_pack), ("torch", g_ref)):
+            for name, g in (("ours", g_ours), ("packed", g_pack), ("torch", g_ref), ("fp8_packed", g_fp8)):
                 with profile(activities=[ProfilerActivity.CUDA]) as prof:
                     for _ in range(5):
                         g.replay()
                     torch.cuda.synchronize()
-                table = prof.key_averages().table(sort_by="cuda_time_total", row_limit=25)
+                avgs = prof.key_averages()
+                table = avgs.table(sort_by="cuda_time_total", row_limit=25)
                 with open(os.path.join(args.profile, "ernie_L%d_%s.txt" % (l, name)), "w") as fh:
                     fh.write(table)
                 print("== L %d %s (5 replays) ==\n%s" % (l, name, table))
+                print(json.dumps({"L": l, "arm": name, "card": info, "kernel_time_split": split(avgs)}), flush=True)
             continue
-        for g in (g_ours, g_pack, g_ref):
+        for g in (g_ours, g_pack, g_ref, g_fp8):
             timed(g, 5)
-        t_ours, t_pack, t_ref = [], [], []
+        t_ours, t_pack, t_ref, t_fp8 = [], [], [], []
         for _ in range(args.windows):
             t_ours.append(timed(g_ours, args.reps))
             t_pack.append(timed(g_pack, args.reps))
             t_ref.append(timed(g_ref, args.reps))
+            t_fp8.append(timed(g_fp8, args.reps))
         gemm, attn = flops(model, args.batch, l)
         real = sum(flops(model, args.batch, l, lens))
-        best_o, best_p, best_r = min(t_ours), min(t_pack), min(t_ref)
-        med_o, med_p, med_r = (sorted(t)[len(t) // 2] for t in (t_ours, t_pack, t_ref))
+        best_o, best_p, best_r, best_8 = min(t_ours), min(t_pack), min(t_ref), min(t_fp8)
+        med_o, med_p, med_r, med_8 = (sorted(t)[len(t) // 2] for t in (t_ours, t_pack, t_ref, t_fp8))
         print(json.dumps({
             "workload": "ernie_base forward, B %d, L %d, padded masks" % (args.batch, l),
             "card": info, "fallbacks": ops.fallbacks(), "logits_cosine_vs_torch": round(cos, 6),
@@ -183,7 +217,12 @@ def main():
             "ours_share_of_bf16_peak": round((gemm + attn) / med_o / PEAK_BF16, 3),
             "torch_share_of_bf16_peak": round((gemm + attn) / med_r / PEAK_BF16, 3),
             "real_tflops": {k: round(real / t / 1e12, 1) for k, t in (("ours", med_o), ("packed", med_p),
-                                                                      ("torch", med_r))},
+                                                                      ("torch", med_r), ("fp8_packed", med_8))},
+            "fp8_packed_seq_per_s": round(args.batch / med_8, 1), "fp8_packed_ms_median": round(med_8 * 1e3, 4),
+            "fp8_packed_ms_best": round(best_8 * 1e3, 4),
+            "fp8_speedup_vs_bf16_packed_median": round(med_p / med_8, 3),
+            "fp8_logits_cosine_vs_bf16_packed": round(cosine(out_fp8, out_pack), 6),
+            "fp8_top1_agreement_vs_bf16_packed": float((out_fp8.argmax(1) == out_pack.argmax(1)).float().mean()),
         }), flush=True)
 
 
