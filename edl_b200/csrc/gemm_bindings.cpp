@@ -316,13 +316,39 @@ void conv1x1_s2_wgrad(const Tensor& x, const Tensor& dy, Tensor& dw, int64_t spl
   TORCH_CHECK(err == nullptr, "edl conv1x1_s2_wgrad failed: ", err);
 }
 
+inline bool aligned16(const Tensor& t) { return reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0; }
+
+// The operand checks shared by every fp8 GEMM entry: A [M, K] and B [N, K] hold e4m3 bytes, D is [M, N] (bf16, or e4m3
+// bytes for the GELU epilogue), all on one CUDA device with 16-byte aligned bases and rows, K % 16 == 0; col_scale /
+// col_shift (optional) are contiguous fp32 [N] on that device.
+void fp8_gemm_checks(const Tensor& A, const Tensor& B, const Tensor& D, const c10::optional<Tensor>& col_scale,
+                     const c10::optional<Tensor>& col_shift, bool q_out) {
+  TORCH_CHECK(A.is_cuda() && B.is_cuda() && D.is_cuda() && A.dim() == 2 && B.dim() == 2 && D.dim() == 2,
+              "A, B and D must be 2-D CUDA tensors");
+  TORCH_CHECK(A.device() == B.device() && A.device() == D.device(), "A, B and D on different devices");
+  TORCH_CHECK(A.element_size() == 1 && B.element_size() == 1, "A and B hold e4m3 bytes");
+  if (q_out) {
+    TORCH_CHECK(D.element_size() == 1, "the GELU e4m3 epilogue writes e4m3 bytes");
+  } else {
+    TORCH_CHECK(D.scalar_type() == at::kBFloat16, "D must be bf16");
+  }
+  TORCH_CHECK(A.stride(1) == 1 && B.stride(1) == 1 && D.stride(1) == 1, "operands need a contiguous last dim");
+  TORCH_CHECK(A.size(1) == B.size(1), "K mismatch: ", A.size(1), " vs ", B.size(1));
+  TORCH_CHECK(D.size(0) == A.size(0) && D.size(1) == B.size(0), "D must be [M, N]");
+  TORCH_CHECK(A.size(1) % 16 == 0 && A.stride(0) % 16 == 0 && B.stride(0) % 16 == 0 &&
+              D.stride(0) % (q_out ? 16 : 8) == 0, "fp8 GEMM needs 16-byte aligned rows");
+  TORCH_CHECK(aligned16(A) && aligned16(B) && aligned16(D), "A, B and D must be 16-byte aligned");
+  for (const auto* t : {&col_scale, &col_shift})
+    if (t->has_value() && (*t)->defined())
+      TORCH_CHECK((*t)->is_cuda() && (*t)->device() == A.device() && (*t)->scalar_type() == at::kFloat &&
+                  (*t)->is_contiguous() && (*t)->numel() == B.size(0),
+                  "col_scale / col_shift must be contiguous fp32 [N] on the operands' device");
+}
+
 // D bf16 [M,N] = relu?((A8[M,K] * B8[N,K]^T) * col_scale + col_shift); A8/B8 are e4m3 bytes (uint8 / float8 tensors)
 void gemm_fp8(const Tensor& A, const Tensor& B, Tensor& D, const c10::optional<Tensor>& col_scale,
               const c10::optional<Tensor>& col_shift, bool relu) {
-  TORCH_CHECK(A.is_cuda() && B.is_cuda() && A.dim() == 2 && B.dim() == 2 && D.dim() == 2);
-  TORCH_CHECK(A.element_size() == 1 && B.element_size() == 1 && D.scalar_type() == at::kBFloat16);
-  TORCH_CHECK(A.stride(1) == 1 && B.stride(1) == 1 && D.stride(1) == 1 && A.size(1) == B.size(1));
-  TORCH_CHECK(D.size(0) == A.size(0) && D.size(1) == B.size(0));
+  fp8_gemm_checks(A, B, D, col_scale, col_shift, false);
   edl::GemmFp8Args g;
   g.A = A.data_ptr();
   g.B = B.data_ptr();
@@ -342,10 +368,19 @@ void gemm_fp8(const Tensor& A, const Tensor& B, Tensor& D, const c10::optional<T
   TORCH_CHECK(err == nullptr, "edl gemm_fp8 failed: ", err);
 }
 
+// q = sat(x / scale) as e4m3 bytes, x bf16 (read as 16-byte vectors), q written 8 bytes at a time; scale and the
+// optional running max|x| `amax` are fp32 device scalars the kernel dereferences
 void quantize_e4m3(const Tensor& x, Tensor& q, const Tensor& scale, const c10::optional<Tensor>& amax) {
-  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && x.is_contiguous());
-  TORCH_CHECK(q.is_cuda() && q.element_size() == 1 && q.is_contiguous() && q.numel() == x.numel());
-  TORCH_CHECK(scale.scalar_type() == at::kFloat && scale.numel() >= 1);
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && x.is_contiguous(), "x must be a contiguous bf16 CUDA tensor");
+  TORCH_CHECK(aligned16(x), "x must be 16-byte aligned");
+  TORCH_CHECK(q.is_cuda() && q.device() == x.device() && q.element_size() == 1 && q.is_contiguous() &&
+              q.numel() == x.numel(), "q must be a contiguous 1-byte tensor of x's size on x's device");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(q.data_ptr()) % 8 == 0, "q must be 8-byte aligned");
+  TORCH_CHECK(scale.is_cuda() && scale.device() == x.device() && scale.scalar_type() == at::kFloat && scale.numel() >= 1,
+              "scale must be an fp32 tensor on x's device");
+  if (amax.has_value() && amax->defined())
+    TORCH_CHECK(amax->is_cuda() && amax->device() == x.device() && amax->scalar_type() == at::kFloat &&
+                amax->numel() >= 1, "amax must be an fp32 tensor on x's device");
   c10::cuda::CUDAGuard guard(x.device());
   edl::quantize_e4m3(x.data_ptr(), q.data_ptr(), x.numel(), scale.data_ptr<float>(), optp<float>(amax),
                      at::cuda::getCurrentCUDAStream().stream());
@@ -375,29 +410,13 @@ void quantize_e4m3_blocks(const Tensor& x, Tensor& q, Tensor& sa) {
 edl::GemmFp8Args blockscaled_args(const Tensor& A, const Tensor& sa, const Tensor& B, const Tensor& sb, const Tensor& D,
                                   const c10::optional<Tensor>& col_scale, const c10::optional<Tensor>& col_shift,
                                   bool relu, bool q_out) {
-  TORCH_CHECK(A.is_cuda() && B.is_cuda() && D.is_cuda() && A.dim() == 2 && B.dim() == 2 && D.dim() == 2);
-  TORCH_CHECK(A.element_size() == 1 && B.element_size() == 1, "A and B hold e4m3 bytes");
-  if (q_out) {
-    TORCH_CHECK(D.element_size() == 1, "the GELU e4m3 epilogue writes e4m3 bytes");
-  } else {
-    TORCH_CHECK(D.scalar_type() == at::kBFloat16, "D must be bf16");
-  }
-  TORCH_CHECK(A.stride(1) == 1 && B.stride(1) == 1 && D.stride(1) == 1, "operands need a contiguous last dim");
-  TORCH_CHECK(A.size(1) == B.size(1), "K mismatch: ", A.size(1), " vs ", B.size(1));
-  TORCH_CHECK(D.size(0) == A.size(0) && D.size(1) == B.size(0), "D must be [M, N]");
+  fp8_gemm_checks(A, B, D, col_scale, col_shift, q_out);
   const int64_t M = A.size(0), N = B.size(0), K = A.size(1), kb = (K + 127) / 128;
-  TORCH_CHECK(K % 16 == 0 && A.stride(0) % 16 == 0 && B.stride(0) % 16 == 0 && D.stride(0) % (q_out ? 16 : 8) == 0,
-              "fp8 GEMM needs 16-byte aligned rows");
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(A.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(B.data_ptr()) % 16 == 0 &&
-              reinterpret_cast<uintptr_t>(D.data_ptr()) % 16 == 0, "A, B and D must be 16-byte aligned");
-  TORCH_CHECK(sa.is_cuda() && sa.scalar_type() == at::kFloat && sa.is_contiguous() && sa.dim() == 2 &&
-              sa.size(0) == kb && sa.size(1) == M, "sa must be contiguous fp32 [ceil(K/128), M]");
-  TORCH_CHECK(sb.is_cuda() && sb.scalar_type() == at::kFloat && sb.is_contiguous() && sb.dim() == 2 &&
-              sb.size(0) == (N + 127) / 128 && sb.size(1) == kb, "sb must be contiguous fp32 [ceil(N/128), ceil(K/128)]");
-  for (const auto* t : {&col_scale, &col_shift})
-    if (t->has_value() && (*t)->defined())
-      TORCH_CHECK((*t)->is_cuda() && (*t)->scalar_type() == at::kFloat && (*t)->is_contiguous() && (*t)->numel() == N,
-                  "col_scale / col_shift must be contiguous fp32 [N]");
+  TORCH_CHECK(sa.is_cuda() && sa.device() == A.device() && sa.scalar_type() == at::kFloat && sa.is_contiguous() &&
+              sa.dim() == 2 && sa.size(0) == kb && sa.size(1) == M, "sa must be contiguous fp32 [ceil(K/128), M]");
+  TORCH_CHECK(sb.is_cuda() && sb.device() == A.device() && sb.scalar_type() == at::kFloat && sb.is_contiguous() &&
+              sb.dim() == 2 && sb.size(0) == (N + 127) / 128 && sb.size(1) == kb,
+              "sb must be contiguous fp32 [ceil(N/128), ceil(K/128)]");
   edl::GemmFp8Args g;
   g.A = A.data_ptr();
   g.B = B.data_ptr();

@@ -36,6 +36,8 @@ class FoldedConv(nn.Module):
         self.register_buffer("scale", torch.ones(cout, dtype=torch.float32))
         self.register_buffer("shift", torch.zeros(cout, dtype=torch.float32))
         self.own_conv3 = os.environ.get("EDL_OWN_CONV3", "1") == "1"
+        self._fp8 = None             # None (bf16), "tensor" or "block": the enabled fp8 mode of a 1x1 convolution
+        self._fp8_cache = None
 
     def load_bn(self, gamma, beta, mean, var, eps=1e-5):
         s = gamma.float() * torch.rsqrt(var.float() + eps)
@@ -84,31 +86,69 @@ class FoldedConv(nn.Module):
         self._amax = torch.zeros(1, dtype=torch.float32, device=self.weight.device)
 
     def finish_calibration(self, margin: float = 1.0):
-        """Freeze the activation scale from the recorded max|x| and quantise the weights per output channel."""
-        from ..ops.fp8 import E4M3_MAX, quantize_weight_rows
+        """Freeze the activation scale from the recorded max|x|; the weights are quantised per output channel."""
+        from ..ops.fp8 import E4M3_MAX
 
         amax = float(self._amax.item()) if getattr(self, "_amax", None) is not None else 0.0
         self._amax = None
         if not self.fp8_eligible() or amax <= 0.0:
             return False
-        q, ws = quantize_weight_rows(self.weight.view(self.cout, self.cin))
-        self.w8 = q
-        self.act_scale = torch.full((1,), amax * margin / E4M3_MAX, dtype=torch.float32, device=q.device)
-        self.deq_scale = (self.act_scale * ws.to(q.device) * self.scale).contiguous()   # act * weight * folded BN
-        self._ones, self._zeros = torch.ones_like(self.scale), torch.zeros_like(self.scale)
+        self.act_scale = torch.full((1,), amax * margin / E4M3_MAX, dtype=torch.float32, device=self.weight.device)
+        self._fp8 = "tensor"
+        self._fp8_cache = None                  # a recalibration: deq_scale carries the new activation scale
+        self._fp8_weights()
         return True
 
     def enable_fp8_blocks(self):
-        """Block-scaled fp8: quantise the weights once per 128x128 block; the input is scaled per row and 128-channel
+        """Block-scaled fp8: the weights are quantised per 128x128 block; the input is scaled per row and 128-channel
         block when the layer runs, so there is nothing to calibrate and no host synchronisation."""
-        from ..ops.fp8 import quantize_weight_blocks
-
         if not self.fp8_eligible():
             return False
-        self.w8 = None                                      # leaves the per-tensor mode
-        self.w8_blocks, self.w_block_scales = quantize_weight_blocks(self.weight.view(self.cout, self.cin))
-        self._ones, self._zeros = torch.ones_like(self.scale), torch.zeros_like(self.scale)
+        self._fp8 = "block"
+        self._fp8_weights()
         return True
+
+    def _fp8_weights(self):
+        """(e4m3 weights, their scales, ones, zeros) of the enabled fp8 mode, quantised from the current weight on its
+        device: rebuilt after a load (``load_state_dict``, ``load_bn``) or a move (``.to()``), like ``_scaled_weight``.
+        Per-tensor: per-output-channel weight scales with the calibrated activation scale and the folded-BN scale
+        multiplied in (``deq_scale``, so it is also keyed on the activation scale); block: one scale per 128x128
+        block."""
+        from ..ops.fp8 import quantize_weight_blocks, quantize_weight_rows
+
+        w, s = self.weight, self.scale
+        key = (self._fp8, w.device, w.data_ptr(), w._version, s.data_ptr(), s._version)
+        if self._fp8 == "tensor":
+            if self.act_scale.device != w.device:
+                self.act_scale = self.act_scale.to(w.device)
+            key += (self.act_scale.data_ptr(), self.act_scale._version)
+        if self._fp8_cache is None or self._fp8_cache[0] != key:
+            w2 = w.detach().view(self.cout, self.cin)
+            if self._fp8 == "block":
+                q, ws = quantize_weight_blocks(w2)
+            else:
+                q, ws = quantize_weight_rows(w2)
+                ws = (self.act_scale * ws.to(q.device) * s).contiguous()     # act * weight * folded BN
+            self._fp8_cache = (key, (q, ws, torch.ones_like(s), torch.zeros_like(s)))
+        return self._fp8_cache[1]
+
+    @property
+    def w8(self):
+        """Per-tensor mode: e4m3 weights [Cout, Cin] (None in the other modes)."""
+        return self._fp8_weights()[0] if self._fp8 == "tensor" else None
+
+    @property
+    def deq_scale(self):
+        return self._fp8_weights()[1] if self._fp8 == "tensor" else None
+
+    @property
+    def w8_blocks(self):
+        """Block mode: e4m3 weights [Cout, Cin] (None in the other modes)."""
+        return self._fp8_weights()[0] if self._fp8 == "block" else None
+
+    @property
+    def w_block_scales(self):
+        return self._fp8_weights()[1] if self._fp8 == "block" else None
 
     def forward(self, x, residual=None):
         fast = (x.is_cuda and x.dtype == torch.bfloat16 and self.k == 1 and self.groups == 1
@@ -122,25 +162,26 @@ class FoldedConv(nn.Module):
             x2 = x.permute(0, 2, 3, 1).reshape(-1, c)
             y = torch.empty((n, self.cout, h, w), device=x.device, dtype=x.dtype, memory_format=torch.channels_last)
             y2 = y.permute(0, 2, 3, 1).reshape(-1, self.cout)
-            if getattr(self, "w8_blocks", None) is not None:
+            if self._fp8 == "block":
                 from ..ops.fp8 import gemm_fp8_blockscaled, quantize_e4m3_blocks
 
+                w8, sb, ones, zeros = self._fp8_weights()
                 x8, sa = quantize_e4m3_blocks(x2)
-                w8, sb = self.w8_blocks, self.w_block_scales
                 if residual is None:
                     gemm_fp8_blockscaled(x8, sa, w8, sb, self.scale, self.shift, self.relu, out=y2)
                     return y
                 gemm_fp8_blockscaled(x8, sa, w8, sb, self.scale, self.shift, False, out=y2)
-                return ops.scale_shift_act(y, self._ones, self._zeros, residual, self.relu)
-            if getattr(self, "w8", None) is not None:
+                return ops.scale_shift_act(y, ones, zeros, residual, self.relu)
+            if self._fp8 == "tensor":
                 from ..ops.fp8 import gemm_fp8, quantize_e4m3
 
+                w8, deq_scale, ones, zeros = self._fp8_weights()
                 x8 = quantize_e4m3(x2, self.act_scale)
                 if residual is None:
-                    gemm_fp8(x8, self.w8, self.deq_scale, self.shift, self.relu, out=y2)
+                    gemm_fp8(x8, w8, deq_scale, self.shift, self.relu, out=y2)
                     return y
-                gemm_fp8(x8, self.w8, self.deq_scale, self.shift, False, out=y2)
-                return ops.scale_shift_act(y, self._ones, self._zeros, residual, self.relu)
+                gemm_fp8(x8, w8, deq_scale, self.shift, False, out=y2)
+                return ops.scale_shift_act(y, ones, zeros, residual, self.relu)
             if residual is None:
                 ops.gemm_bf16(x2, self.weight.view(self.cout, self.cin), out=y2, col_scale=self.scale,
                               col_shift=self.shift, relu=self.relu)
@@ -244,8 +285,7 @@ class ResNeXt(nn.Module):
         if calib_batch is None:
             raise ValueError("enable_fp8(scaling='tensor') needs a calibration batch")
         for c in convs:
-            c.w8_blocks = None                              # leaves the block-scaled mode
-        for c in convs:
+            c._fp8 = None                                   # calibrate on the bf16 forward
             c.begin_calibration()
         self.forward_features(calib_batch)
         return sum(1 for c in convs if c.finish_calibration(margin))

@@ -38,6 +38,8 @@ def quantize_e4m3(x: torch.Tensor, scale: torch.Tensor, amax: Optional[torch.Ten
     from . import native, count_launch
 
     x = x.contiguous()
+    if x.is_cuda and x.data_ptr() % 16 != 0:
+        x = x.clone()                       # the kernel reads 16-byte vectors: a fresh allocation is aligned
     q = out if out is not None else torch.empty(x.shape, dtype=torch.uint8, device=x.device)
     if x.is_cuda:
         native().quantize_e4m3(x, q, scale, amax)

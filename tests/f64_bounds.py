@@ -62,6 +62,15 @@ ResNet50, every BatchNorm mode, the trainer and its graph replays; NVIDIA H100 8
     saved statistics, staged / vs exact                         c1 0.50 / 0.10
     running statistics, staged / vs exact                       c1 0.17 / 0.08
     pools, global pool backward                                 c1 1.000   c2 1.00
+and layer by layer inside the ResNeXt teacher's inference forward (tests/test_teacher_oracle_gpu.py: ResNeXt101_32x16d,
+ResNeXt50_32x4d and ResNeXt_tiny with random folded BatchNorm, every convolution path, a graph replay; NVIDIA H100 80GB
+HBM3, 700 W power limit):
+
+    teacher bf16 layers (1x1, fused / two-kernel residual,     c1 1.000   c2 1.00
+      widened / stride-2 / subsampled grouped 3x3, stem, classifier)
+    FP8 block layers (fp8_tau, criterion 1 alone)              c1 0.773
+    FP8 per-tensor layers (fp8_tensor_tau, criterion 1 alone;  c1 0.817
+      the bound is derived from the block model, these are its first measurements)
 c1 sits at 1 because a correctly rounded element near a rounding midpoint has an error of half an ulp.
 
 Set ``EDL_F64_BOUNDS_LOG`` to a file name to append one JSON line per check with both ratios."""
@@ -675,6 +684,34 @@ def dilate2_ref(x):
     out = torch.zeros(n, c, 2 * h, 2 * w, dtype=x.dtype, device=x.device)
     out[:, :, ::2, ::2] = x
     return out
+
+
+# ------------------------------------------------------------------------------------------------------ fp8 GEMMs
+# The tensor core adds the e4m3 products of a 32-deep MMA with fewer significant bits than fp32 (about 14): 2^-12 of the
+# magnitude per MMA.  The block-scaled GEMM promotes each 128-deep k-block (four MMAs) into an fp32 accumulator; the
+# per-tensor GEMM keeps one accumulator in the MMA chain for all of K.
+def fp8_tau(k):
+    """Per-element slack factor (times the magnitude) of the block-scaled GEMM: the tensor core's k-block sums, one fp32
+    promotion per k-block, the bias, the addend and the bf16 conversion's input."""
+    return 2.0 ** -10 + (math.ceil(k / 128) + 3) * EPS32
+
+
+def fp8_tensor_tau(k):
+    """The same model for the per-tensor GEMM, with no per-k-block promotion: 2^-12 per 32-deep MMA over all of K, then
+    the epilogue's fma and the bf16 conversion's input.  Derived, not fitted."""
+    return math.ceil(k / 32) * 2.0 ** -12 + 3 * EPS32
+
+
+def dequant_a(q, sa):
+    """float64 [M, K] = e4m3(q) * sa[k // 128, m]"""
+    k = q.shape[1]
+    return q.view(torch.float8_e4m3fn).double() * sa.double().t().repeat_interleave(128, 1)[:, :k]
+
+
+def dequant_w(q, sw):
+    """float64 [N, K] = e4m3(q) * sw[n // 128, k // 128]"""
+    n, k = q.shape
+    return q.view(torch.float8_e4m3fn).double() * sw.double().repeat_interleave(128, 0)[:n].repeat_interleave(128, 1)[:, :k]
 
 
 # ----------------------------------------------------------------------------------------------- guarded windows

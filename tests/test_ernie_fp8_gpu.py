@@ -32,17 +32,11 @@ if not torch.cuda.is_available():
 from edl_b200 import ops  # noqa: E402
 from edl_b200.models import ernie, teacher_zoo  # noqa: E402
 from edl_b200.ops import fp8  # noqa: E402
-from f64_bounds import EPS32, Guarded, check_bf16, guarded, ulp  # noqa: E402
+from f64_bounds import Guarded, check_bf16, dequant_a, dequant_w, fp8_tau, guarded, ulp  # noqa: E402
 from test_ernie_gpu import _inputs  # noqa: E402
 
 DEV = torch.device("cuda", 0)
 E4M3_NAN = 0x7F
-
-
-def fp8_tau(k):
-    """Per-element slack factor (times the magnitude) of the block-scaled GEMM: the tensor core's k-block sums, one fp32
-    promotion per k-block, the bias, the addend and the bf16 conversion's input."""
-    return 2.0 ** -10 + (math.ceil(k / 128) + 3) * EPS32
 
 
 def _bits(t):
@@ -55,17 +49,6 @@ def _flat_guard(shape, fill, dtype, pad=64):
     buf = torch.full((n + 2 * pad,), fill, dtype=dtype, device=DEV)
     g = Guarded(buf, buf[pad:pad + n], fill)
     return g, g.t.view(*shape)
-
-
-def _dequant_a(q, sa):
-    """float64 [M, K] = e4m3(q) * sa[k // 128, m]"""
-    k = q.shape[1]
-    return q.view(torch.float8_e4m3fn).double() * sa.double().t().repeat_interleave(128, 1)[:, :k]
-
-
-def _dequant_w(q, sw):
-    n, k = q.shape
-    return q.view(torch.float8_e4m3fn).double() * sw.double().repeat_interleave(128, 0)[:n].repeat_interleave(128, 1)[:, :k]
 
 
 def _operands(m, n, k, seed, zero_row=None):
@@ -147,7 +130,7 @@ def test_residual_epilogue_vs_float64(m, n, k):
     torch.cuda.synchronize()
     assert ops.fallbacks() == {}, ops.fallbacks()
     out.assert_untouched("fp8 residual epilogue output")
-    a64, w64 = _dequant_a(qa, sa), _dequant_w(qw, sw)
+    a64, w64 = dequant_a(qa, sa), dequant_w(qw, sw)
     ref = a64 @ w64.t() + bias.double() + add.t.double()
     mag = a64.abs() @ w64.abs().t() + bias.double().abs() + add.t.double().abs()
     check_bf16(out.t, ref, mag, tau=fp8_tau(k), criteria=(1,), what="fp8 residual epilogue %d x %d x %d" % (m, n, k))
@@ -179,7 +162,7 @@ def test_gelu_e4m3_epilogue_vs_float64(m, n, k):
     sa_g.assert_untouched("fp8 GELU epilogue sa_out")
     assert float(sa_out[0, zero]) == 1.0 and not q.t[zero, :128].any()
 
-    a64, w64 = _dequant_a(qa, sa), _dequant_w(qw, sw)
+    a64, w64 = dequant_a(qa, sa), dequant_w(qw, sw)
     pre = a64 @ w64.t() + bias.double()
     bnd = fp8_tau(k) * (a64.abs() @ w64.abs().t() + bias.double().abs())
     g64 = 0.5 * pre * (1 + torch.erf(pre / math.sqrt(2)))
