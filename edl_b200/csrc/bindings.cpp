@@ -684,6 +684,7 @@ void wait_flag_async(const Tensor& flag, const c10::optional<Tensor>& seq, int64
 
 void register_gemm_bindings(pybind11::module_& m);  // gemm_bindings.cpp
 void register_transformer_bindings(pybind11::module_& m);  // transformer_bindings.cpp
+void register_lstm_bindings(pybind11::module_& m);  // lstm_bindings.cpp
 void register_jpeg_bindings(pybind11::module_& m);  // jpeg_decode.cpp
 void register_vmm_bindings(pybind11::module_& m);   // vmm.cpp
 
@@ -751,6 +752,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("wait_flag_async", &wait_flag_async);
   register_gemm_bindings(m);
   register_transformer_bindings(m);
+  register_lstm_bindings(m);
   register_jpeg_bindings(m);
   register_vmm_bindings(m);
 }

@@ -240,4 +240,16 @@ void embedding_layernorm_e4m3_fwd(const int64_t* ids, const int64_t* pos_ids, co
                                   const float* gamma, const float* beta, void* y, void* q, float* sa, int64_t rows, int C,
                                   float eps, int* err, cudaStream_t s);
 
+// ---- lstm.cu: bidirectional LSTM recurrence of the BiLSTM student (H = 128; layouts in lstm.cu's header) ----
+constexpr int kLstmHidden = 128;
+bool lstm_supported(int B, int L, int E, int H);
+// xproj bf16 [L * B, 8H] (thread order), whh bf16 [2, 4H, H] (nn.LSTM layout, 16-byte aligned), lengths int32 [B];
+// writes hs bf16 [(L + 2) * B, 2H], hn bf16 [2, B, H], gates bf16 [L * B, 2, H, 4], cs fp32 [L * B, 2, H]
+const char* lstm_fwd(const void* xproj, const void* whh, const int* lengths, void* hs, void* hn, void* gates, float* cs,
+                     int B, int L, cudaStream_t stream);
+// dy bf16 (b, t, c) at b * dy_sb + t * dy_st + c, or nullptr (zero); dhn bf16 [2, B, H] or nullptr;
+// writes dgates bf16 [L * B, 8H] (nn.LSTM row order per direction)
+const char* lstm_bwd(const void* whh, const int* lengths, const void* gates, const float* cs, const void* dy,
+                     int64_t dy_sb, int64_t dy_st, const void* dhn, void* dgates, int B, int L, cudaStream_t stream);
+
 }  // namespace edl

@@ -1,5 +1,5 @@
 """Small workloads of the reference's examples: fit_a_line regression, the MNIST distill student and
-teacher CNNs, the BOW / CNN NLP distill students.
+teacher CNNs, the BOW / CNN NLP distill students and the bidirectional LSTM student.
 
 References: example/fit_a_line/fluid/fit_a_line.py:33-44 (``fc(13 -> 1)``);
 example/distill/mnist_distill/train_with_fleet.py:134-145 (LeNet-ish student, served CNN teacher);
@@ -75,6 +75,41 @@ class TextCNN(nn.Module):
     def forward(self, ids):
         h = torch.tanh(self.conv(self.emb(ids).transpose(1, 2))).max(-1).values
         return self.fc(h)
+
+
+class BiLSTM(nn.Module):
+    """Bidirectional LSTM sentiment student: embedding -> ``ops.lstm`` -> [h_n forward | h_n reverse] -> tanh(fc1) -> fc2
+    (the head of ``BOW``).  The LSTM parameters live in an ``nn.LSTM`` submodule used as their container, so state
+    dicts of a torch-trained BiLSTM load unchanged; the recurrence itself runs on ``ops.lstm`` (csrc/lstm.cu on CUDA).
+    A sample's length is its last non-pad position + 1, computed on the device; a pad inside a sentence is read as the
+    zero embedding row, as ``BOW``'s masking does."""
+
+    def __init__(self, vocab_size=30000, emb_dim=128, hidden=128, num_labels=2, padding_idx=0):
+        super().__init__()
+        self.emb = nn.Embedding(vocab_size, emb_dim, padding_idx=padding_idx)
+        self.lstm = nn.LSTM(emb_dim, hidden, batch_first=True, bidirectional=True)
+        self.fc1 = nn.Linear(2 * hidden, hidden)
+        self.fc2 = nn.Linear(hidden, num_labels)
+        self.padding_idx = padding_idx
+
+    def lstm_params(self):
+        return [getattr(self.lstm, n) for n in ("weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0",
+                                                "weight_ih_l0_reverse", "weight_hh_l0_reverse",
+                                                "bias_ih_l0_reverse", "bias_hh_l0_reverse")]
+
+    def lengths(self, ids):
+        pos = torch.arange(1, ids.shape[1] + 1, device=ids.device)
+        return ((ids != self.padding_idx) * pos).amax(1)
+
+    def forward(self, ids):
+        from .. import ops
+
+        x = self.emb(ids)
+        if x.is_cuda:
+            x = x.to(torch.bfloat16)
+        _, h_n = ops.lstm(x, self.lengths(ids), self.lstm_params())
+        h = torch.cat([h_n[0], h_n[1]], -1).to(self.fc1.weight.dtype)
+        return self.fc2(torch.tanh(self.fc1(h)))
 
 
 def kl_distill_loss(student_logits, teacher_logits, temperature=1.0):

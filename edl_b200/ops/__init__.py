@@ -99,6 +99,7 @@ from .transformer import (attention, attention_supported, layer_norm, layer_norm
                           embedding_layernorm, embedding_layernorm_supported, attention_varlen,
                           attention_varlen_supported, layer_norm_e4m3, layer_norm_e4m3_supported,
                           embedding_layernorm_e4m3, embedding_layernorm_e4m3_supported)
+from .rnn import lstm, lstm_supported  # noqa: E402
 
 __all__ = [
     "native", "native_available", "launches", "reset_launches", "count_fallback", "fallbacks", "reset_fallbacks",
@@ -115,4 +116,5 @@ __all__ = [
     "drop_bn_hook", "attention", "attention_supported", "layer_norm", "layer_norm_supported", "embedding_layernorm",
     "embedding_layernorm_supported", "attention_varlen", "attention_varlen_supported", "layer_norm_e4m3",
     "layer_norm_e4m3_supported", "embedding_layernorm_e4m3", "embedding_layernorm_e4m3_supported",
+    "lstm", "lstm_supported",
 ]

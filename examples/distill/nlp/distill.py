@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Sentence-classification distillation: BOW / TextCNN student, served sequence teacher, ``KL_T`` loss
+"""Sentence-classification distillation: BOW / TextCNN / BiLSTM student, served sequence teacher, ``KL_T`` loss
 with T=2 and a batch generator carrying token ids (reference: example/distill/nlp/distill.py:98-196,
 model.py:54-135; the reference's teacher is an ERNIE served by Paddle Serving -- any served model
 that returns ``logits`` works here; a TextCNN stands in when none is given)."""
@@ -13,7 +13,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))))
 from paddle_edl.distill.distill_reader import DistillReader  # noqa: E402
 from paddle_edl.distill.teacher_server import TeacherServer  # noqa: E402
-from paddle_edl.models.small import BOW, TextCNN, kl_distill_loss  # noqa: E402
+from paddle_edl.models.small import BOW, BiLSTM, TextCNN, kl_distill_loss  # noqa: E402
 
 
 def corpus(n, vocab, seq, seed):
@@ -27,7 +27,7 @@ def corpus(n, vocab, seq, seed):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="bow", choices=["bow", "cnn"])
+    ap.add_argument("--model", default="bow", choices=["bow", "cnn", "lstm"])
     ap.add_argument("--teachers", default="")
     ap.add_argument("--T", type=float, default=2.0)
     ap.add_argument("--epochs", type=int, default=2)
@@ -38,7 +38,12 @@ def main():
         teacher = TextCNN(args.vocab).eval()
         srv = TeacherServer(teacher, ["ids"], ["logits"], {"ids": [64]}).start()
         args.teachers = srv.endpoint
-    student = BOW(args.vocab) if args.model == "bow" else TextCNN(args.vocab)
+    dev = torch.device("cpu")
+    if args.model == "lstm":            # the LSTM student runs on the GPU when there is one (csrc/lstm.cu)
+        dev = torch.device("cuda" if torch.cuda.is_available() else "cpu")
+        student = BiLSTM(args.vocab).to(dev)
+    else:
+        student = BOW(args.vocab) if args.model == "bow" else TextCNN(args.vocab)
     opt = torch.optim.AdamW(student.parameters(), 1e-3)
 
     def batch_gen():
@@ -55,9 +60,9 @@ def main():
     reader = dr.set_batch_generator(batch_gen)
     for epoch in range(args.epochs):
         for i, (ids, label, t_logits) in enumerate(reader()):
-            logits = student(torch.from_numpy(ids))
-            loss = kl_distill_loss(logits, torch.from_numpy(t_logits), args.T) + \
-                torch.nn.functional.cross_entropy(logits, torch.from_numpy(label[:, 0]))
+            logits = student(torch.from_numpy(ids).to(dev))
+            loss = kl_distill_loss(logits, torch.from_numpy(t_logits).to(dev), args.T) + \
+                torch.nn.functional.cross_entropy(logits, torch.from_numpy(label[:, 0]).to(dev))
             opt.zero_grad()
             loss.backward()
             opt.step()

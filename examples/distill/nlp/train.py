@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Train the small student (BOW / TextCNN) alone on hard labels -- the baseline the distilled student is
+"""Train the small student (BOW / TextCNN / BiLSTM) alone on hard labels -- the baseline the distilled student is
 compared with (reference: example/distill/nlp/train.py)."""
 import argparse
 import os
@@ -11,15 +11,23 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.abspath(os.path.join(HERE, "..", "..", "..")))
 from reader import TsvReader, batches, synthetic_corpus  # noqa: E402
-from paddle_edl.models.small import BOW, TextCNN  # noqa: E402
+from paddle_edl.models.small import BOW, BiLSTM, TextCNN  # noqa: E402
 
 
-def evaluate(model, data):
+def build_model(name, vocab):
+    """(model, device): the LSTM student runs on the GPU when there is one (csrc/lstm.cu), the others on the CPU."""
+    if name == "lstm":
+        dev = torch.device("cuda" if torch.cuda.is_available() else "cpu")
+        return BiLSTM(vocab).to(dev), dev
+    return (BOW(vocab) if name == "bow" else TextCNN(vocab)), torch.device("cpu")
+
+
+def evaluate(model, data, dev=torch.device("cpu")):
     model.eval()
     hit = n = 0
     with torch.no_grad():
         for ids, label in data:
-            pred = model(torch.from_numpy(ids)).argmax(-1)
+            pred = model(torch.from_numpy(ids).to(dev)).argmax(-1).cpu()
             hit += int((pred == torch.from_numpy(label[:, 0])).sum())
             n += len(label)
     model.train()
@@ -28,7 +36,7 @@ def evaluate(model, data):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="bow", choices=["bow", "cnn"])
+    ap.add_argument("--model", default="bow", choices=["bow", "cnn", "lstm"])
     ap.add_argument("--train_tsv", default=None)
     ap.add_argument("--dev_tsv", default=None)
     ap.add_argument("--epochs", type=int, default=3)
@@ -46,15 +54,16 @@ def main():
         vocab = args.vocab
         train_iter = lambda ep: batches(synthetic_corpus(args.samples, vocab, args.seq_len, ep), 16)   # noqa: E731
         dev_data = list(batches(synthetic_corpus(256, vocab, args.seq_len, 10_000), 16))
-    model = BOW(vocab) if args.model == "bow" else TextCNN(vocab)
+    model, dev = build_model(args.model, vocab)
     opt = torch.optim.AdamW(model.parameters(), 1e-3)
     for ep in range(args.epochs):
         for ids, label in train_iter(ep):
-            loss = torch.nn.functional.cross_entropy(model(torch.from_numpy(ids)), torch.from_numpy(label[:, 0]))
+            loss = torch.nn.functional.cross_entropy(model(torch.from_numpy(ids).to(dev)),
+                                                     torch.from_numpy(label[:, 0]).to(dev))
             opt.zero_grad()
             loss.backward()
             opt.step()
-        print("epoch %d loss %.4f dev acc %.4f" % (ep, float(loss), evaluate(model, dev_data)), flush=True)
+        print("epoch %d loss %.4f dev acc %.4f" % (ep, float(loss), evaluate(model, dev_data, dev)), flush=True)
 
 
 if __name__ == "__main__":
