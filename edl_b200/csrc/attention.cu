@@ -23,6 +23,11 @@
 // pair of maps (tensormap.replace of the global address and the row count of a template map, published with
 // tensormap.cp_fenceproxy); the attention kernel acquires them and runs the same body with L = len_b.  A sequence's
 // output thus depends on its own rows only, whatever the others hold (NaN included), and nothing is stored outside it.
+//
+// Training (padded layout only): with lse != nullptr the kernel also stores, per (b, h, query), lse = m + log2(l) in the
+// log2 units of the scaled scores (m the row max of S / 8 * log2(e), l the row sum over the bf16-rounded probabilities), or
+// +inf for a row without a valid key; attention_bwd.cu recomputes P = exp2(S / 8 * log2(e) - lse) from it.  The store
+// sits after O is formed, so O does not depend on whether lse is given.
 #include <cuda.h>
 
 #include <type_traits>
@@ -71,7 +76,7 @@ struct Varlen {
 template <typename Seq>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO,
-                     const uint8_t* __restrict__ mask, Seq seq, int H) {
+                     const uint8_t* __restrict__ mask, Seq seq, int H, float* __restrict__ lse) {
   constexpr bool kVarlen = std::is_same<Seq, Varlen>::value;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -224,6 +229,13 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
       l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
       inv[r] = l[r] > 0.f ? 1.f / l[r] : 0.f;
     }
+    if (!kVarlen && lse != nullptr && (lane & 3) == 0) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int qi = q0 + cw * 64 + row + 8 * r;
+        if (qi < L) lse[((int64_t)b * H + h) * L + qi] = l[r] > 0.f ? m[r] + log2f(l[r]) : INFINITY;
+      }
+    }
     uint8_t* st = sq + cw * kHalfBytes;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -277,14 +289,14 @@ attention_varlen_maps_kernel(const __grid_constant__ CUtensorMap tmQKV, const __
 
 template <typename Seq>
 const char* launch_attention(const CUtensorMap& tmQKV, const CUtensorMap& tmO, const uint8_t* mask, Seq seq, int H,
-                             dim3 grid, cudaStream_t stream) {
+                             dim3 grid, cudaStream_t stream, float* lse = nullptr) {
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(attention_fwd_kernel<Seq>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
     if (e != cudaSuccess) return cudaGetErrorString(e);
     attr_set = true;
   }
-  attention_fwd_kernel<Seq><<<grid, kAttnThreads, kAttnSmem, stream>>>(tmQKV, tmO, mask, seq, H);
+  attention_fwd_kernel<Seq><<<grid, kAttnThreads, kAttnSmem, stream>>>(tmQKV, tmO, mask, seq, H, lse);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
@@ -309,11 +321,12 @@ bool attention_supported(int B, int L, int H, int head_dim) {
   return B >= 1 && B <= 65535 && L >= 1 && L <= kAttnMaxLen && H >= 1 && H <= 65535 && head_dim == 64;
 }
 
-const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream) {
+const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream,
+                          float* lse) {
   if (!attention_supported(B, L, H, 64)) return "attention_fwd: unsupported shape (head dim 64, 1 <= L <= 512)";
   alignas(64) CUtensorMap tmQKV, tmO;
   if (const char* e = encode_attention_maps(&tmQKV, &tmO, qkv, out, L, B, H)) return e;
-  return launch_attention<int>(tmQKV, tmO, mask, L, H, dim3((L + 127) / 128, H, B), stream);
+  return launch_attention<int>(tmQKV, tmO, mask, L, H, dim3((L + 127) / 128, H, B), stream, lse);
 }
 
 bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim) {

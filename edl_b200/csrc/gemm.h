@@ -54,6 +54,12 @@ struct GemmArgs {
   // D = gelu(A*B^T * col_scale + col_shift), erf form, fp32 (inference; B K-major, no addend / ReLU / statistics).
   // Persistent kernel only.
   bool gelu = false;
+  // with gelu: also store the pre-activation u = A*B^T * col_scale + col_shift as bf16 [M, N] (row pitch ld_u), the
+  // training forward of FFN1
+  void* gelu_u = nullptr;
+  int64_t ld_u = 0;
+  // D = (A*B) * gelu'(add_src) in fp32 (B MN-major, add_src = u): the dgrad of FFN2 that yields dU of FFN1
+  bool gelu_grad = false;
   // fused "GEMM -> peer ship" (EPI 0 only): D may be a PEER GPU's buffer (NVLink-mapped address);
   // every CTA TMA-stores its tile there, and the CTA that completes last publishes
   // *ship_flag (peer address) = seq with release/system semantics -- no separate copy kernel.

@@ -117,6 +117,44 @@ void gemm_bf16_gelu(const Tensor& A, const Tensor& B, const Tensor& D, const c10
   TORCH_CHECK(err == nullptr, "edl gemm_bf16_gelu failed: ", err);
 }
 
+void check_like_d(const Tensor& U, const edl::GemmArgs& g, const char* name) {
+  TORCH_CHECK(U.is_cuda() && U.scalar_type() == at::kBFloat16 && U.dim() == 2 && U.size(0) == g.M && U.size(1) == g.N &&
+              U.stride(1) == 1 && U.stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(U.data_ptr()) % 16 == 0, name,
+              " must be bf16 [M, N] with 16-byte aligned rows");
+}
+
+// Training forward of FFN1: D = gelu(u) and U = u = A * B^T + col_shift (bf16), one persistent GEMM.
+void gemm_bf16_gelu_train(const Tensor& A, const Tensor& B, const Tensor& D, const Tensor& U,
+                          const c10::optional<Tensor>& col_shift) {
+  edl::GemmArgs g = gemm_operands(A, B, false, false);
+  check_like_d(D, g, "D");
+  check_like_d(U, g, "U");
+  g.D = D.data_ptr();
+  g.ldd = D.stride(0);
+  g.col_shift = optp<float>(col_shift);
+  g.gelu = true;
+  g.gelu_u = U.data_ptr();
+  g.ld_u = U.stride(0);
+  c10::cuda::CUDAGuard guard(A.device());
+  const char* err = edl::gemm_bf16(g, at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl gemm_bf16_gelu_train failed: ", err);
+}
+
+// FFN2's dgrad through the GELU: D = (A * B) * gelu'(U), A = dY [M, K], B = W2 [K, N] (MN-major), U = u [M, N].
+void gemm_bf16_gelu_grad(const Tensor& A, const Tensor& B, const Tensor& D, const Tensor& U) {
+  edl::GemmArgs g = gemm_operands(A, B, false, true);
+  check_like_d(D, g, "D");
+  check_like_d(U, g, "U");
+  g.D = D.data_ptr();
+  g.ldd = D.stride(0);
+  g.add_src = U.data_ptr();
+  g.ld_add = U.stride(0);
+  g.gelu_grad = true;
+  c10::cuda::CUDAGuard guard(A.device());
+  const char* err = edl::gemm_bf16(g, at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl gemm_bf16_gelu_grad failed: ", err);
+}
+
 // fp32 scratch for the partial tiles of a split reduction (optional: the kernels report it missing or too small)
 void set_partials(const c10::optional<Tensor>& partials, float** ptr, int64_t* elems) {
   if (!partials.has_value() || !partials->defined()) return;
@@ -583,6 +621,8 @@ void conv3x3_infer(const Tensor& x, const Tensor& w, Tensor& y, const c10::optio
 void register_gemm_bindings(pybind11::module_& m) {
   m.def("gemm_bf16", &gemm_bf16);
   m.def("gemm_bf16_gelu", &gemm_bf16_gelu);
+  m.def("gemm_bf16_gelu_train", &gemm_bf16_gelu_train);
+  m.def("gemm_bf16_gelu_grad", &gemm_bf16_gelu_grad);
   m.def("gemm_wgrad_bf16", &gemm_wgrad_bf16);
   m.def("conv3x3", &conv3x3);
   m.def("set_persistent_gemm", &edl::set_persistent_gemm);

@@ -67,6 +67,9 @@ struct PersistParams {
   signed char tap_dh[9], tap_dw[9], tap_w[9];
   // debug: per-phase clock64() stamps of CTA 0 (tools/trace_persist.py), [3 rows][kTraceTiles][8 phases]: row 0 producer, row 2 consumers
   long long* trace;
+  // GELU == 2: the pre-activation u = acc * scale + shift, bf16 [M, N] with row pitch ld_aux
+  __nv_bfloat16* aux;
+  long long ld_aux;
 };
 constexpr int kTraceTiles = 16;
 #define EDL_TRACE(role, tile, phase)                                                                    \
@@ -138,9 +141,17 @@ EDL_DEVICE void issue_bn_tiles(const PersistParams& p, int tm, int nn0, int rows
   __syncwarp();
 }
 
-// GELU: inference epilogue y = gelu(acc * scale + shift) with the erf form 0.5 v (1 + erf(v / sqrt 2)) in fp32 (the
-// FFN1 GEMM of a Transformer encoder, bias in col_shift).  A compile-time switch: the other instantiations are unchanged.
-template <int BLOCK_N, int STAGES, int MODE, int BNR, int ASTAGES, int EPIW, bool GELU = false>
+// GELU: compile-time epilogue variants (0 = none; the other instantiations are unchanged by them).
+//   1  inference: y = gelu(acc * scale + shift) with the erf form 0.5 v (1 + erf(v / sqrt 2)) in fp32 (the FFN1 GEMM of
+//      a Transformer encoder, bias in col_shift)
+//   2  training forward: the same y, and also u = acc * scale + shift as bf16 into p.aux (what the backward reads)
+//   3  training dgrad (MODE 1): D = acc * gelu'(u) with gelu'(u) = Phi(u) + u phi(u) in fp32, u the bf16 addend tile
+//      (FFN2's dgrad writes dU directly)
+EDL_DEVICE float gelu_grad(float u) {
+  return 0.5f * (1.f + erff(u * 0.70710678118654752f)) + u * 0.39894228040143268f * __expf(-0.5f * u * u);
+}
+
+template <int BLOCK_N, int STAGES, int MODE, int BNR, int ASTAGES, int EPIW, int GELU = 0>
 __global__ void __launch_bounds__(128 + EPIW * 32, 1)
 gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmAdd,
@@ -544,8 +555,13 @@ gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             const int r = row + 8 * h;
             const uint32_t w = ptx::lds32(hp + r * 128 + ((chunk ^ (r & 7)) << 4));
             const float2 t2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
-            v[2 * h] += t2.x;
-            v[2 * h + 1] += t2.y;
+            if constexpr (GELU == 3) {
+              v[2 * h] *= gelu_grad(t2.x);
+              v[2 * h + 1] *= gelu_grad(t2.y);
+            } else {
+              v[2 * h] += t2.x;
+              v[2 * h + 1] += t2.y;
+            }
           }
         }
         if (bn_mask) {
@@ -573,7 +589,16 @@ gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 #pragma unroll
             for (int e = 0; e < 4; ++e) v[e] = fmaxf(v[e], 0.f);
           }
-          if constexpr (GELU) {
+          if constexpr (GELU == 2) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int r = m0 + row + 8 * h;
+              if (r < p.M && col < p.N)
+                *reinterpret_cast<__nv_bfloat162*>(p.aux + (int64_t)r * p.ld_aux + col) =
+                    __floats2bfloat162_rn(v[2 * h], v[2 * h + 1]);
+            }
+          }
+          if constexpr (GELU == 1 || GELU == 2) {
 #pragma unroll
             for (int e = 0; e < 4; ++e) v[e] = 0.5f * v[e] * (1.f + erff(v[e] * 0.70710678118654752f));
           }
@@ -874,7 +899,7 @@ bool g_epi16 = [] {
   return e != nullptr && e[0] == '1' && e[1] == '6';
 }();
 
-template <int BLOCK_N, int STAGES, int MODE, int BNR, int ASTAGES, int EPIW, bool GELU>
+template <int BLOCK_N, int STAGES, int MODE, int BNR, int ASTAGES, int EPIW, int GELU>
 const char* launch_pe(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const PersistParams& p,
                      cudaStream_t stream, const CUtensorMap* tmAdd = nullptr, const CUtensorMap* tmBnX = nullptr,
                      const CUtensorMap* tmBnY = nullptr) {
@@ -899,7 +924,7 @@ const char* launch_pe(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUte
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
-template <int BLOCK_N, int STAGES, int MODE, int BNR = 0, int ASTAGES = 0, bool GELU = false>
+template <int BLOCK_N, int STAGES, int MODE, int BNR = 0, int ASTAGES = 0, int GELU = 0>
 const char* launch_p(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const PersistParams& p,
                      cudaStream_t stream, const CUtensorMap* tmAdd = nullptr, const CUtensorMap* tmBnX = nullptr,
                      const CUtensorMap* tmBnY = nullptr) {
@@ -944,7 +969,7 @@ const char* gemm_bf16_persistent(const GemmArgs& g, cudaStream_t stream) {
   // L2 -> SM path delivers when every SM pulls; with N = 256 the
   // A tile is reused twice as often and the requirement drops to 96 B / clk.
   // (not with the GELU epilogue: with the erf expansion the 256-column tile spills its accumulators)
-  const bool wide = g_wide_tiles && !g.gelu && !g.b_mn_major && g.bn.x == nullptr && g.col_stats == nullptr && g.N % 256 == 0 &&
+  const bool wide = g_wide_tiles && !g.gelu && !g.gelu_grad && !g.b_mn_major && g.bn.x == nullptr && g.col_stats == nullptr && g.N % 256 == 0 &&
                     g.K >= 256 &&
                     (int64_t)((g.M + kBlockM - 1) / kBlockM) * (g.N / 256) >= kNumSMs;
   const int bn = n64 ? 64 : (wide ? 256 : 128);
@@ -995,10 +1020,24 @@ const char* gemm_bf16_persistent(const GemmArgs& g, cudaStream_t stream) {
     return n64 ? launch_p<64, 4, 1, 2>(tmA, tmB, tmD, p, stream, padd, &tmBx, pby)
                : launch_p<128, 3, 1, 2>(tmA, tmB, tmD, p, stream, padd, &tmBx, pby);
   }
+  if (g.gelu_grad) {
+    if (!g.b_mn_major || g.add_src == nullptr || g.gelu || g.col_stats != nullptr || g.relu || g.col_scale != nullptr ||
+        g.col_shift != nullptr)
+      return "gemm GELU-gradient epilogue: dgrad GEMM (B MN-major) with u as the addend only";
+    return n64 ? launch_p<64, 6, 1, 0, 0, 3>(tmA, tmB, tmD, p, stream, padd)
+               : launch_p<128, 5, 1, 0, 0, 3>(tmA, tmB, tmD, p, stream, padd);
+  }
   if (g.gelu) {
     if (g.b_mn_major || g.add_src != nullptr || g.col_stats != nullptr || g.relu)
       return "gemm GELU epilogue: forward GEMM (B K-major) with an optional scale / shift only";
-    return n64 ? launch_p<64, 6, 0, 0, 0, true>(tmA, tmB, tmD, p, stream) : launch_p<128, 5, 0, 0, 0, true>(tmA, tmB, tmD, p, stream);
+    if (g.gelu_u != nullptr) {
+      if (g.N % 8 != 0 || g.ld_u % 8 != 0 || (reinterpret_cast<uintptr_t>(g.gelu_u) & 15) != 0)
+        return "gemm GELU epilogue: u needs N % 8 == 0 and 16-byte aligned rows";
+      p.aux = reinterpret_cast<__nv_bfloat16*>(g.gelu_u);
+      p.ld_aux = g.ld_u;
+      return n64 ? launch_p<64, 6, 0, 0, 0, 2>(tmA, tmB, tmD, p, stream) : launch_p<128, 5, 0, 0, 0, 2>(tmA, tmB, tmD, p, stream);
+    }
+    return n64 ? launch_p<64, 6, 0, 0, 0, 1>(tmA, tmB, tmD, p, stream) : launch_p<128, 5, 0, 0, 0, 1>(tmA, tmB, tmD, p, stream);
   }
   if (!g.b_mn_major) {
     if (wide) return launch_p<256, 3, 0>(tmA, tmB, tmD, p, stream, padd);

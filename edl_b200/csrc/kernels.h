@@ -210,8 +210,15 @@ void wait_flag_async(const void* flag, const void* seq_ptr, uint32_t seq_imm, do
 constexpr int kAttnMaxLen = 512;
 bool attention_supported(int B, int L, int H, int head_dim);
 // qkv bf16 [B * L, 3 * H * 64] (Q | K | V column blocks, 16-byte aligned), mask uint8 [B, L] (1 = attend; nullptr: all),
-// out bf16 [B * L, H * 64].  Returns nullptr or an error string.
-const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream);
+// out bf16 [B * L, H * 64].  lse: nullptr, or fp32 [B, H, L] that receives what the backward needs to recompute the
+// probabilities (attention.cu).  Returns nullptr or an error string.
+const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream,
+                          float* lse = nullptr);
+// Backward of attention_fwd (attention_bwd.cu): from qkv, the forward's out and lse and the output gradient dout
+// (bf16 [B * L, H * 64]) writes dqkv bf16 [B * L, 3 * H * 64] (dQ | dK | dV in the layout of qkv).  delta: fp32 [B, H, L]
+// workspace.  Deterministic, no atomics.
+const char* attention_bwd(const void* qkv, const uint8_t* mask, const void* out, const float* lse, const void* dout,
+                          void* dqkv, float* delta, int B, int L, int H, cudaStream_t stream);
 bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim);
 // Packed sequences: qkv bf16 [T, 3 * H * 64], sequence b in rows [cu_seqlens[b], cu_seqlens[b + 1]) (int32 device
 // offsets, 1 <= length <= max_len <= 512), key_mask uint8 [T] (1 = attend; nullptr: all), out bf16 [T, H * 64];
@@ -239,6 +246,17 @@ void embedding_layernorm_e4m3_fwd(const int64_t* ids, const int64_t* pos_ids, co
                                   int64_t n_word, const void* pos, int64_t n_pos, const void* seg, int64_t n_seg,
                                   const float* gamma, const float* beta, void* y, void* q, float* sa, int64_t rows, int C,
                                   float eps, int* err, cudaStream_t s);
+// Backward of layernorm_fwd from the saved pre-LN input x (statistics recomputed): dx bf16 [rows, C]; per-CTA fp32
+// partials of dgamma / dbeta in part [layernorm_bwd_ctas(rows), 2, C], reduced in a fixed order into dgamma, dbeta [C].
+int layernorm_bwd_ctas(int64_t rows);
+void layernorm_bwd(const void* x, const void* dy, const float* gamma, void* dx, float* part, float* dgamma,
+                   float* dbeta, int64_t rows, int C, float eps, cudaStream_t s);
+// Backward of embedding_layernorm_fwd: re-gathers the row sum and writes its gradient dE fp32 [rows, C] (the gradient of
+// each of the three gathered table rows), plus dgamma / dbeta as in layernorm_bwd.
+void embedding_layernorm_bwd(const int64_t* ids, const int64_t* pos_ids, const int64_t* seg_ids, const void* word,
+                             int64_t n_word, const void* pos, int64_t n_pos, const void* seg, int64_t n_seg,
+                             const void* dy, const float* gamma, float* dE, float* part, float* dgamma, float* dbeta,
+                             int64_t rows, int C, float eps, cudaStream_t s);
 
 // ---- lstm.cu: bidirectional LSTM recurrence of the BiLSTM student (H = 128; layouts in lstm.cu's header) ----
 constexpr int kLstmHidden = 128;

@@ -1,4 +1,5 @@
-// torch bindings for the Transformer encoder kernels (attention.cu, layernorm.cu and its quantising variants).
+// torch bindings for the Transformer encoder kernels (attention.cu, attention_bwd.cu, layernorm.cu and its quantising
+// variants).
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -14,7 +15,8 @@ void check_bf16_2d(const Tensor& t, const char* name) {
 }
 
 // qkv [B * L, 3 * H * 64], mask uint8 [B, L] or None, out [B * L, H * 64]
-void attention_fwd(const Tensor& qkv, const c10::optional<Tensor>& mask, Tensor& out, int64_t B, int64_t L, int64_t H) {
+void attention_fwd(const Tensor& qkv, const c10::optional<Tensor>& mask, Tensor& out, int64_t B, int64_t L, int64_t H,
+                   const c10::optional<Tensor>& lse) {
   check_bf16_2d(qkv, "qkv");
   check_bf16_2d(out, "out");
   TORCH_CHECK(qkv.size(0) == B * L && qkv.size(1) == 3 * H * 64, "qkv must be [B * L, 3 * H * 64]");
@@ -26,10 +28,41 @@ void attention_fwd(const Tensor& qkv, const c10::optional<Tensor>& mask, Tensor&
                 "mask must be a contiguous uint8 [B, L] CUDA tensor");
     mp = mask->data_ptr<uint8_t>();
   }
+  float* lp = nullptr;
+  if (lse.has_value() && lse->defined()) {
+    TORCH_CHECK(lse->is_cuda() && lse->scalar_type() == at::kFloat && lse->is_contiguous() && lse->numel() == B * H * L,
+                "lse must be a contiguous fp32 [B, H, L] CUDA tensor");
+    lp = lse->data_ptr<float>();
+  }
   c10::cuda::CUDAGuard guard(qkv.device());
   const char* err = edl::attention_fwd(qkv.data_ptr(), mp, out.data_ptr(), (int)B, (int)L, (int)H,
-                                       at::cuda::getCurrentCUDAStream().stream());
+                                       at::cuda::getCurrentCUDAStream().stream(), lp);
   TORCH_CHECK(err == nullptr, "edl attention_fwd failed: ", err);
+}
+
+// dqkv [B * L, 3 * H * 64] from qkv, the forward's out and lse [B, H, L], dout [B * L, H * 64]; delta fp32 [B, H, L]
+void attention_bwd(const Tensor& qkv, const c10::optional<Tensor>& mask, const Tensor& out, const Tensor& lse,
+                   const Tensor& dout, Tensor& dqkv, Tensor& delta, int64_t B, int64_t L, int64_t H) {
+  for (const Tensor* t : {&qkv, &out, &dout, static_cast<const Tensor*>(&dqkv)}) check_bf16_2d(*t, "attention_bwd operand");
+  TORCH_CHECK(qkv.size(0) == B * L && qkv.size(1) == 3 * H * 64 && dqkv.sizes() == qkv.sizes(),
+              "qkv / dqkv must be [B * L, 3 * H * 64]");
+  TORCH_CHECK(out.size(0) == B * L && out.size(1) == H * 64 && dout.sizes() == out.sizes(), "out / dout: [B * L, H * 64]");
+  for (const Tensor* t : {&lse, static_cast<const Tensor*>(&delta)})
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() == B * H * L,
+                "lse / delta must be contiguous fp32 [B, H, L] CUDA tensors");
+  for (const Tensor* t : {&qkv, &out, &dout, static_cast<const Tensor*>(&dqkv)})
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0 && t->device() == qkv.device());
+  const uint8_t* mp = nullptr;
+  if (mask.has_value() && mask->defined()) {
+    TORCH_CHECK(mask->is_cuda() && mask->scalar_type() == at::kByte && mask->is_contiguous() && mask->numel() == B * L,
+                "mask must be a contiguous uint8 [B, L] CUDA tensor");
+    mp = mask->data_ptr<uint8_t>();
+  }
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const char* err = edl::attention_bwd(qkv.data_ptr(), mp, out.data_ptr(), lse.data_ptr<float>(), dout.data_ptr(),
+                                       dqkv.data_ptr(), delta.data_ptr<float>(), (int)B, (int)L, (int)H,
+                                       at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl attention_bwd failed: ", err);
 }
 
 // qkv [T, 3 * H * 64], cu_seqlens int32 [B + 1], key_mask uint8 [T] or None, out [T, H * 64], maps uint8 [B * 256]
@@ -98,6 +131,49 @@ void embedding_layernorm_fwd(const Tensor& ids, const Tensor& pos_ids, const Ten
                                err.data_ptr<int>(), at::cuda::getCurrentCUDAStream().stream());
 }
 
+// x, dy, dx bf16 [rows, C]; part fp32 [layernorm_bwd_ctas(rows) * 2 * C]; dgamma / dbeta fp32 [C]
+void layernorm_bwd(const Tensor& x, const Tensor& dy, const Tensor& gamma, Tensor& dx, Tensor& part, Tensor& dgamma,
+                   Tensor& dbeta, double eps) {
+  for (const Tensor* t : {&x, &dy, static_cast<const Tensor*>(&dx)}) check_bf16_2d(*t, "layernorm_bwd operand");
+  const int64_t rows = x.size(0), C = x.size(1);
+  TORCH_CHECK(edl::layernorm_supported((int)C) && dy.sizes() == x.sizes() && dx.sizes() == x.sizes(),
+              "layernorm_bwd: C % 8 == 0, 8 <= C <= 1024, x / dy / dx of one shape");
+  check_affine(dgamma, dbeta, C);
+  TORCH_CHECK(gamma.is_cuda() && gamma.scalar_type() == at::kFloat && gamma.is_contiguous() && gamma.numel() == C);
+  TORCH_CHECK(part.is_cuda() && part.scalar_type() == at::kFloat && part.is_contiguous() &&
+              part.numel() >= (int64_t)edl::layernorm_bwd_ctas(rows) * 2 * C, "part: fp32 [ctas * 2 * C]");
+  c10::cuda::CUDAGuard guard(x.device());
+  edl::layernorm_bwd(x.data_ptr(), dy.data_ptr(), gamma.data_ptr<float>(), dx.data_ptr(), part.data_ptr<float>(),
+                     dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), rows, (int)C, (float)eps,
+                     at::cuda::getCurrentCUDAStream().stream());
+}
+
+// dE fp32 [rows, C]: the gradient of the gathered row sum of embedding_layernorm_fwd
+void embedding_layernorm_bwd(const Tensor& ids, const Tensor& pos_ids, const Tensor& seg_ids, const Tensor& word,
+                             const Tensor& pos, const Tensor& seg, const Tensor& dy, const Tensor& gamma, Tensor& dE,
+                             Tensor& part, Tensor& dgamma, Tensor& dbeta, double eps) {
+  const int64_t rows = ids.numel();
+  for (const Tensor* t : {&ids, &pos_ids, &seg_ids})
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kLong && t->is_contiguous() && t->numel() == rows,
+                "ids: contiguous int64 CUDA tensors of one size");
+  for (const Tensor* t : {&word, &pos, &seg, &dy}) check_bf16_2d(*t, "embedding_layernorm_bwd operand");
+  const int64_t C = word.size(1);
+  TORCH_CHECK(edl::layernorm_supported((int)C) && pos.size(1) == C && seg.size(1) == C && dy.size(0) == rows &&
+              dy.size(1) == C, "embedding_layernorm_bwd: tables and dy of one width C, C % 8 == 0, 8 <= C <= 1024");
+  TORCH_CHECK(dE.is_cuda() && dE.scalar_type() == at::kFloat && dE.is_contiguous() && dE.numel() == rows * C,
+              "dE: contiguous fp32 [rows, C]");
+  check_affine(dgamma, dbeta, C);
+  TORCH_CHECK(gamma.is_cuda() && gamma.scalar_type() == at::kFloat && gamma.is_contiguous() && gamma.numel() == C);
+  TORCH_CHECK(part.is_cuda() && part.scalar_type() == at::kFloat && part.is_contiguous() &&
+              part.numel() >= (int64_t)edl::layernorm_bwd_ctas(rows) * 2 * C, "part: fp32 [ctas * 2 * C]");
+  c10::cuda::CUDAGuard guard(ids.device());
+  edl::embedding_layernorm_bwd(ids.data_ptr<int64_t>(), pos_ids.data_ptr<int64_t>(), seg_ids.data_ptr<int64_t>(),
+                               word.data_ptr(), word.size(0), pos.data_ptr(), pos.size(0), seg.data_ptr(), seg.size(0),
+                               dy.data_ptr(), gamma.data_ptr<float>(), dE.data_ptr<float>(), part.data_ptr<float>(),
+                               dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), rows, (int)C, (float)eps,
+                               at::cuda::getCurrentCUDAStream().stream());
+}
+
 // q uint8 [rows, C] (contiguous), sa fp32 [ceil(C/128), rows]: the block quantisation of the stored y
 void check_quant_out(const Tensor& y, const Tensor& q, const Tensor& sa) {
   const int64_t rows = y.size(0), C = y.size(1);
@@ -156,6 +232,10 @@ void register_transformer_bindings(pybind11::module_& m) {
   m.def("attention_varlen_supported", &edl::attention_varlen_supported);
   m.def("layernorm_fwd", &layernorm_fwd);
   m.def("layernorm_supported", &edl::layernorm_supported);
+  m.def("attention_bwd", &attention_bwd);
+  m.def("layernorm_bwd", &layernorm_bwd);
+  m.def("layernorm_bwd_ctas", &edl::layernorm_bwd_ctas);
+  m.def("embedding_layernorm_bwd", &embedding_layernorm_bwd);
   m.def("embedding_layernorm_fwd", &embedding_layernorm_fwd);
   m.def("layernorm_e4m3_fwd", &layernorm_e4m3_fwd);
   m.def("embedding_layernorm_e4m3_fwd", &embedding_layernorm_e4m3_fwd);

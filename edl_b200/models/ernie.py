@@ -309,9 +309,62 @@ class ErnieEncoder(nn.Module):
         return F.linear(pooled, self.cls_w.to(f32), self.cls_b.to(f32))
 
 
+class ErnieStudent(ErnieEncoder):
+    """A trainable ``ErnieEncoder``: the Transformer student of the NLP distillation.
+
+    Same layers and parameter names as ``ErnieEncoder``, so a trained student's ``state_dict()`` loads into an
+    ``ErnieEncoder`` of the same configuration and can be served by ``teacher_server`` unchanged.  The parameters are
+    fp32 master copies; on CUDA each forward casts the matrices to bf16 and runs the training kernels of
+    ops/transformer.py (attention and its backward, LayerNorm and embedding-LayerNorm with their backward, FFN1 with
+    the GELU training epilogue and FFN2's gelu'-epilogue dgrad, residual gradients fused into the dgrad GEMMs).  On CPU
+    the forward is the encoder's float32 reference under torch autograd.  Dropout is not implemented (p = 0).
+
+    ``forward`` also takes the token ids alone: positions are then 0 .. L - 1, segments 0 and the mask ``ids != 0``."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.requires_grad_(True)
+
+    def enable_fp8(self, scaling="block"):
+        raise ValueError("ErnieStudent trains in bf16; load its state dict into an ErnieEncoder to serve it in FP8")
+
+    def forward(self, input_ids, position_ids=None, segment_ids=None, input_mask=None):
+        """ids int64 [B, L] (and optionally the other three feeds, [B, L]).  Returns fp32 logits [B, num_labels]."""
+        b, l = input_ids.shape[0], input_ids.shape[1]
+        ids = input_ids.reshape(b, l).long()
+        pos = (torch.arange(l, device=ids.device).expand(b, l) if position_ids is None
+               else position_ids.reshape(b, l).long())
+        seg = torch.zeros_like(ids) if segment_ids is None else segment_ids.reshape(b, l).long()
+        keep = (ids != 0) if input_mask is None else (input_mask.reshape(b, l) != 0)
+        c = self.hidden
+        if not self.word_emb.is_cuda:
+            return self._forward_reference(ids, pos, seg, lambda qkv: ops.attention(qkv, keep, b, l, self.heads,
+                                                                                    self.head_dim),
+                                           lambda x: x.view(b, l, c)[:, 0])
+        mask = keep.to(torch.uint8).contiguous()
+        x = ops.embedding_layernorm_trainable(ids, pos, seg, self.word_emb, self.pos_emb, self.seg_emb, self.emb_ln_g,
+                                              self.emb_ln_b, self.eps)
+        for lyr in self.layers:
+            h = ops.attention_block(x, lyr.qkv_w, lyr.qkv_b, lyr.out_w, lyr.out_b, mask, b, l, self.heads)
+            x = ops.layer_norm_trainable(h, lyr.ln1_g, lyr.ln1_b, self.eps)
+            h = ops.gelu_ffn(x, lyr.ffn1_w, lyr.ffn1_b, lyr.ffn2_w, lyr.ffn2_b)
+            x = ops.layer_norm_trainable(h, lyr.ln2_g, lyr.ln2_b, self.eps)
+        bf = torch.bfloat16
+        pooled = torch.tanh(ops.linear_bf16(x.view(b, l, c)[:, 0], self.pool_w.to(bf), self.pool_b))
+        n = self.num_labels
+        pad = max(CLS_PAD, -(-n // CLS_PAD) * CLS_PAD) - n          # TMA-describable classifier rows, as the encoder
+        logits = ops.linear_bf16(pooled, F.pad(self.cls_w, (0, 0, 0, pad)).to(bf), F.pad(self.cls_b, (0, pad)))
+        return logits[:, :n].float()
+
+
 def ernie_base(num_labels=2):
     """ERNIE 1.0 base: vocabulary 18000, hidden 768, 12 layers, 12 heads, FFN 3072, 513 positions, 2 segment types."""
     return ErnieEncoder(18000, 768, 12, 12, 3072, 513, 2, num_labels)
+
+
+def ernie_student(num_labels=2):
+    """The Transformer student: the teacher's vocabulary (18000) and feeds, hidden 384, 4 layers, 6 heads, FFN 1536."""
+    return ErnieStudent(18000, 384, 4, 6, 1536, 513, 2, num_labels)
 
 
 def ernie_tiny(num_labels=2):

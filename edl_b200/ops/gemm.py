@@ -369,6 +369,57 @@ def linear_bf16(x, weight, bias=None, relu=False, gelu=False):
     return _LinearFn.apply(x, weight, bias, relu, *_grad_sink(weight), *_grad_sink(bias))
 
 
+def _gelu_gemm_ok(*ts):
+    from . import native
+
+    return (all(t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(-1) == 1 and t.stride(0) % 8 == 0
+                and t.data_ptr() % 16 == 0 for t in ts) and native().persistent_gemm_enabled())
+
+
+def gemm_bf16_gelu_train(x, w, bias=None):
+    """The training forward of a GELU linear layer: returns (y, u) with u = bf16(x @ w^T + bias) and
+    y = bf16(gelu(x @ w^T + bias)) (erf form, from the fp32 value, so y is what the inference epilogue stores).
+    x [M, K], w [N, K] bf16, N % 8 == 0; one persistent GEMM whose epilogue writes both."""
+    from . import native, count_launch, count_fallback
+
+    m, n = x.shape[0], w.shape[0]
+    if x.is_cuda and n % 8 == 0 and _gelu_gemm_ok(x, w):
+        y = torch.empty((m, n), device=x.device, dtype=torch.bfloat16)
+        u = torch.empty_like(y)
+        native().gemm_bf16_gelu_train(x, w, y, u, bias.float().contiguous() if bias is not None else None)
+        count_launch()
+        return y, u
+    if x.is_cuda:
+        count_fallback("gemm_bf16_gelu_train: no kernel for %s x %s: fp32 matmul on the library"
+                       % (tuple(x.shape), tuple(w.shape)))
+    uf = x.float() @ w.float().t() + (bias.float() if bias is not None else 0.0)
+    return torch.nn.functional.gelu(uf).to(x.dtype), uf.to(x.dtype)
+
+
+def gelu_grad_reference(u):
+    """gelu'(u) = Phi(u) + u phi(u) in fp32."""
+    uf = u.float()
+    return 0.5 * (1.0 + torch.erf(uf * 0.7071067811865476)) + uf * 0.3989422804014327 * torch.exp(-0.5 * uf * uf)
+
+
+def gemm_bf16_gelu_grad(dy, w, u):
+    """dU = (dy @ w) * gelu'(u) in fp32, stored bf16: the dgrad of the layer after a GELU, dy [M, N2], w [N2, N] bf16
+    (that layer's weight), u [M, N] the saved pre-activation.  One persistent dgrad GEMM; gelu'(u) is applied in its
+    epilogue, which reads u through the fused-addend path."""
+    from . import native, count_launch, count_fallback
+
+    m, n = dy.shape[0], w.shape[1]
+    if dy.is_cuda and n % 8 == 0 and _gelu_gemm_ok(dy, w, u):
+        du = torch.empty((m, n), device=dy.device, dtype=torch.bfloat16)
+        native().gemm_bf16_gelu_grad(dy, w, du, u)
+        count_launch()
+        return du
+    if dy.is_cuda:
+        count_fallback("gemm_bf16_gelu_grad: no kernel for %s x %s: fp32 matmul on the library"
+                       % (tuple(dy.shape), tuple(w.shape)))
+    return ((dy.float() @ w.float()) * gelu_grad_reference(u)).to(dy.dtype)
+
+
 # EDL_PAIR_WGRAD=0: the library's weight gradient for the 32-channel stem convolutions as well
 PAIR_WGRAD = __import__("os").environ.get("EDL_PAIR_WGRAD", "1") == "1"
 

@@ -60,7 +60,7 @@ def attention(qkv, mask, batch, seq_len, heads, head_dim=64, out=None):
     m = None
     if mask is not None:
         m = mask if (mask.dtype == torch.uint8 and mask.is_contiguous()) else (mask != 0).to(torch.uint8).contiguous()
-    native().attention_fwd(qkv, m, out, batch, seq_len, heads)
+    native().attention_fwd(qkv, m, out, batch, seq_len, heads, None)
     count_launch()
     return out
 
@@ -263,3 +263,328 @@ def embedding_layernorm_e4m3(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta,
                % (word.shape[1], word.dtype))
     y = embedding_layernorm_reference(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps)
     return (y,) + quantize_e4m3_blocks_reference(y)
+
+
+# ------------------------------------------------------------------------------------------------------------ training
+# The training path of the Transformer student (models/ernie.py ErnieStudent).  Each entry point below takes the float
+# master parameters and casts the matrices to bf16 at every forward.  On CUDA the forward and backward run on the
+# package's kernels (attention.cu / attention_bwd.cu, layernorm.cu, the persistent GEMM with its GELU epilogues); on CPU,
+# and for shapes the kernels do not take (counted through ``count_fallback`` on CUDA), the float32 references run under
+# torch autograd.  Dropout is not implemented: the student trains with p = 0.  Nothing reads back to the host, so a
+# whole training step can be captured in a CUDA graph.
+def _needs_grad(*ts):
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
+
+
+def _bf16(t):
+    return t if t.dtype == torch.bfloat16 else t.to(torch.bfloat16)
+
+
+def _bias_grad(db, bias, sink):
+    """A bias gradient the way ``_LinearFn`` delivers it: into the flat gradient bucket when the parameter has a sink
+    (returns None to autograd), else returned in the parameter's dtype."""
+    s, ready = sink
+    if s is not None:
+        s.add_(db)
+        if ready is not None:
+            ready()
+        return None
+    return db.to(bias.dtype)
+
+
+def _wgrad_to(dy, x, w, sink):
+    from .gemm import _wgrad
+
+    g = _wgrad(dy, x, w.shape, *sink)
+    return None if g is None else g.to(w.dtype)
+
+
+def attention_train_supported(x, batch, seq_len, heads, head_dim=64) -> bool:
+    from . import native
+
+    return (x.is_cuda and x.dim() == 2 and x.shape[0] == batch * seq_len and x.shape[1] % 8 == 0
+            and native().attention_supported(batch, seq_len, heads, head_dim))
+
+
+def attention_forward_saved(qkv, mask, batch, seq_len, heads):
+    """The kernel forward with the statistics the backward needs: (out bf16 [B * L, H * 64], lse fp32 [B, H, L])."""
+    from . import native, count_launch
+
+    out = torch.empty((batch * seq_len, heads * 64), device=qkv.device, dtype=torch.bfloat16)
+    lse = torch.empty((batch, heads, seq_len), device=qkv.device, dtype=torch.float32)
+    native().attention_fwd(qkv, mask, out, batch, seq_len, heads, lse)
+    count_launch()
+    return out, lse
+
+
+def attention_backward(qkv, mask, out, lse, dout, batch, seq_len, heads):
+    """dqkv bf16 [B * L, 3 * H * 64] (dQ | dK | dV in qkv's layout) of ``attention``, from the forward's ``out`` and
+    ``lse`` (``attention_forward_saved``) and the output gradient ``dout``."""
+    from . import native, count_launch
+
+    dqkv = torch.empty_like(qkv)
+    delta = torch.empty((batch, heads, seq_len), device=qkv.device, dtype=torch.float32)
+    native().attention_bwd(qkv, mask, out, lse, _bf16(dout).contiguous(), dqkv, delta, batch, seq_len, heads)
+    count_launch(3)
+    return dqkv
+
+
+def _mask_u8(mask, device):
+    if mask is None:
+        return None
+    return mask if (mask.dtype == torch.uint8 and mask.is_contiguous()) else (mask != 0).to(torch.uint8).contiguous()
+
+
+class _AttentionFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, qkv, mask, batch, seq_len, heads):
+        qkv = _bf16(qkv).contiguous()
+        out, lse = attention_forward_saved(qkv, mask, batch, seq_len, heads)
+        ctx.save_for_backward(qkv, mask, out, lse)
+        ctx.shape = (batch, seq_len, heads)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        qkv, mask, out, lse = ctx.saved_tensors
+        return attention_backward(qkv, mask, out, lse, dout, *ctx.shape), None, None, None, None
+
+
+def attention_trainable(qkv, mask, batch, seq_len, heads, head_dim=64):
+    """``attention`` with a gradient: the kernel path saves lse and runs attention_bwd.cu in the backward."""
+    if qkv.is_cuda and attention_supported(_bf16(qkv).contiguous(), batch, seq_len, heads, head_dim):
+        return _AttentionFn.apply(qkv, _mask_u8(mask, qkv.device), batch, seq_len, heads)
+    if qkv.is_cuda:
+        _count("attention: no training kernel for B %d, L %d, H %d, head dim %d: float32 math on the library"
+               % (batch, seq_len, heads, head_dim))
+    return attention_reference(qkv.float(), mask, batch, seq_len, heads, head_dim)
+
+
+class _AttentionBlockFn(torch.autograd.Function):
+    """h = attention(x W_qkv^T + b_qkv) W_o^T + b_o + x, the attention half of a post-LN encoder layer before its
+    LayerNorm.  Backward: dctx = dh W_o, dqkv by attention_bwd.cu, and dx = dqkv W_qkv + dh as ONE dgrad GEMM with the
+    residual gradient as its fused addend; dW_qkv and dW_o through ``_wgrad``."""
+
+    @staticmethod
+    def forward(ctx, x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, sinks):
+        from .gemm import gemm_bf16
+
+        x = _bf16(x).contiguous()
+        wq, wo = _bf16(qkv_w).contiguous(), _bf16(out_w).contiguous()
+        qkv = gemm_bf16(x, wq, col_shift=qkv_b.float())
+        o, lse = attention_forward_saved(qkv, mask, batch, seq_len, heads)
+        h = gemm_bf16(o, wo, col_shift=out_b.float(), add=x)
+        ctx.save_for_backward(x, wq, wo, qkv, o, lse, mask, qkv_w, qkv_b, out_w, out_b)
+        ctx.shape, ctx.sinks = (batch, seq_len, heads), sinks
+        return h
+
+    @staticmethod
+    def backward(ctx, dh):
+        from .gemm import gemm_bf16
+
+        x, wq, wo, qkv, o, lse, mask, qkv_w, qkv_b, out_w, out_b = ctx.saved_tensors
+        dh = _bf16(dh).contiguous()
+        dctx = gemm_bf16(dh, wo, b_mn_major=True)
+        dqkv = attention_backward(qkv, mask, o, lse, dctx, *ctx.shape)
+        dx = gemm_bf16(dqkv, wq, b_mn_major=True, add=dh) if ctx.needs_input_grad[0] else None
+        s = ctx.sinks
+        g = [None] * 4
+        if ctx.needs_input_grad[1]:
+            g[0] = _wgrad_to(dqkv, x, qkv_w, s[0])
+        if ctx.needs_input_grad[2]:
+            g[1] = _bias_grad(dqkv.float().sum(0), qkv_b, s[1])
+        if ctx.needs_input_grad[3]:
+            g[2] = _wgrad_to(dh, o, out_w, s[2])
+        if ctx.needs_input_grad[4]:
+            g[3] = _bias_grad(dh.float().sum(0), out_b, s[3])
+        return (dx, *g, None, None, None, None, None)
+
+
+def attention_block_reference(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads):
+    f = torch.float32
+    xf = x.float()
+    qkv = torch.nn.functional.linear(xf, qkv_w.to(f), qkv_b.to(f))
+    o = attention_reference(qkv, mask, batch, seq_len, heads, qkv_w.shape[0] // (3 * heads))
+    return torch.nn.functional.linear(o, out_w.to(f), out_b.to(f)) + xf
+
+
+def attention_block(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads):
+    """Attention sub-layer with its residual: attention(x W_qkv^T + b_qkv) W_o^T + b_o + x, x [B * L, C] (bf16 on
+    CUDA), the weights in any float dtype (cast to bf16 here), ``mask`` [B, L] (nonzero = attend) or None.  Returns
+    bf16 on the kernel path (the input of the following LayerNorm); differentiable in x and the four parameters."""
+    from .gemm import _grad_sink
+
+    c = x.shape[-1]
+    if x.is_cuda and c % 8 == 0 and c == heads * 64 and attention_train_supported(x, batch, seq_len, heads):
+        sinks = tuple(_grad_sink(p) for p in (qkv_w, qkv_b, out_w, out_b))
+        return _AttentionBlockFn.apply(x, qkv_w, qkv_b, out_w, out_b, _mask_u8(mask, x.device), batch, seq_len, heads,
+                                       sinks)
+    if x.is_cuda:
+        _count("attention_block: no kernel for B %d, L %d, H %d, width %d: float32 math on the library"
+               % (batch, seq_len, heads, c))
+    return attention_block_reference(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads)
+
+
+class _GeluFfnFn(torch.autograd.Function):
+    """h = gelu(x W1^T + b1) W2^T + b2 + x, the feed-forward half of a post-LN encoder layer before its LayerNorm.
+    FFN1 runs the GELU training epilogue (stores gelu(u) for FFN2 and u for the backward); FFN2's dgrad applies gelu'(u)
+    in its epilogue, so dU comes out of one GEMM; dx = dU W1 + dh is one dgrad GEMM with the residual gradient fused."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2, sinks):
+        from .gemm import gemm_bf16, gemm_bf16_gelu_train
+
+        x = _bf16(x).contiguous()
+        w1h, w2h = _bf16(w1).contiguous(), _bf16(w2).contiguous()
+        y, u = gemm_bf16_gelu_train(x, w1h, b1.float())
+        h = gemm_bf16(y, w2h, col_shift=b2.float(), add=x)
+        ctx.save_for_backward(x, w1h, w2h, y, u, w1, b1, w2, b2)
+        ctx.sinks = sinks
+        return h
+
+    @staticmethod
+    def backward(ctx, dh):
+        from .gemm import gemm_bf16, gemm_bf16_gelu_grad
+
+        x, w1h, w2h, y, u, w1, b1, w2, b2 = ctx.saved_tensors
+        dh = _bf16(dh).contiguous()
+        du = gemm_bf16_gelu_grad(dh, w2h, u)
+        dx = gemm_bf16(du, w1h, b_mn_major=True, add=dh) if ctx.needs_input_grad[0] else None
+        s = ctx.sinks
+        g = [None] * 4
+        if ctx.needs_input_grad[1]:
+            g[0] = _wgrad_to(du, x, w1, s[0])
+        if ctx.needs_input_grad[2]:
+            g[1] = _bias_grad(du.float().sum(0), b1, s[1])
+        if ctx.needs_input_grad[3]:
+            g[2] = _wgrad_to(dh, y, w2, s[2])
+        if ctx.needs_input_grad[4]:
+            g[3] = _bias_grad(dh.float().sum(0), b2, s[3])
+        return (dx, *g, None)
+
+
+def gelu_ffn_reference(x, w1, b1, w2, b2):
+    f = torch.float32
+    xf = x.float()
+    u = torch.nn.functional.linear(xf, w1.to(f), b1.to(f))
+    return torch.nn.functional.linear(torch.nn.functional.gelu(u), w2.to(f), b2.to(f)) + xf
+
+
+def gelu_ffn(x, w1, b1, w2, b2):
+    """Feed-forward sub-layer with its residual: gelu(x W1^T + b1) W2^T + b2 + x (erf GELU), x [rows, C] (bf16 on
+    CUDA), weights in any float dtype.  This is the trainable GELU linear: its backward needs FFN2's dgrad, which is
+    where gelu'(u) is applied.  Returns bf16 on the kernel path; differentiable in x and the four parameters."""
+    from .gemm import _grad_sink, _tma_compatible
+    from . import native
+
+    ffn, c = w1.shape
+    if (x.is_cuda and x.dim() == 2 and c % 8 == 0 and ffn % 8 == 0 and native().persistent_gemm_enabled()
+            and _tma_compatible(_bf16(x).contiguous(), _bf16(w1), None, ffn)):
+        sinks = tuple(_grad_sink(p) for p in (w1, b1, w2, b2))
+        return _GeluFfnFn.apply(x, w1, b1, w2, b2, sinks)
+    if x.is_cuda:
+        _count("gelu_ffn: no kernel for x %s, FFN %d (persistent GEMM on, widths % 8 == 0): float32 math on the library"
+               % (tuple(x.shape), ffn))
+    return gelu_ffn_reference(x, w1, b1, w2, b2)
+
+
+def _ln_part(rows, c, device):
+    from . import native
+
+    return torch.empty(native().layernorm_bwd_ctas(rows) * 2 * c, device=device, dtype=torch.float32)
+
+
+class _LayerNormFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, gamma, beta, eps):
+        from . import native, count_launch
+
+        x = _bf16(x).contiguous()
+        y = torch.empty_like(x)
+        native().layernorm_fwd(x, gamma.float().contiguous(), beta.float().contiguous(), y, float(eps))
+        count_launch()
+        ctx.save_for_backward(x, gamma, beta)
+        ctx.eps = eps
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        from . import native, count_launch
+
+        x, gamma, beta = ctx.saved_tensors
+        dy = _bf16(dy).contiguous()
+        dx = torch.empty_like(x)
+        c = x.shape[1]
+        dg = torch.empty(c, device=x.device, dtype=torch.float32)
+        db = torch.empty_like(dg)
+        native().layernorm_bwd(x, dy, gamma.float().contiguous(), dx, _ln_part(x.shape[0], c, x.device), dg, db,
+                               float(ctx.eps))
+        count_launch(2)
+        return dx, dg.to(gamma.dtype), db.to(beta.dtype), None
+
+
+def layer_norm_trainable(x, gamma, beta, eps=1e-12):
+    """``layer_norm`` with a gradient: the forward kernel, and layernorm_bwd (dx from the saved input, dgamma / dbeta by
+    per-CTA partials and a fixed-order reduction)."""
+    if x.is_cuda and layer_norm_supported(_bf16(x).contiguous()):
+        return _LayerNormFn.apply(x, gamma, beta, eps)
+    if x.is_cuda:
+        _count("layer_norm: no training kernel for %s %s: float32 math on the library" % (tuple(x.shape), x.dtype))
+    return layer_norm_reference(x.float(), gamma, beta, eps)
+
+
+_ONE_HOT_ROWS = 1024
+
+
+def _table_grad(dE, idx, rows):
+    if rows <= _ONE_HOT_ROWS:
+        return torch.nn.functional.one_hot(idx, rows).to(dE.dtype).t() @ dE
+    return torch.ops.aten.embedding_dense_backward(dE, idx, rows, -1, False)
+
+
+class _EmbeddingLayerNormFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps):
+        tabs = tuple(_bf16(t).contiguous() for t in (word, pos, seg))
+        ids, pos_ids, seg_ids = (t.reshape(-1).to(word.device, torch.int64).contiguous() for t in (ids, pos_ids, seg_ids))
+        y = embedding_layernorm(ids, pos_ids, seg_ids, *tabs, gamma, beta, eps)
+        ctx.save_for_backward(ids, pos_ids, seg_ids, *tabs, gamma, beta)
+        ctx.eps = eps
+        ctx.dtypes = (word.dtype, pos.dtype, seg.dtype)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        from . import native, count_launch
+
+        ids, pos_ids, seg_ids, word, pos, seg, gamma, beta = ctx.saved_tensors
+        rows, c = ids.numel(), word.shape[1]
+        dE = torch.empty((rows, c), device=word.device, dtype=torch.float32)
+        dg = torch.empty(c, device=word.device, dtype=torch.float32)
+        db = torch.empty_like(dg)
+        native().embedding_layernorm_bwd(ids, pos_ids, seg_ids, word, pos, seg, _bf16(dy).contiguous(),
+                                         gamma.float().contiguous(), dE, _ln_part(rows, c, word.device), dg, db,
+                                         float(ctx.eps))
+        count_launch(2)
+        # the three table gradients, dE summed per table row.  The word table: the library's embedding backward, the
+        # call nn.Embedding makes for the BiLSTM student.  The position and segment tables (at most _ONE_HOT_ROWS rows)
+        # see every id many times per batch, where that call was measured to vary from run to run; for them the sum is a
+        # one-hot GEMM, which is bitwise reproducible.
+        grads = [None if not ctx.needs_input_grad[3 + i] else _table_grad(dE, idx, tab.shape[0]).to(dt)
+                 for i, (idx, tab, dt) in enumerate(zip((ids, pos_ids, seg_ids), (word, pos, seg), ctx.dtypes))]
+        return None, None, None, *grads, dg.to(gamma.dtype), db.to(beta.dtype), None
+
+
+def embedding_layernorm_trainable(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps=1e-12):
+    """``embedding_layernorm`` with a gradient in the three tables and gamma / beta (tables in any float dtype, cast
+    to bf16 for the kernels).  Out-of-range ids raise as in ``embedding_layernorm``."""
+    c = word.shape[1]
+    from . import native
+
+    if word.is_cuda and all(t.is_cuda and t.dim() == 2 and t.shape[1] == c for t in (pos, seg)) \
+            and native().layernorm_supported(c):
+        return _EmbeddingLayerNormFn.apply(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps)
+    if word.is_cuda:
+        _count("embedding_layernorm: no training kernel for width %d: float32 math on the library" % c)
+    f = torch.float32
+    return embedding_layernorm_reference(ids, pos_ids, seg_ids, word.to(f), pos.to(f), seg.to(f), gamma, beta, eps)

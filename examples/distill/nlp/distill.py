@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Sentence-classification distillation: BOW / TextCNN / BiLSTM student, served sequence teacher, ``KL_T`` loss
+"""Sentence-classification distillation: BOW / TextCNN / BiLSTM / Transformer student, served sequence teacher, ``KL_T`` loss
 with T=2 and a batch generator carrying token ids (reference: example/distill/nlp/distill.py:98-196,
 model.py:54-135; the reference's teacher is an ERNIE served by Paddle Serving -- any served model
 that returns ``logits`` works here; a TextCNN stands in when none is given)."""
@@ -14,6 +14,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.dirna
 from paddle_edl.distill.distill_reader import DistillReader  # noqa: E402
 from paddle_edl.distill.teacher_server import TeacherServer  # noqa: E402
 from paddle_edl.models.small import BOW, BiLSTM, TextCNN, kl_distill_loss  # noqa: E402
+from paddle_edl.models.ernie import ernie_student  # noqa: E402
 
 
 def corpus(n, vocab, seq, seed):
@@ -27,7 +28,7 @@ def corpus(n, vocab, seq, seed):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="bow", choices=["bow", "cnn", "lstm"])
+    ap.add_argument("--model", default="bow", choices=["bow", "cnn", "lstm", "ernie"])
     ap.add_argument("--teachers", default="")
     ap.add_argument("--T", type=float, default=2.0)
     ap.add_argument("--epochs", type=int, default=2)
@@ -39,12 +40,13 @@ def main():
         srv = TeacherServer(teacher, ["ids"], ["logits"], {"ids": [64]}).start()
         args.teachers = srv.endpoint
     dev = torch.device("cpu")
-    if args.model == "lstm":            # the LSTM student runs on the GPU when there is one (csrc/lstm.cu)
+    if args.model in ("lstm", "ernie"):  # these students run on the GPU when there is one
         dev = torch.device("cuda" if torch.cuda.is_available() else "cpu")
-        student = BiLSTM(args.vocab).to(dev)
+        # the Transformer student builds its four feeds from the ids (positions 0.., segment 0, mask ids != 0)
+        student = (BiLSTM(args.vocab) if args.model == "lstm" else ernie_student()).to(dev)
     else:
         student = BOW(args.vocab) if args.model == "bow" else TextCNN(args.vocab)
-    opt = torch.optim.AdamW(student.parameters(), 1e-3)
+    opt = torch.optim.AdamW(student.parameters(), 1e-4 if args.model == "ernie" else 1e-3)   # a Transformer wants less
 
     def batch_gen():
         buf = []

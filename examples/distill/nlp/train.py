@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Train the small student (BOW / TextCNN / BiLSTM) alone on hard labels -- the baseline the distilled student is
+"""Train the small student (BOW / TextCNN / BiLSTM / Transformer) alone on hard labels -- the baseline the distilled student is
 compared with (reference: example/distill/nlp/train.py)."""
 import argparse
 import os
@@ -12,13 +12,16 @@ sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.abspath(os.path.join(HERE, "..", "..", "..")))
 from reader import TsvReader, batches, synthetic_corpus  # noqa: E402
 from paddle_edl.models.small import BOW, BiLSTM, TextCNN  # noqa: E402
+from paddle_edl.models.ernie import ernie_student  # noqa: E402
 
 
 def build_model(name, vocab):
-    """(model, device): the LSTM student runs on the GPU when there is one (csrc/lstm.cu), the others on the CPU."""
-    if name == "lstm":
+    """(model, device): the LSTM and Transformer students run on the GPU when there is one (csrc/lstm.cu, the encoder
+    kernels), the others on the CPU.  The Transformer student has the teacher's 18000-id vocabulary and builds its four
+    feeds from the ids (positions 0.., segment 0, mask ids != 0)."""
+    if name in ("lstm", "ernie"):
         dev = torch.device("cuda" if torch.cuda.is_available() else "cpu")
-        return BiLSTM(vocab).to(dev), dev
+        return (BiLSTM(vocab) if name == "lstm" else ernie_student()).to(dev), dev
     return (BOW(vocab) if name == "bow" else TextCNN(vocab)), torch.device("cpu")
 
 
@@ -36,7 +39,7 @@ def evaluate(model, data, dev=torch.device("cpu")):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="bow", choices=["bow", "cnn", "lstm"])
+    ap.add_argument("--model", default="bow", choices=["bow", "cnn", "lstm", "ernie"])
     ap.add_argument("--train_tsv", default=None)
     ap.add_argument("--dev_tsv", default=None)
     ap.add_argument("--epochs", type=int, default=3)
@@ -55,7 +58,7 @@ def main():
         train_iter = lambda ep: batches(synthetic_corpus(args.samples, vocab, args.seq_len, ep), 16)   # noqa: E731
         dev_data = list(batches(synthetic_corpus(256, vocab, args.seq_len, 10_000), 16))
     model, dev = build_model(args.model, vocab)
-    opt = torch.optim.AdamW(model.parameters(), 1e-3)
+    opt = torch.optim.AdamW(model.parameters(), 1e-4 if args.model == "ernie" else 1e-3)   # a Transformer wants less
     for ep in range(args.epochs):
         for ids, label in train_iter(ep):
             loss = torch.nn.functional.cross_entropy(model(torch.from_numpy(ids).to(dev)),
