@@ -28,12 +28,18 @@
 // log2 units of the scaled scores (m the row max of S / 8 * log2(e), l the row sum over the bf16-rounded probabilities), or
 // +inf for a row without a valid key; attention_bwd.cu recomputes P = exp2(S / 8 * log2(e) - lse) from it.  The store
 // sits after O is formed, so O does not depend on whether lse is given.
+//
+// Dropout on the attention probabilities (padded training instantiation, kDrop): element (b, h, i, j) of P has the
+// flat index ((b H + h) L + i) L + j in the mask of philox.cuh.  A dropped probability is zeroed in the bf16 A fragment
+// after the row sum has taken it, so m, l and lse stay those of the undropped softmax (lse is bitwise the p = 0 lse) and
+// the scale 1 / (1 - p) is applied to the fp32 output together with 1 / l.
 #include <cuda.h>
 
 #include <type_traits>
 
 #include "gemm.h"
 #include "kernels.h"
+#include "philox.cuh"
 #include "ptx.cuh"
 
 namespace edl {
@@ -73,11 +79,13 @@ struct Varlen {
 };
 
 // Seq = int: the padded layout, seq = L for every sequence (tmQKV / tmO span the whole batch).  Seq = Varlen: packed.
-template <typename Seq>
+// kDrop: dropout on P with the mask of `drop` (padded layout only).
+template <typename Seq, bool kDrop = false>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO,
-                     const uint8_t* __restrict__ mask, Seq seq, int H, float* __restrict__ lse) {
+                     const uint8_t* __restrict__ mask, Seq seq, int H, float* __restrict__ lse, const PhiloxArgs drop) {
   constexpr bool kVarlen = std::is_same<Seq, Varlen>::value;
+  static_assert(!(kVarlen && kDrop), "dropout: padded layout only");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -155,6 +163,13 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};      // running max (scaled, log2 units) and row sum
+    [[maybe_unused]] PhiloxKey pk;
+    [[maybe_unused]] uint64_t nrow[2];                          // flat mask index of key 0 of this thread's two rows
+    if constexpr (kDrop) {
+      pk = philox_key(drop);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) nrow[r] = (((uint64_t)b * H + h) * L + (q0 + cw * 64 + row + 8 * r)) * (uint64_t)L;
+    }
     ptx::mbar_wait(q_bar, 0);
     const uint64_t dq = ptx::make_smem_desc(ptx::smem_u32(sq + cw * kHalfBytes), 16, 1024);
     for (int kt = 0; kt < n_kt; ++kt) {
@@ -198,12 +213,18 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
       float ls[2] = {0.f, 0.f};
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const uint32_t lo = pack_bf16(exp2f(sc[4 * j] - base[0]), exp2f(sc[4 * j + 1] - base[0]));
-        const uint32_t hi = pack_bf16(exp2f(sc[4 * j + 2] - base[1]), exp2f(sc[4 * j + 3] - base[1]));
+        uint32_t lo = pack_bf16(exp2f(sc[4 * j] - base[0]), exp2f(sc[4 * j + 1] - base[0]));
+        uint32_t hi = pack_bf16(exp2f(sc[4 * j + 2] - base[1]), exp2f(sc[4 * j + 3] - base[1]));
         const float2 flo = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&lo));
         const float2 fhi = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&hi));
         ls[0] += flo.x + flo.y;
         ls[1] += fhi.x + fhi.y;
+        if constexpr (kDrop) {
+          const int key = kt * 64 + j * 8 + cq;
+          const uint32_t k0 = dropout_keep2(pk, nrow[0] + key), k1 = dropout_keep2(pk, nrow[1] + key);
+          lo &= ((k0 & 1u) ? 0xFFFFu : 0u) | ((k0 & 2u) ? 0xFFFF0000u : 0u);
+          hi &= ((k1 & 1u) ? 0xFFFFu : 0u) | ((k1 & 2u) ? 0xFFFF0000u : 0u);
+        }
         pa[j >> 1][(j & 1) * 2] = lo;
         pa[j >> 1][(j & 1) * 2 + 1] = hi;
       }
@@ -227,7 +248,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
     for (int r = 0; r < 2; ++r) {
       l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
       l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
-      inv[r] = l[r] > 0.f ? 1.f / l[r] : 0.f;
+      inv[r] = l[r] > 0.f ? (kDrop ? drop.scale / l[r] : 1.f / l[r]) : 0.f;
     }
     if (!kVarlen && lse != nullptr && (lane & 3) == 0) {
 #pragma unroll
@@ -287,16 +308,17 @@ attention_varlen_maps_kernel(const __grid_constant__ CUtensorMap tmQKV, const __
                  ::"l"(reinterpret_cast<uint64_t>(maps + 2 * b + i)), "r"(ptx::smem_u32(s + i)) : "memory");
 }
 
-template <typename Seq>
+template <typename Seq, bool kDrop = false>
 const char* launch_attention(const CUtensorMap& tmQKV, const CUtensorMap& tmO, const uint8_t* mask, Seq seq, int H,
-                             dim3 grid, cudaStream_t stream, float* lse = nullptr) {
+                             dim3 grid, cudaStream_t stream, float* lse = nullptr, const PhiloxArgs& drop = PhiloxArgs{}) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attention_fwd_kernel<Seq>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
+    cudaError_t e = cudaFuncSetAttribute(attention_fwd_kernel<Seq, kDrop>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kAttnSmem);
     if (e != cudaSuccess) return cudaGetErrorString(e);
     attr_set = true;
   }
-  attention_fwd_kernel<Seq><<<grid, kAttnThreads, kAttnSmem, stream>>>(tmQKV, tmO, mask, seq, H, lse);
+  attention_fwd_kernel<Seq, kDrop><<<grid, kAttnThreads, kAttnSmem, stream>>>(tmQKV, tmO, mask, seq, H, lse, drop);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
@@ -322,11 +344,14 @@ bool attention_supported(int B, int L, int H, int head_dim) {
 }
 
 const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream,
-                          float* lse) {
+                          float* lse, const PhiloxArgs* drop) {
   if (!attention_supported(B, L, H, 64)) return "attention_fwd: unsupported shape (head dim 64, 1 <= L <= 512)";
+  if (drop != nullptr && lse == nullptr) return "attention_fwd: dropout is a training feature (give lse)";
   alignas(64) CUtensorMap tmQKV, tmO;
   if (const char* e = encode_attention_maps(&tmQKV, &tmO, qkv, out, L, B, H)) return e;
-  return launch_attention<int>(tmQKV, tmO, mask, L, H, dim3((L + 127) / 128, H, B), stream, lse);
+  const dim3 grid((L + 127) / 128, H, B);
+  if (drop != nullptr) return launch_attention<int, true>(tmQKV, tmO, mask, L, H, grid, stream, lse, *drop);
+  return launch_attention<int>(tmQKV, tmO, mask, L, H, grid, stream, lse);
 }
 
 bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim) {

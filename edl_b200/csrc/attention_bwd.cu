@@ -16,10 +16,16 @@
 // laid out like qkv: [B * L, 3 * H * 64] with dQ | dK | dV column blocks, so the QKV projection's dgrad and weight
 // gradient each take dqkv as one operand.
 //
-// Budgets (ptxas -v, sm_90a, 128 threads): attn_bwd_dkdv 175 registers, attn_bwd_dq 134, attn_bwd_delta 40, no spills;
+// Dropout (kDrop, the forward's attention dropout): with Z = keep * 1 / (1 - p) regenerated per element from (b, h, i, j)
+// (philox.cuh; the mask does not depend on the tile order), dV = (Z o P)^T dO and dS = P o (Z o dP - D), D taken over the
+// stored, dropped O as before (FlashAttention-2's identity).  A row without a valid key still gets zero gradients.
+//
+// Budgets (ptxas -v, sm_90a, 128 threads): attn_bwd_dkdv 175 registers (228 with dropout), attn_bwd_dq 134 (242),
+// attn_bwd_delta 40, no spills;
 // static shared memory 36.5 KB (dkdv: Q, Q^T, dO, dO^T tiles + lse / D) and 27.1 KB (dq: K, K^T, V tiles + key flags).
 #include "common.cuh"
 #include "kernels.h"
+#include "philox.cuh"
 
 namespace edl {
 namespace {
@@ -121,10 +127,11 @@ attn_bwd_delta(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __res
   }
 }
 
+template <bool kDrop>
 __global__ void __launch_bounds__(128)
 attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ mask,
               const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse, const float* __restrict__ delta,
-              __nv_bfloat16* __restrict__ dqkv, int L, int H) {
+              __nv_bfloat16* __restrict__ dqkv, int L, int H, const PhiloxArgs drop) {
   __shared__ alignas(16) __nv_bfloat16 sQ[kT * kP], sQt[kT * kP], sO[kT * kP], sOt[kT * kP];
   __shared__ float sL[kT], sD[kT];
   const int k0 = blockIdx.x * kT, h = blockIdx.y, b = blockIdx.z;
@@ -151,6 +158,8 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
   for (int j = 0; j < 8; ++j)
 #pragma unroll
     for (int e = 0; e < 4; ++e) dk[j][e] = dv[j][e] = 0.f;
+  [[maybe_unused]] PhiloxKey pk;
+  if constexpr (kDrop) pk = philox_key(drop);
 
   for (int q0 = 0; q0 < L; q0 += kT) {
     __syncthreads();                                        // the previous tiles (or the K / V staging) are consumed
@@ -162,6 +171,17 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
       sD[threadIdx.x] = q < L ? delta[sh + q] : 0.f;
     }
     __syncthreads();
+    // keep bits of this thread's 32 elements, bit j * 4 + e of accumulator element [j][e] (formed before the
+    // accumulators are live: the Philox rounds then need no registers the products hold)
+    [[maybe_unused]] uint32_t km = 0;
+    if constexpr (kDrop) {
+#pragma unroll 1
+      for (int i = 0; i < 32; ++i) {
+        const int qc = (i >> 2) * 8 + 2 * t + (i & 1);
+        const uint64_t n = ((uint64_t)sh + (q0 + qc)) * (uint64_t)L + (key0 + 8 * ((i >> 1) & 1));
+        km |= dropout_keep(pk, n) ? 1u << i : 0u;
+      }
+    }
     // S^T (keys x queries) and dP^T = V dO^T
     float p[8][4], dp[8][4];
 #pragma unroll
@@ -176,8 +196,14 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
       for (int e = 0; e < 4; ++e) {
         const int qc = j * 8 + 2 * t + (e & 1);
         const float pe = kv[e >> 1] ? exp2f(p[j][e] * kScaleLog2 - sL[qc]) : 0.f;
-        p[j][e] = pe;
-        dp[j][e] = pe * (dp[j][e] - sD[qc]);
+        if constexpr (kDrop) {
+          const float z = (km >> (j * 4 + e)) & 1u ? pk.scale : 0.f;
+          p[j][e] = pe * z;
+          dp[j][e] = pe * (dp[j][e] * z - sD[qc]);
+        } else {
+          p[j][e] = pe;
+          dp[j][e] = pe * (dp[j][e] - sD[qc]);
+        }
       }
     // dV += P^T dO, dK += dS^T Q (the queries are the k dimension: B operands from the transposed tiles)
     uint32_t pa[4][4], sa[4][4];
@@ -198,10 +224,11 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
   store_rows(dv, drow + (2 * H + h) * 64, ldq, key0, L, t, 1.f);
 }
 
+template <bool kDrop>
 __global__ void __launch_bounds__(128)
 attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ mask,
             const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse, const float* __restrict__ delta,
-            __nv_bfloat16* __restrict__ dqkv, int L, int H) {
+            __nv_bfloat16* __restrict__ dqkv, int L, int H, const PhiloxArgs drop) {
   __shared__ alignas(16) __nv_bfloat16 sK[kT * kP], sKt[kT * kP], sV[kT * kP];
   __shared__ uint8_t sM[kT];
   const int q0 = blockIdx.x * kT, h = blockIdx.y, b = blockIdx.z;
@@ -229,6 +256,8 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
   for (int j = 0; j < 8; ++j)
 #pragma unroll
     for (int e = 0; e < 4; ++e) dq[j][e] = 0.f;
+  [[maybe_unused]] PhiloxKey pk;
+  if constexpr (kDrop) pk = philox_key(drop);
 
   for (int kb = 0; kb < L; kb += kT) {
     __syncthreads();
@@ -247,13 +276,25 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
     mma_rows(s, qf, sK, g, t);
     mma_rows(dp, of, sV, g, t);
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
+    for (int j = 0; j < 8; ++j) {
+      [[maybe_unused]] uint32_t keep[2];
+      if constexpr (kDrop) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+          keep[r] = dropout_keep2(pk, ((uint64_t)sh + (qr + 8 * r)) * (uint64_t)L + (kb + j * 8 + 2 * t));
+      }
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int kc = j * 8 + 2 * t + (e & 1);
         const float pe = sM[kc] ? exp2f(s[j][e] * kScaleLog2 - rl[e >> 1]) : 0.f;
-        s[j][e] = pe * (dp[j][e] - rd[e >> 1]);
+        if constexpr (kDrop) {
+          const float z = (keep[e >> 1] >> (e & 1)) & 1u ? pk.scale : 0.f;
+          s[j][e] = pe * (dp[j][e] * z - rd[e >> 1]);
+        } else {
+          s[j][e] = pe * (dp[j][e] - rd[e >> 1]);
+        }
       }
+    }
     uint32_t sa[4][4];
     acc_to_afrag(s, sa);
 #pragma unroll
@@ -270,7 +311,7 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
 }  // namespace
 
 const char* attention_bwd(const void* qkv, const uint8_t* mask, const void* out, const float* lse, const void* dout,
-                          void* dqkv, float* delta, int B, int L, int H, cudaStream_t stream) {
+                          void* dqkv, float* delta, int B, int L, int H, cudaStream_t stream, const PhiloxArgs* drop) {
   if (!attention_supported(B, L, H, 64)) return "attention_bwd: unsupported shape (head dim 64, 1 <= L <= 512)";
   const auto* q = reinterpret_cast<const __nv_bfloat16*>(qkv);
   const auto* o = reinterpret_cast<const __nv_bfloat16*>(out);
@@ -279,8 +320,13 @@ const char* attention_bwd(const void* qkv, const uint8_t* mask, const void* out,
   const int64_t rows = (int64_t)B * L;
   attn_bwd_delta<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(o, d, delta, B, L, H);
   const dim3 grid((L + kT - 1) / kT, H, B);
-  attn_bwd_dkdv<<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H);
-  attn_bwd_dq<<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H);
+  if (drop != nullptr) {
+    attn_bwd_dkdv<true><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, *drop);
+    attn_bwd_dq<true><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, *drop);
+  } else {
+    attn_bwd_dkdv<false><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, PhiloxArgs{});
+    attn_bwd_dq<false><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, PhiloxArgs{});
+  }
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }

@@ -527,6 +527,7 @@ const char* gemm_bf16(const GemmArgs& g, cudaStream_t stream) {
   if (!g.a_mn_major && g.ship_flag == nullptr && persistent_gemm_enabled()) return gemm_bf16_persistent(g, stream);
   if (g.add_src != nullptr) return "gemm add_src is implemented by the persistent kernel only";
   if (g.gelu || g.gelu_grad) return "gemm GELU epilogue is implemented by the persistent kernel only";
+  if (g.dropout != nullptr) return "gemm residual-dropout epilogue is implemented by the persistent kernel only";
   if (g.a_mn_major && g.b_mn_major)   // weight gradient
     return n64 ? launch_variant<64, 4, true, true, 1>(g, stream) : launch_variant<128, 3, true, true, 1>(g, stream);
   if (!g.a_mn_major && !g.b_mn_major)

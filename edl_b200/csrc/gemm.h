@@ -5,6 +5,8 @@
 
 namespace edl {
 
+struct PhiloxArgs;   // kernels.h
+
 // Fused BatchNorm-backward reduction (persistent dgrad kernels): the GEMM / conv output D is the gradient
 // dy of a BN layer's output; the epilogue accumulates dsums[0:C] += sum(dy_m), dsums[C:2C] += sum(dy_m * xhat)
 // (dy_m = dy masked by the layer's ReLU) so that the BN backward needs no reduction pass of its own.
@@ -60,6 +62,9 @@ struct GemmArgs {
   int64_t ld_u = 0;
   // D = (A*B) * gelu'(add_src) in fp32 (B MN-major, add_src = u): the dgrad of FFN2 that yields dU of FFN1
   bool gelu_grad = false;
+  // D = add_src + Z o (A*B^T + col_shift), Z the dropout mask of *dropout at flat index row * N + col (B K-major, an
+  // addend, no scale / ReLU / statistics): the residual branch of a Transformer layer in training.  Persistent kernel only.
+  const PhiloxArgs* dropout = nullptr;
   // fused "GEMM -> peer ship" (EPI 0 only): D may be a PEER GPU's buffer (NVLink-mapped address);
   // every CTA TMA-stores its tile there, and the CTA that completes last publishes
   // *ship_flag (peer address) = seq with release/system semantics -- no separate copy kernel.

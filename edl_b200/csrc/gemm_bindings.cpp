@@ -4,6 +4,7 @@
 #include <torch/extension.h>
 
 #include "gemm.h"
+#include "kernels.h"
 
 namespace {
 using torch::Tensor;
@@ -153,6 +154,23 @@ void gemm_bf16_gelu_grad(const Tensor& A, const Tensor& B, const Tensor& D, cons
   c10::cuda::CUDAGuard guard(A.device());
   const char* err = edl::gemm_bf16(g, at::cuda::getCurrentCUDAStream().stream());
   TORCH_CHECK(err == nullptr, "edl gemm_bf16_gelu_grad failed: ", err);
+}
+
+// A residual branch with dropout: D = add + Z o (A * B^T + col_shift), Z the mask of `drop` at flat index row * N + col.
+void gemm_bf16_residual_dropout(const Tensor& A, const Tensor& B, const Tensor& D, const c10::optional<Tensor>& col_shift,
+                                const Tensor& add, const edl::PhiloxArgs& drop) {
+  edl::GemmArgs g = gemm_operands(A, B, false, false);
+  check_like_d(D, g, "D");
+  check_like_d(add, g, "add");
+  g.D = D.data_ptr();
+  g.ldd = D.stride(0);
+  g.col_shift = optp<float>(col_shift);
+  g.add_src = add.data_ptr();
+  g.ld_add = add.stride(0);
+  g.dropout = &drop;
+  c10::cuda::CUDAGuard guard(A.device());
+  const char* err = edl::gemm_bf16(g, at::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(err == nullptr, "edl gemm_bf16_residual_dropout failed: ", err);
 }
 
 // fp32 scratch for the partial tiles of a split reduction (optional: the kernels report it missing or too small)
@@ -623,6 +641,7 @@ void register_gemm_bindings(pybind11::module_& m) {
   m.def("gemm_bf16_gelu", &gemm_bf16_gelu);
   m.def("gemm_bf16_gelu_train", &gemm_bf16_gelu_train);
   m.def("gemm_bf16_gelu_grad", &gemm_bf16_gelu_grad);
+  m.def("gemm_bf16_residual_dropout", &gemm_bf16_residual_dropout);
   m.def("gemm_wgrad_bf16", &gemm_wgrad_bf16);
   m.def("conv3x3", &conv3x3);
   m.def("set_persistent_gemm", &edl::set_persistent_gemm);

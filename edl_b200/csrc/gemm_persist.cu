@@ -20,6 +20,7 @@
 #include "gemm.h"
 #include "kernels.h"
 #include "launch.h"
+#include "philox.cuh"
 #include "ptx.cuh"
 
 namespace edl {
@@ -70,6 +71,8 @@ struct PersistParams {
   // GELU == 2: the pre-activation u = acc * scale + shift, bf16 [M, N] with row pitch ld_aux
   __nv_bfloat16* aux;
   long long ld_aux;
+  // GELU == 4: the dropout mask of the GEMM result
+  PhiloxArgs drop;
 };
 constexpr int kTraceTiles = 16;
 #define EDL_TRACE(role, tile, phase)                                                                    \
@@ -147,6 +150,9 @@ EDL_DEVICE void issue_bn_tiles(const PersistParams& p, int tm, int nn0, int rows
 //   2  training forward: the same y, and also u = acc * scale + shift as bf16 into p.aux (what the backward reads)
 //   3  training dgrad (MODE 1): D = acc * gelu'(u) with gelu'(u) = Phi(u) + u phi(u) in fp32, u the bf16 addend tile
 //      (FFN2's dgrad writes dU directly)
+//   4  residual dropout (MODE 0): D = add + Z o (acc + shift), Z = keep * 1 / (1 - p) of the mask of p.drop at flat
+//      index row * N + col (philox.cuh); dropout acts before the addend, and a dropped element stores the addend's bits.
+//      The residual branches of a Transformer encoder layer (attention output projection, FFN2)
 EDL_DEVICE float gelu_grad(float u) {
   return 0.5f * (1.f + erff(u * 0.70710678118654752f)) + u * 0.39894228040143268f * __expf(-0.5f * u * u);
 }
@@ -542,11 +548,26 @@ gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       [[maybe_unused]] uint32_t mword[2] = {0u, 0u};
       const uint32_t mbase = ptx::smem_u32(sy) + row * 16 + grp * (kColsPerGrp / 8);
       if (bn_mask) ptx::mbar_wait(bn_bar, tc & 1);
+      // GELU == 4: keep bits of this thread's elements, bits 4 j + 2 h (+ 1) for column pair j of row row + 8 h, formed in
+      // a rolled loop (unrolled into the epilogue, the Philox rounds would spill the accumulators)
+      [[maybe_unused]] uint64_t kmask = 0;
+      if constexpr (GELU == 4) {
+        static_assert(kColsPerGrp / 8 * 4 <= 64, "keep bits of a thread");
+        const PhiloxKey pk = philox_key(p.drop);
+#pragma unroll 1
+        for (int j = 0; j < kColsPerGrp / 8; ++j) {
+          const uint64_t col = (uint64_t)(n0 + grp * kColsPerGrp + j * 8 + cq);
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            kmask |= (uint64_t)dropout_keep2(pk, (uint64_t)(m0 + row + 8 * h) * (uint64_t)p.N + col) << (4 * j + 2 * h);
+        }
+      }
 #pragma unroll
       for (int j = 0; j < kColsPerGrp / 8; ++j) {
         const int tcol = grp * kColsPerGrp + j * 8 + cq;        // column inside the tile
         const int col = n0 + tcol;
         float v[4] = {acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]};
+        [[maybe_unused]] float addv[4];                         // GELU == 4: the addend, added after the dropout
         const uint32_t hp = ptx::smem_u32(sd) + (tcol >> 6) * (kBlockM * 128) + cq * 2;
         const int chunk = (tcol >> 3) & 7;
         if (has_add) {
@@ -558,6 +579,9 @@ gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             if constexpr (GELU == 3) {
               v[2 * h] *= gelu_grad(t2.x);
               v[2 * h + 1] *= gelu_grad(t2.y);
+            } else if constexpr (GELU == 4) {
+              addv[2 * h] = t2.x;
+              addv[2 * h + 1] = t2.y;
             } else {
               v[2 * h] += t2.x;
               v[2 * h + 1] += t2.y;
@@ -601,6 +625,14 @@ gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           if constexpr (GELU == 1 || GELU == 2) {
 #pragma unroll
             for (int e = 0; e < 4; ++e) v[e] = 0.5f * v[e] * (1.f + erff(v[e] * 0.70710678118654752f));
+          }
+          if constexpr (GELU == 4) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const uint32_t kb = (uint32_t)(kmask >> (4 * j + 2 * h));
+              v[2 * h] = (kb & 1u) ? fmaf(v[2 * h], p.drop.scale, addv[2 * h]) : addv[2 * h];
+              v[2 * h + 1] = (kb & 2u) ? fmaf(v[2 * h + 1], p.drop.scale, addv[2 * h + 1]) : addv[2 * h + 1];
+            }
           }
         }
 #pragma unroll
@@ -928,7 +960,7 @@ template <int BLOCK_N, int STAGES, int MODE, int BNR = 0, int ASTAGES = 0, int G
 const char* launch_p(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const PersistParams& p,
                      cudaStream_t stream, const CUtensorMap* tmAdd = nullptr, const CUtensorMap* tmBnX = nullptr,
                      const CUtensorMap* tmBnY = nullptr) {
-  if constexpr (BLOCK_N >= 128) {
+  if constexpr (BLOCK_N >= 128 && GELU != 4) {    // (the residual-dropout epilogue spills with 16 warps' registers)
     if (g_epi16)
       return launch_pe<BLOCK_N, STAGES, MODE, BNR, ASTAGES, 16, GELU>(tmA, tmB, tmD, p, stream, tmAdd, tmBnX, tmBnY);
   }
@@ -969,7 +1001,7 @@ const char* gemm_bf16_persistent(const GemmArgs& g, cudaStream_t stream) {
   // L2 -> SM path delivers when every SM pulls; with N = 256 the
   // A tile is reused twice as often and the requirement drops to 96 B / clk.
   // (not with the GELU epilogue: with the erf expansion the 256-column tile spills its accumulators)
-  const bool wide = g_wide_tiles && !g.gelu && !g.gelu_grad && !g.b_mn_major && g.bn.x == nullptr && g.col_stats == nullptr && g.N % 256 == 0 &&
+  const bool wide = g_wide_tiles && !g.gelu && !g.gelu_grad && g.dropout == nullptr && !g.b_mn_major && g.bn.x == nullptr && g.col_stats == nullptr && g.N % 256 == 0 &&
                     g.K >= 256 &&
                     (int64_t)((g.M + kBlockM - 1) / kBlockM) * (g.N / 256) >= kNumSMs;
   const int bn = n64 ? 64 : (wide ? 256 : 128);
@@ -996,6 +1028,14 @@ const char* gemm_bf16_persistent(const GemmArgs& g, cudaStream_t stream) {
       return "gemm add_src needs N % 8 == 0 and 16-byte aligned rows";
     if (const char* e = tmap2d(&tmAdd, g.add_src, g.N, g.M, g.ld_add, 64, kBlockM)) return e;
     padd = &tmAdd;
+  }
+  if (g.dropout != nullptr) {
+    if (g.b_mn_major || g.add_src == nullptr || g.gelu || g.gelu_grad || g.bn.x != nullptr || g.col_stats != nullptr ||
+        g.relu || g.col_scale != nullptr)
+      return "gemm residual-dropout epilogue: forward GEMM (B K-major) with an addend and an optional shift only";
+    p.drop = *g.dropout;
+    return n64 ? launch_p<64, 6, 0, 0, 0, 4>(tmA, tmB, tmD, p, stream, padd)
+               : launch_p<128, 5, 0, 0, 0, 4>(tmA, tmB, tmD, p, stream, padd);
   }
   if (g.bn.x != nullptr) {
     // dgrad whose output is the gradient of a BatchNorm output: reduce it in the epilogue

@@ -6,6 +6,22 @@
 
 namespace edl {
 
+// ---- dropout masks (philox.cuh): one (seed, offset) pair per dropout site, drawn from torch's CUDA generator by the
+// bindings.  Element n of the site is kept iff word n % 4 of Philox4x32-10(key = seed, counter = (n / 4, offset)) is
+// >= threshold = floor(p * 2^32); a kept element is scaled by scale = fp32(1 / (1 - p)).  Under CUDA-graph capture the
+// seed and offset are read at run time from seed_ptr and offset_ptr (+ offset_intragraph), so every replay draws anew.
+struct PhiloxArgs {
+  uint64_t seed = 0;
+  uint64_t offset = 0;
+  const int64_t* seed_ptr = nullptr;     // captured: the seed lives here
+  const int64_t* offset_ptr = nullptr;   // captured: the offset is *offset_ptr + offset_intragraph
+  uint64_t offset_intragraph = 0;
+  uint32_t threshold = 0;
+  float scale = 1.f;
+};
+// y = Z o x over n bf16 elements (dropout.cu); any n, any 2-byte alignment
+void dropout_apply(const void* x, void* y, int64_t n, const PhiloxArgs& drop, cudaStream_t s);
+
 // ---- bn.cu ----
 void bn_stats(const void* x, float* sums, int64_t M, int C, cudaStream_t stream);
 // mask (optional, residual + ReLU only): also write the ReLU mask bits uint8 [M, C / 8] of the stored output; needs
@@ -211,14 +227,16 @@ constexpr int kAttnMaxLen = 512;
 bool attention_supported(int B, int L, int H, int head_dim);
 // qkv bf16 [B * L, 3 * H * 64] (Q | K | V column blocks, 16-byte aligned), mask uint8 [B, L] (1 = attend; nullptr: all),
 // out bf16 [B * L, H * 64].  lse: nullptr, or fp32 [B, H, L] that receives what the backward needs to recompute the
-// probabilities (attention.cu).  Returns nullptr or an error string.
+// probabilities (attention.cu).  drop (training, with lse): dropout on the probabilities, element (b, h, i, j) at flat
+// index ((b H + h) L + i) L + j of the mask.  Returns nullptr or an error string.
 const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream,
-                          float* lse = nullptr);
+                          float* lse = nullptr, const PhiloxArgs* drop = nullptr);
 // Backward of attention_fwd (attention_bwd.cu): from qkv, the forward's out and lse and the output gradient dout
 // (bf16 [B * L, H * 64]) writes dqkv bf16 [B * L, 3 * H * 64] (dQ | dK | dV in the layout of qkv).  delta: fp32 [B, H, L]
-// workspace.  Deterministic, no atomics.
+// workspace.  drop: the forward's dropout (the same mask is regenerated).  Deterministic, no atomics.
 const char* attention_bwd(const void* qkv, const uint8_t* mask, const void* out, const float* lse, const void* dout,
-                          void* dqkv, float* delta, int B, int L, int H, cudaStream_t stream);
+                          void* dqkv, float* delta, int B, int L, int H, cudaStream_t stream,
+                          const PhiloxArgs* drop = nullptr);
 bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim);
 // Packed sequences: qkv bf16 [T, 3 * H * 64], sequence b in rows [cu_seqlens[b], cu_seqlens[b + 1]) (int32 device
 // offsets, 1 <= length <= max_len <= 512), key_mask uint8 [T] (1 = attend; nullptr: all), out bf16 [T, H * 64];
@@ -232,11 +250,12 @@ bool layernorm_supported(int C);
 void layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y, int64_t rows, int C, float eps,
                    cudaStream_t s);
 // the same over x[r] = word[ids[r]] + pos[pos_ids[r]] + seg[seg_ids[r]] (bf16 tables [*, C], sum in fp32).  An id
-// outside its table reads nothing (the row sums the other tables) and sets *err to 1.
+// outside its table reads nothing (the row sums the other tables) and sets *err to 1.  drop (training): dropout on the
+// output, element (r, c) at flat index r * C + c of the mask.
 void embedding_layernorm_fwd(const int64_t* ids, const int64_t* pos_ids, const int64_t* seg_ids, const void* word,
                              int64_t n_word, const void* pos, int64_t n_pos, const void* seg, int64_t n_seg,
                              const float* gamma, const float* beta, void* y, int64_t rows, int C, float eps, int* err,
-                             cudaStream_t s);
+                             cudaStream_t s, const PhiloxArgs* drop = nullptr);
 // Quantising variants: also q e4m3 [rows, C] (contiguous, 8-byte aligned) and sa fp32 [ceil(C/128), rows] of the stored
 // bf16 y, bit for bit what quantize_e4m3_blocks (gemm.h) makes of y: s = max|y| / 448 per row and 128-column block (1
 // for an all-zero block), q = sat(y / s).
@@ -252,11 +271,12 @@ int layernorm_bwd_ctas(int64_t rows);
 void layernorm_bwd(const void* x, const void* dy, const float* gamma, void* dx, float* part, float* dgamma,
                    float* dbeta, int64_t rows, int C, float eps, cudaStream_t s);
 // Backward of embedding_layernorm_fwd: re-gathers the row sum and writes its gradient dE fp32 [rows, C] (the gradient of
-// each of the three gathered table rows), plus dgamma / dbeta as in layernorm_bwd.
+// each of the three gathered table rows), plus dgamma / dbeta as in layernorm_bwd.  drop: the forward's output dropout
+// (applied to dy as it is loaded).
 void embedding_layernorm_bwd(const int64_t* ids, const int64_t* pos_ids, const int64_t* seg_ids, const void* word,
                              int64_t n_word, const void* pos, int64_t n_pos, const void* seg, int64_t n_seg,
                              const void* dy, const float* gamma, float* dE, float* part, float* dgamma, float* dbeta,
-                             int64_t rows, int C, float eps, cudaStream_t s);
+                             int64_t rows, int C, float eps, cudaStream_t s, const PhiloxArgs* drop = nullptr);
 
 // ---- lstm.cu: bidirectional LSTM recurrence of the BiLSTM student (H = 128; layouts in lstm.cu's header) ----
 constexpr int kLstmHidden = 128;

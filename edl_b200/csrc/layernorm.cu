@@ -12,12 +12,16 @@
 // registers over the rows of its warp; a CTA sums its eight warps in warp order into one fp32 partial row, and a second
 // kernel adds the partials of all CTAs in CTA order: no atomics, bitwise reproducible.  The embedding variant (EMB)
 // re-gathers word + pos + seg the way the forward does and writes the row gradient dE in fp32.
+// Dropout on the embedding-LayerNorm output (training, DROP): the forward multiplies y by Z = keep * 1 / (1 - p) of the
+// mask of philox.cuh at flat index row * C + col before the bf16 store, and the backward applies the same Z to dy as
+// it loads it.  Plain LayerNorm has no dropout.
 // Budgets (ptxas -v, 256 threads): layernorm_bwd_kernel 159 registers, embedding variant 161, no spills; 32 KB static
 // shared memory for the partial sums.
 #include <cuda_fp8.h>
 
 #include "common.cuh"
 #include "kernels.h"
+#include "philox.cuh"
 
 namespace edl {
 namespace {
@@ -32,11 +36,22 @@ struct LnQuant {
   int64_t rows;
 };
 
-// x: this lane's chunks of the row (chunk c of the lane is columns (c * 32 + lane) * 8 ..), n8 = C / 8
-template <bool Q = false>
+// y[e] *= Z of the eight elements at flat mask index n .. n + 7 (n % 8 == 0)
+EDL_DEVICE void dropout8(const PhiloxKey& k, uint64_t n, float (&y)[8]) {
+  const uint4 w0 = philox_group(k, n >> 2), w1 = philox_group(k, (n >> 2) + 1);
+  const uint32_t w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+#pragma unroll
+  for (int e = 0; e < 8; ++e) y[e] = w[e] >= k.threshold ? y[e] * k.scale : 0.f;
+}
+
+// x: this lane's chunks of the row (chunk c of the lane is columns (c * 32 + lane) * 8 ..), n8 = C / 8.  DROP: dropout
+// on the stored y with the mask indices nrow + col.
+template <bool Q = false, bool DROP = false>
 EDL_DEVICE void ln_store(float (&x)[kLnChunks][8], int lane, int n8, int C, const float* __restrict__ gamma,
                          const float* __restrict__ beta, float eps, __nv_bfloat16* __restrict__ yrow,
-                         [[maybe_unused]] const LnQuant& qo = LnQuant{}) {
+                         [[maybe_unused]] const LnQuant& qo = LnQuant{}, [[maybe_unused]] const PhiloxKey& pk = {},
+                         [[maybe_unused]] uint64_t nrow = 0) {
+  static_assert(!(Q && DROP), "dropout: bf16 output only");
   float s = 0.f;
 #pragma unroll
   for (int c = 0; c < kLnChunks; ++c)
@@ -103,6 +118,7 @@ EDL_DEVICE void ln_store(float (&x)[kLnChunks][8], int lane, int n8, int C, cons
       float y[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) y[e] = fmaf((x[c][e] - mean) * rstd, g[e], bb[e]);
+      if constexpr (DROP) dropout8(pk, nrow + k * 8, y);
       st_vec(yrow + k * 8, pack8(y));
     }
   }
@@ -130,14 +146,14 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ 
   ln_store<Q>(v, lane, n8, C, gamma, beta, eps, y + r * C, LnQuant{q + r * C, sa + r, rows});
 }
 
-template <bool Q>
+template <bool Q, bool DROP = false>
 __global__ void __launch_bounds__(kLnWarps * 32)
 embedding_layernorm_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ pos_ids,
                            const int64_t* __restrict__ seg_ids, const __nv_bfloat16* __restrict__ word, int64_t n_word,
                            const __nv_bfloat16* __restrict__ pos, int64_t n_pos, const __nv_bfloat16* __restrict__ seg,
                            int64_t n_seg, const float* __restrict__ gamma, const float* __restrict__ beta,
                            __nv_bfloat16* __restrict__ y, int64_t rows, int C, float eps, int* err,
-                           uint8_t* __restrict__ q, float* __restrict__ sa) {
+                           uint8_t* __restrict__ q, float* __restrict__ sa, const PhiloxArgs drop) {
   const int lane = threadIdx.x & 31;
   const int64_t r = (int64_t)blockIdx.x * kLnWarps + (threadIdx.x >> 5);
   if (r >= rows) return;
@@ -170,7 +186,10 @@ embedding_layernorm_kernel(const int64_t* __restrict__ ids, const int64_t* __res
       }
     }
   }
-  ln_store<Q>(v, lane, n8, C, gamma, beta, eps, y + r * C, LnQuant{q + r * C, sa + r, rows});
+  if constexpr (DROP)
+    ln_store<Q, true>(v, lane, n8, C, gamma, beta, eps, y + r * C, LnQuant{}, philox_key(drop), (uint64_t)r * C);
+  else
+    ln_store<Q>(v, lane, n8, C, gamma, beta, eps, y + r * C, LnQuant{q + r * C, sa + r, rows});
 }
 
 constexpr int kLnBwdMaxCtas = 264;
@@ -218,14 +237,15 @@ EDL_DEVICE void ln_bwd_row(const __nv_bfloat16* __restrict__ x, const int64_t* _
   }
 }
 
-template <bool EMB>
+template <bool EMB, bool DROP = false>
 __global__ void __launch_bounds__(kLnWarps * 32)
 layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ x, const int64_t* __restrict__ ids,
                      const int64_t* __restrict__ pos_ids, const int64_t* __restrict__ seg_ids,
                      const __nv_bfloat16* __restrict__ word, int64_t n_word, const __nv_bfloat16* __restrict__ pos,
                      int64_t n_pos, const __nv_bfloat16* __restrict__ seg, int64_t n_seg,
                      const __nv_bfloat16* __restrict__ dy, const float* __restrict__ gamma, void* __restrict__ dx,
-                     float* __restrict__ part, int64_t rows, int C, float eps) {
+                     float* __restrict__ part, int64_t rows, int C, float eps, const PhiloxArgs drop) {
+  static_assert(EMB || !DROP, "dropout: embedding-LayerNorm only");
   __shared__ float red[kLnWarps][kLnMaxC];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int n8 = C / 8;
@@ -261,6 +281,7 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ x, const int64_t* __restr
       const int k = c * 32 + lane;
       if (k >= n8) continue;
       unpack8(ld_vec(dy + r * C + k * 8), d[c]);
+      if constexpr (DROP) dropout8(philox_key(drop), (uint64_t)r * C + k * 8, d[c]);
       const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma) + 2 * k), g1 = __ldg(reinterpret_cast<const float4*>(gamma) + 2 * k + 1);
       const float gm[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
 #pragma unroll
@@ -334,19 +355,20 @@ void layernorm_bwd(const void* x, const void* dy, const float* gamma, void* dx, 
   const int ctas = layernorm_bwd_ctas(rows);
   layernorm_bwd_kernel<false><<<ctas, kLnWarps * 32, 0, s>>>(
       reinterpret_cast<const __nv_bfloat16*>(x), nullptr, nullptr, nullptr, nullptr, 0, nullptr, 0, nullptr, 0,
-      reinterpret_cast<const __nv_bfloat16*>(dy), gamma, dx, part, rows, C, eps);
+      reinterpret_cast<const __nv_bfloat16*>(dy), gamma, dx, part, rows, C, eps, PhiloxArgs{});
   layernorm_bwd_reduce<<<(2 * C + 255) / 256, 256, 0, s>>>(part, ctas, C, dgamma, dbeta);
 }
 
 void embedding_layernorm_bwd(const int64_t* ids, const int64_t* pos_ids, const int64_t* seg_ids, const void* word,
                              int64_t n_word, const void* pos, int64_t n_pos, const void* seg, int64_t n_seg,
                              const void* dy, const float* gamma, float* dE, float* part, float* dgamma, float* dbeta,
-                             int64_t rows, int C, float eps, cudaStream_t s) {
+                             int64_t rows, int C, float eps, cudaStream_t s, const PhiloxArgs* drop) {
   const int ctas = layernorm_bwd_ctas(rows);
-  layernorm_bwd_kernel<true><<<ctas, kLnWarps * 32, 0, s>>>(
+  auto kern = drop != nullptr ? layernorm_bwd_kernel<true, true> : layernorm_bwd_kernel<true>;
+  kern<<<ctas, kLnWarps * 32, 0, s>>>(
       nullptr, ids, pos_ids, seg_ids, reinterpret_cast<const __nv_bfloat16*>(word), n_word,
       reinterpret_cast<const __nv_bfloat16*>(pos), n_pos, reinterpret_cast<const __nv_bfloat16*>(seg), n_seg,
-      reinterpret_cast<const __nv_bfloat16*>(dy), gamma, dE, part, rows, C, eps);
+      reinterpret_cast<const __nv_bfloat16*>(dy), gamma, dE, part, rows, C, eps, drop != nullptr ? *drop : PhiloxArgs{});
   layernorm_bwd_reduce<<<(2 * C + 255) / 256, 256, 0, s>>>(part, ctas, C, dgamma, dbeta);
 }
 
@@ -371,12 +393,14 @@ void layernorm_e4m3_fwd(const void* x, const float* gamma, const float* beta, vo
 void embedding_layernorm_fwd(const int64_t* ids, const int64_t* pos_ids, const int64_t* seg_ids, const void* word,
                              int64_t n_word, const void* pos, int64_t n_pos, const void* seg, int64_t n_seg,
                              const float* gamma, const float* beta, void* y, int64_t rows, int C, float eps, int* err,
-                             cudaStream_t s) {
+                             cudaStream_t s, const PhiloxArgs* drop) {
   if (rows <= 0) return;
-  embedding_layernorm_kernel<false><<<(unsigned)((rows + kLnWarps - 1) / kLnWarps), kLnWarps * 32, 0, s>>>(
+  auto kern = drop != nullptr ? embedding_layernorm_kernel<false, true> : embedding_layernorm_kernel<false>;
+  kern<<<(unsigned)((rows + kLnWarps - 1) / kLnWarps), kLnWarps * 32, 0, s>>>(
       ids, pos_ids, seg_ids, reinterpret_cast<const __nv_bfloat16*>(word), n_word,
       reinterpret_cast<const __nv_bfloat16*>(pos), n_pos, reinterpret_cast<const __nv_bfloat16*>(seg), n_seg, gamma,
-      beta, reinterpret_cast<__nv_bfloat16*>(y), rows, C, eps, err, nullptr, nullptr);
+      beta, reinterpret_cast<__nv_bfloat16*>(y), rows, C, eps, err, nullptr, nullptr,
+      drop != nullptr ? *drop : PhiloxArgs{});
 }
 
 void embedding_layernorm_e4m3_fwd(const int64_t* ids, const int64_t* pos_ids, const int64_t* seg_ids, const void* word,
@@ -387,7 +411,7 @@ void embedding_layernorm_e4m3_fwd(const int64_t* ids, const int64_t* pos_ids, co
   embedding_layernorm_kernel<true><<<(unsigned)((rows + kLnWarps - 1) / kLnWarps), kLnWarps * 32, 0, s>>>(
       ids, pos_ids, seg_ids, reinterpret_cast<const __nv_bfloat16*>(word), n_word,
       reinterpret_cast<const __nv_bfloat16*>(pos), n_pos, reinterpret_cast<const __nv_bfloat16*>(seg), n_seg, gamma,
-      beta, reinterpret_cast<__nv_bfloat16*>(y), rows, C, eps, err, reinterpret_cast<uint8_t*>(q), sa);
+      beta, reinterpret_cast<__nv_bfloat16*>(y), rows, C, eps, err, reinterpret_cast<uint8_t*>(q), sa, PhiloxArgs{});
 }
 
 }  // namespace edl

@@ -1,13 +1,51 @@
 // torch bindings for the Transformer encoder kernels (attention.cu, attention_bwd.cu, layernorm.cu and its quantising
-// variants).
+// variants, dropout.cu).
 #include <ATen/cuda/CUDAContext.h>
+#include <ATen/cuda/CUDAGeneratorImpl.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
+
+#include <cmath>
+#include <mutex>
 
 #include "kernels.h"
 
 namespace {
 using torch::Tensor;
+
+// One dropout site: 4 offset units of the default CUDA generator of `device` (graph-safe: under capture the kernels read
+// the seed and offset through the generator's device pointers), threshold floor(p * 2^32) and scale fp32(1 / (1 - p)).
+edl::PhiloxArgs dropout_draw(int64_t device, double p) {
+  TORCH_CHECK(p > 0.0 && p < 1.0, "dropout_draw: 0 < p < 1");
+  auto gen = at::get_generator_or_default<at::CUDAGeneratorImpl>(
+      std::nullopt, at::cuda::detail::getDefaultCUDAGenerator((c10::DeviceIndex)device));
+  at::PhiloxCudaState st;
+  {
+    std::lock_guard<std::mutex> lock(gen->mutex_);
+    st = gen->philox_cuda_state(4);
+  }
+  edl::PhiloxArgs a;
+  if (st.captured_) {
+    a.seed_ptr = st.seed_.ptr;
+    a.offset_ptr = st.offset_.ptr;
+    a.offset_intragraph = st.offset_intragraph_;
+  } else {
+    a.seed = st.seed_.val;
+    a.offset = st.offset_.val;
+  }
+  a.threshold = (uint32_t)std::floor(p * 4294967296.0);
+  a.scale = (float)(1.0 / (1.0 - p));
+  return a;
+}
+
+// y = Z o x, x / y bf16 CUDA tensors of one size (contiguous)
+void dropout_fwd(const Tensor& x, Tensor& y, const edl::PhiloxArgs& drop) {
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && x.is_contiguous() && y.is_cuda() &&
+              y.scalar_type() == at::kBFloat16 && y.is_contiguous() && y.numel() == x.numel() &&
+              y.device() == x.device(), "dropout: x, y contiguous bf16 CUDA tensors of one size");
+  c10::cuda::CUDAGuard guard(x.device());
+  edl::dropout_apply(x.data_ptr(), y.data_ptr(), x.numel(), drop, at::cuda::getCurrentCUDAStream().stream());
+}
 
 void check_bf16_2d(const Tensor& t, const char* name) {
   TORCH_CHECK(t.is_cuda() && t.dim() == 2 && t.scalar_type() == at::kBFloat16 && t.is_contiguous(), name,
@@ -16,7 +54,7 @@ void check_bf16_2d(const Tensor& t, const char* name) {
 
 // qkv [B * L, 3 * H * 64], mask uint8 [B, L] or None, out [B * L, H * 64]
 void attention_fwd(const Tensor& qkv, const c10::optional<Tensor>& mask, Tensor& out, int64_t B, int64_t L, int64_t H,
-                   const c10::optional<Tensor>& lse) {
+                   const c10::optional<Tensor>& lse, const edl::PhiloxArgs* drop) {
   check_bf16_2d(qkv, "qkv");
   check_bf16_2d(out, "out");
   TORCH_CHECK(qkv.size(0) == B * L && qkv.size(1) == 3 * H * 64, "qkv must be [B * L, 3 * H * 64]");
@@ -36,13 +74,14 @@ void attention_fwd(const Tensor& qkv, const c10::optional<Tensor>& mask, Tensor&
   }
   c10::cuda::CUDAGuard guard(qkv.device());
   const char* err = edl::attention_fwd(qkv.data_ptr(), mp, out.data_ptr(), (int)B, (int)L, (int)H,
-                                       at::cuda::getCurrentCUDAStream().stream(), lp);
+                                       at::cuda::getCurrentCUDAStream().stream(), lp, drop);
   TORCH_CHECK(err == nullptr, "edl attention_fwd failed: ", err);
 }
 
 // dqkv [B * L, 3 * H * 64] from qkv, the forward's out and lse [B, H, L], dout [B * L, H * 64]; delta fp32 [B, H, L]
 void attention_bwd(const Tensor& qkv, const c10::optional<Tensor>& mask, const Tensor& out, const Tensor& lse,
-                   const Tensor& dout, Tensor& dqkv, Tensor& delta, int64_t B, int64_t L, int64_t H) {
+                   const Tensor& dout, Tensor& dqkv, Tensor& delta, int64_t B, int64_t L, int64_t H,
+                   const edl::PhiloxArgs* drop) {
   for (const Tensor* t : {&qkv, &out, &dout, static_cast<const Tensor*>(&dqkv)}) check_bf16_2d(*t, "attention_bwd operand");
   TORCH_CHECK(qkv.size(0) == B * L && qkv.size(1) == 3 * H * 64 && dqkv.sizes() == qkv.sizes(),
               "qkv / dqkv must be [B * L, 3 * H * 64]");
@@ -61,7 +100,7 @@ void attention_bwd(const Tensor& qkv, const c10::optional<Tensor>& mask, const T
   c10::cuda::CUDAGuard guard(qkv.device());
   const char* err = edl::attention_bwd(qkv.data_ptr(), mp, out.data_ptr(), lse.data_ptr<float>(), dout.data_ptr(),
                                        dqkv.data_ptr(), delta.data_ptr<float>(), (int)B, (int)L, (int)H,
-                                       at::cuda::getCurrentCUDAStream().stream());
+                                       at::cuda::getCurrentCUDAStream().stream(), drop);
   TORCH_CHECK(err == nullptr, "edl attention_bwd failed: ", err);
 }
 
@@ -110,7 +149,7 @@ void layernorm_fwd(const Tensor& x, const Tensor& gamma, const Tensor& beta, Ten
 
 void embedding_layernorm_fwd(const Tensor& ids, const Tensor& pos_ids, const Tensor& seg_ids, const Tensor& word,
                              const Tensor& pos, const Tensor& seg, const Tensor& gamma, const Tensor& beta, Tensor& y,
-                             double eps, Tensor& err) {
+                             double eps, Tensor& err, const edl::PhiloxArgs* drop) {
   const int64_t rows = ids.numel();
   for (const Tensor* t : {&ids, &pos_ids, &seg_ids})
     TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kLong && t->is_contiguous() && t->numel() == rows,
@@ -128,7 +167,7 @@ void embedding_layernorm_fwd(const Tensor& ids, const Tensor& pos_ids, const Ten
   edl::embedding_layernorm_fwd(ids.data_ptr<int64_t>(), pos_ids.data_ptr<int64_t>(), seg_ids.data_ptr<int64_t>(),
                                word.data_ptr(), word.size(0), pos.data_ptr(), pos.size(0), seg.data_ptr(), seg.size(0),
                                gamma.data_ptr<float>(), beta.data_ptr<float>(), y.data_ptr(), rows, (int)C, (float)eps,
-                               err.data_ptr<int>(), at::cuda::getCurrentCUDAStream().stream());
+                               err.data_ptr<int>(), at::cuda::getCurrentCUDAStream().stream(), drop);
 }
 
 // x, dy, dx bf16 [rows, C]; part fp32 [layernorm_bwd_ctas(rows) * 2 * C]; dgamma / dbeta fp32 [C]
@@ -151,7 +190,7 @@ void layernorm_bwd(const Tensor& x, const Tensor& dy, const Tensor& gamma, Tenso
 // dE fp32 [rows, C]: the gradient of the gathered row sum of embedding_layernorm_fwd
 void embedding_layernorm_bwd(const Tensor& ids, const Tensor& pos_ids, const Tensor& seg_ids, const Tensor& word,
                              const Tensor& pos, const Tensor& seg, const Tensor& dy, const Tensor& gamma, Tensor& dE,
-                             Tensor& part, Tensor& dgamma, Tensor& dbeta, double eps) {
+                             Tensor& part, Tensor& dgamma, Tensor& dbeta, double eps, const edl::PhiloxArgs* drop) {
   const int64_t rows = ids.numel();
   for (const Tensor* t : {&ids, &pos_ids, &seg_ids})
     TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kLong && t->is_contiguous() && t->numel() == rows,
@@ -171,7 +210,7 @@ void embedding_layernorm_bwd(const Tensor& ids, const Tensor& pos_ids, const Ten
                                word.data_ptr(), word.size(0), pos.data_ptr(), pos.size(0), seg.data_ptr(), seg.size(0),
                                dy.data_ptr(), gamma.data_ptr<float>(), dE.data_ptr<float>(), part.data_ptr<float>(),
                                dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), rows, (int)C, (float)eps,
-                               at::cuda::getCurrentCUDAStream().stream());
+                               at::cuda::getCurrentCUDAStream().stream(), drop);
 }
 
 // q uint8 [rows, C] (contiguous), sa fp32 [ceil(C/128), rows]: the block quantisation of the stored y
@@ -226,6 +265,15 @@ void embedding_layernorm_e4m3_fwd(const Tensor& ids, const Tensor& pos_ids, cons
 }  // namespace
 
 void register_transformer_bindings(pybind11::module_& m) {
+  // a drawn dropout site; seed / offset are the values the kernels use (0 when captured: then read at run time)
+  pybind11::class_<edl::PhiloxArgs>(m, "PhiloxArgs")
+      .def_readonly("seed", &edl::PhiloxArgs::seed)
+      .def_readonly("offset", &edl::PhiloxArgs::offset)
+      .def_readonly("threshold", &edl::PhiloxArgs::threshold)
+      .def_readonly("scale", &edl::PhiloxArgs::scale)
+      .def_property_readonly("captured", [](const edl::PhiloxArgs& a) { return a.seed_ptr != nullptr; });
+  m.def("dropout_draw", &dropout_draw);
+  m.def("dropout_fwd", &dropout_fwd);
   m.def("attention_fwd", &attention_fwd);
   m.def("attention_supported", &edl::attention_supported);
   m.def("attention_varlen_fwd", &attention_varlen_fwd);

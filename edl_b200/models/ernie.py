@@ -317,12 +317,30 @@ class ErnieStudent(ErnieEncoder):
     fp32 master copies; on CUDA each forward casts the matrices to bf16 and runs the training kernels of
     ops/transformer.py (attention and its backward, LayerNorm and embedding-LayerNorm with their backward, FFN1 with
     the GELU training epilogue and FFN2's gelu'-epilogue dgrad, residual gradients fused into the dgrad GEMMs).  On CPU
-    the forward is the encoder's float32 reference under torch autograd.  Dropout is not implemented (p = 0).
+    the forward is the encoder's float32 reference under torch autograd.
+
+    Dropout (keyword-only ``hidden_dropout`` / ``attention_dropout``, default 0; only while ``self.training``) sits
+    where BERT puts it.  Each site draws one (seed, offset) pair of 4 offset units from the default CUDA generator of
+    the device (``ops.transformer.dropout_keep_reference`` is the mask), in this order per forward:
+      1. the embedding-LayerNorm output (hidden), index row * C + col, in the embedding-LayerNorm kernel;
+      then per layer
+      2. the attention probabilities (attention), index ((b H + h) L + i) L + j, in the attention kernels;
+      3. the attention output branch before its residual add (hidden), index row * C + col, in the output projection's
+         GEMM epilogue;
+      4. the FFN output branch before its residual add (hidden), index row * C + col, in FFN2's GEMM epilogue;
+      and last
+      5. the pooled [CLS] features before the classifier (hidden), index b * C + col, through ``ops.dropout``.
+    A step thus advances the generator offset by 4 * (2 + 3 * layers).  A site with p = 0 draws nothing and runs the
+    p = 0 kernels; on CPU the sites are ``F.dropout``.  Dropout adds no parameters or buffers.
 
     ``forward`` also takes the token ids alone: positions are then 0 .. L - 1, segments 0 and the mask ``ids != 0``."""
 
-    def __init__(self, *args, **kwargs):
+    def __init__(self, *args, hidden_dropout=0.0, attention_dropout=0.0, **kwargs):
         super().__init__(*args, **kwargs)
+        for p in (hidden_dropout, attention_dropout):
+            if not 0.0 <= float(p) < 1.0:
+                raise ValueError("ErnieStudent: dropout probabilities must satisfy 0 <= p < 1, got %r" % p)
+        self.hidden_dropout, self.attention_dropout = float(hidden_dropout), float(attention_dropout)
         self.requires_grad_(True)
 
     def enable_fp8(self, scaling="block"):
@@ -337,24 +355,44 @@ class ErnieStudent(ErnieEncoder):
         seg = torch.zeros_like(ids) if segment_ids is None else segment_ids.reshape(b, l).long()
         keep = (ids != 0) if input_mask is None else (input_mask.reshape(b, l) != 0)
         c = self.hidden
+        hd, ad = (self.hidden_dropout, self.attention_dropout) if self.training else (0.0, 0.0)
         if not self.word_emb.is_cuda:
+            if hd > 0.0 or ad > 0.0:
+                return self._forward_dropout_cpu(ids, pos, seg, keep, hd, ad)
             return self._forward_reference(ids, pos, seg, lambda qkv: ops.attention(qkv, keep, b, l, self.heads,
                                                                                     self.head_dim),
                                            lambda x: x.view(b, l, c)[:, 0])
         mask = keep.to(torch.uint8).contiguous()
         x = ops.embedding_layernorm_trainable(ids, pos, seg, self.word_emb, self.pos_emb, self.seg_emb, self.emb_ln_g,
-                                              self.emb_ln_b, self.eps)
+                                              self.emb_ln_b, self.eps, dropout_p=hd)
         for lyr in self.layers:
-            h = ops.attention_block(x, lyr.qkv_w, lyr.qkv_b, lyr.out_w, lyr.out_b, mask, b, l, self.heads)
+            h = ops.attention_block(x, lyr.qkv_w, lyr.qkv_b, lyr.out_w, lyr.out_b, mask, b, l, self.heads,
+                                    attn_dropout=ad, hidden_dropout=hd)
             x = ops.layer_norm_trainable(h, lyr.ln1_g, lyr.ln1_b, self.eps)
-            h = ops.gelu_ffn(x, lyr.ffn1_w, lyr.ffn1_b, lyr.ffn2_w, lyr.ffn2_b)
+            h = ops.gelu_ffn(x, lyr.ffn1_w, lyr.ffn1_b, lyr.ffn2_w, lyr.ffn2_b, dropout_p=hd)
             x = ops.layer_norm_trainable(h, lyr.ln2_g, lyr.ln2_b, self.eps)
         bf = torch.bfloat16
         pooled = torch.tanh(ops.linear_bf16(x.view(b, l, c)[:, 0], self.pool_w.to(bf), self.pool_b))
+        pooled = ops.dropout(pooled, hd)
         n = self.num_labels
         pad = max(CLS_PAD, -(-n // CLS_PAD) * CLS_PAD) - n          # TMA-describable classifier rows, as the encoder
         logits = ops.linear_bf16(pooled, F.pad(self.cls_w, (0, 0, 0, pad)).to(bf), F.pad(self.cls_b, (0, pad)))
         return logits[:, :n].float()
+
+
+    def _forward_dropout_cpu(self, ids, pos, seg, keep, hd, ad):
+        """The float32 training forward on CPU with dropout at the documented sites (F.dropout masks)."""
+        b, l = ids.shape
+        x = ops.embedding_layernorm_trainable(ids, pos, seg, self.word_emb, self.pos_emb, self.seg_emb, self.emb_ln_g,
+                                              self.emb_ln_b, self.eps, dropout_p=hd)
+        for lyr in self.layers:
+            h = ops.attention_block(x, lyr.qkv_w, lyr.qkv_b, lyr.out_w, lyr.out_b, keep, b, l, self.heads,
+                                    attn_dropout=ad, hidden_dropout=hd)
+            x = ops.layer_norm_trainable(h, lyr.ln1_g, lyr.ln1_b, self.eps)
+            h = ops.gelu_ffn(x, lyr.ffn1_w, lyr.ffn1_b, lyr.ffn2_w, lyr.ffn2_b, dropout_p=hd)
+            x = ops.layer_norm_trainable(h, lyr.ln2_g, lyr.ln2_b, self.eps)
+        pooled = ops.dropout(torch.tanh(F.linear(x.view(b, l, self.hidden)[:, 0], self.pool_w, self.pool_b)), hd)
+        return F.linear(pooled, self.cls_w, self.cls_b)
 
 
 def ernie_base(num_labels=2):
@@ -362,9 +400,10 @@ def ernie_base(num_labels=2):
     return ErnieEncoder(18000, 768, 12, 12, 3072, 513, 2, num_labels)
 
 
-def ernie_student(num_labels=2):
-    """The Transformer student: the teacher's vocabulary (18000) and feeds, hidden 384, 4 layers, 6 heads, FFN 1536."""
-    return ErnieStudent(18000, 384, 4, 6, 1536, 513, 2, num_labels)
+def ernie_student(num_labels=2, dropout=0.0):
+    """The Transformer student: the teacher's vocabulary (18000) and feeds, hidden 384, 4 layers, 6 heads, FFN 1536;
+    ``dropout`` sets both its hidden and attention dropout (BERT trains with 0.1)."""
+    return ErnieStudent(18000, 384, 4, 6, 1536, 513, 2, num_labels, hidden_dropout=dropout, attention_dropout=dropout)
 
 
 def ernie_tiny(num_labels=2):

@@ -100,8 +100,8 @@ from .transformer import (attention, attention_supported, layer_norm, layer_norm
                           attention_varlen_supported, layer_norm_e4m3, layer_norm_e4m3_supported,
                           embedding_layernorm_e4m3, embedding_layernorm_e4m3_supported)
 from .transformer import (attention_block, attention_trainable, embedding_layernorm_trainable, gelu_ffn,  # noqa: E402
-                          layer_norm_trainable)
-from .gemm import gemm_bf16_gelu_grad, gemm_bf16_gelu_train  # noqa: E402
+                          layer_norm_trainable, dropout, dropout_keep_reference)
+from .gemm import gemm_bf16_gelu_grad, gemm_bf16_gelu_train, gemm_bf16_residual_dropout  # noqa: E402
 from .rnn import lstm, lstm_supported  # noqa: E402
 
 __all__ = [

@@ -420,6 +420,27 @@ def gemm_bf16_gelu_grad(dy, w, u):
     return ((dy.float() @ w.float()) * gelu_grad_reference(u)).to(dy.dtype)
 
 
+def gemm_bf16_residual_dropout(x, w, bias, add, drop):
+    """A residual branch with dropout, D = add + Z o (x @ w^T + bias) in fp32, stored bf16: x [M, K], w [N, K] bf16,
+    ``add`` [M, N] bf16 (the residual), ``drop`` a drawn dropout site (``ops.transformer._draw``) whose mask Z is taken
+    at flat index row * N + col.  A dropped element stores ``add`` bitwise.  One persistent GEMM; the mask is applied
+    in its epilogue before the addend."""
+    from . import native, count_launch, count_fallback
+    from .transformer import _fallback_z
+
+    m, n = x.shape[0], w.shape[0]
+    if x.is_cuda and n % 8 == 0 and _gelu_gemm_ok(x, w, add):
+        d = torch.empty((m, n), device=x.device, dtype=torch.bfloat16)
+        native().gemm_bf16_residual_dropout(x, w, d, bias.float().contiguous() if bias is not None else None, add, drop)
+        count_launch()
+        return d
+    if x.is_cuda:
+        count_fallback("gemm_bf16_residual_dropout: no kernel for %s x %s: fp32 matmul on the library"
+                       % (tuple(x.shape), tuple(w.shape)))
+    v = x.float() @ w.float().t() + (bias.float() if bias is not None else 0.0)
+    return (add.float() + _fallback_z(drop, (m, n), x.device) * v).to(add.dtype)
+
+
 # EDL_PAIR_WGRAD=0: the library's weight gradient for the 32-channel stem convolutions as well
 PAIR_WGRAD = __import__("os").environ.get("EDL_PAIR_WGRAD", "1") == "1"
 

@@ -6,7 +6,10 @@ kernel cannot take (head dim other than 64, sequences longer than 512, a hidden 
 runs the same reference math on the library through ``count_fallback``.
 
 ``layer_norm_e4m3`` and ``embedding_layernorm_e4m3`` also return the block-scaled e4m3 copy of their bf16 output
-(``ops.fp8.quantize_e4m3_blocks``), written by the same kernel, for the FP8 teacher's next GEMM."""
+(``ops.fp8.quantize_e4m3_blocks``), written by the same kernel, for the FP8 teacher's next GEMM.
+
+Dropout (training): one mask definition for every kernel, the float32 fallback and the tests, see
+``dropout_keep_reference``."""
 from __future__ import annotations
 
 import torch
@@ -18,10 +21,130 @@ def _count(reason):
     count_fallback(reason)
 
 
+# ------------------------------------------------------------------------------------------------------------ dropout
+# A dropout site draws one (seed, offset) pair from the default CUDA generator of its device, consuming 4 offset units
+# (so torch.manual_seed governs the masks, and a CUDA graph draws fresh ones on every replay).  Element n of the site's
+# flat index space is kept iff word n % 4 of Philox4x32-10 with key (seed_lo, seed_hi) and counter
+# (floor(n / 4)_lo, floor(n / 4)_hi, offset_lo, offset_hi) is >= floor(p * 2^32); kept elements are scaled by
+# fp32(1 / (1 - p)).  The kernels evaluate the same rule (csrc/philox.cuh).  On CPU the sites use F.dropout.
+_M32 = 0xFFFFFFFF
+_PHILOX_M = (0xD2511F53, 0xCD9E8D57)
+_PHILOX_W = (0x9E3779B9, 0xBB67AE85)
+
+
+def _check_p(p):
+    p = float(p)
+    if not 0.0 <= p < 1.0:
+        raise ValueError("dropout probability must satisfy 0 <= p < 1, got %r" % p)
+    return p
+
+
+def _mulhilo(m, c):
+    """(hi, lo) 32-bit words of the 64-bit product m * c (c int64 in [0, 2^32)) without leaving int64."""
+    a, b = c * (m & 0xFFFF), c * (m >> 16)            # < 2^48 each
+    return (b + (a >> 16)) >> 16, (a + ((b & 0xFFFF) << 16)) & _M32
+
+
+def philox4x32_10(key, ctr):
+    """Philox4x32-10 of int64 tensors holding 32-bit words: key (k0, k1), counter (c0, c1, c2, c3) -> four words."""
+    k0, k1 = key
+    c0, c1, c2, c3 = ctr
+    for r in range(10):
+        if r:
+            k0, k1 = (k0 + _PHILOX_W[0]) & _M32, (k1 + _PHILOX_W[1]) & _M32
+        hi0, lo0 = _mulhilo(_PHILOX_M[0], c0)
+        hi1, lo1 = _mulhilo(_PHILOX_M[1], c2)
+        c0, c1, c2, c3 = hi1 ^ c1 ^ k0, lo1, hi0 ^ c3 ^ k1, lo0
+    return c0, c1, c2, c3
+
+
+def _keep(seed, offset, index, threshold):
+    index = index.to(torch.int64)
+    g = index >> 2
+    w = lambda v: torch.full_like(index, v & _M32)   # noqa: E731
+    words = philox4x32_10((w(seed), w(seed >> 32)), (g & _M32, g >> 32, w(offset), w(offset >> 32)))
+    word = torch.stack(words, -1).gather(-1, (index & 3).unsqueeze(-1)).squeeze(-1)
+    return word >= threshold
+
+
+def dropout_keep_reference(seed, offset, index, p):
+    """The keep mask (bool, index's shape and device) of a dropout site with generator state (seed, offset) at the flat
+    element indices ``index`` (int64 tensor), in torch int64 arithmetic on any device.  The single host-side statement
+    of the rule the kernels use; the scale of a kept element is ``fp32(1 / (1 - p))``."""
+    p = _check_p(p)
+    return _keep(int(seed), int(offset), index, int(p * 4294967296.0))
+
+
+def _draw(device, p):
+    """Draw one dropout site (p > 0) from the default CUDA generator of ``device``."""
+    from . import native
+
+    return native().dropout_draw(device.index if device.index is not None else torch.cuda.current_device(), p)
+
+
+def _fallback_z(drop, shape, device):
+    """Z = keep * scale (float32, ``shape``) of a drawn site over the flat indices of ``shape``: the kernels' mask for
+    the float32 fallback.  Needs the host values of the draw, so it cannot run under CUDA-graph capture."""
+    if drop.captured:
+        raise RuntimeError("dropout: the float32 fallback cannot be captured in a CUDA graph")
+    n = 1
+    for d in shape:
+        n *= d
+    keep = _keep(drop.seed, drop.offset, torch.arange(n, device=device), drop.threshold)
+    return (keep.float() * drop.scale).view(shape)
+
+
+def _site_z(t, p, shape):
+    """Z of a dropout site on the float32 reference path: None at p = 0, F.dropout's mask on CPU, the kernels' mask
+    (one generator draw) on CUDA."""
+    if p == 0.0:
+        return None
+    if not t.is_cuda:
+        return torch.nn.functional.dropout(torch.ones(shape, dtype=torch.float32), p, True)
+    return _fallback_z(_draw(t.device, p), shape, t.device)
+
+
+def _dropout_apply(x, drop):
+    from . import native, count_launch
+
+    y = torch.empty_like(x)
+    native().dropout_fwd(x, y, drop)
+    count_launch()
+    return y
+
+
+class _DropoutFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, drop):
+        ctx.drop = drop
+        return _dropout_apply(x, drop)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return _dropout_apply(dy.contiguous(), ctx.drop), None
+
+
+def dropout(x, p, training=True):
+    """Inverted dropout: zero each element with probability ``p`` and scale the others by 1 / (1 - p).  Identity when
+    not ``training`` or at p = 0 (no generator draw).  On CUDA, bf16 runs dropout.cu with the package's mask over the
+    flat index of ``x`` (one draw of 4 offset units); other dtypes take the same mask in float32 math through
+    ``count_fallback``.  On CPU it is ``F.dropout``."""
+    p = _check_p(p)
+    if not training or p == 0.0:
+        return x
+    if not x.is_cuda:
+        return torch.nn.functional.dropout(x, p, True)
+    if x.dtype == torch.bfloat16:
+        return _DropoutFn.apply(x.contiguous(), _draw(x.device, p))
+    _count("dropout: no kernel for %s: float32 math on the library" % x.dtype)
+    return (x.float() * _site_z(x, p, tuple(x.shape))).to(x.dtype)
+
+
 # ---------------------------------------------------------------------------------------------------------- attention
-def attention_reference(qkv, mask, batch, seq_len, heads, head_dim=64):
+def attention_reference(qkv, mask, batch, seq_len, heads, head_dim=64, drop_z=None):
     """Float32 math of ``attention``: softmax(Q K^T / sqrt(head_dim) with masked keys at -inf) V; a query row without a
-    valid key is 0.  Returns [B * L, H * head_dim] in qkv's dtype."""
+    valid key is 0.  ``drop_z`` [B, H, L, L]: dropout (keep * scale) on the probabilities.  Returns [B * L, H * head_dim]
+    in qkv's dtype."""
     x = qkv.float().view(batch, seq_len, 3, heads, head_dim)
     q, k, v = (x[:, :, i].transpose(1, 2) for i in range(3))           # [B, H, L, d]
     s = (q @ k.transpose(-1, -2)) / head_dim ** 0.5
@@ -31,6 +154,8 @@ def attention_reference(qkv, mask, batch, seq_len, heads, head_dim=64):
     mx = s.amax(-1, keepdim=True)
     p = torch.exp(s - torch.where(torch.isinf(mx), torch.zeros_like(mx), mx))
     den = p.sum(-1, keepdim=True)
+    if drop_z is not None:
+        p = p * drop_z
     o = (p @ v) / torch.where(den > 0, den, torch.ones_like(den))
     return o.transpose(1, 2).reshape(batch * seq_len, heads * head_dim).to(qkv.dtype)
 
@@ -60,7 +185,7 @@ def attention(qkv, mask, batch, seq_len, heads, head_dim=64, out=None):
     m = None
     if mask is not None:
         m = mask if (mask.dtype == torch.uint8 and mask.is_contiguous()) else (mask != 0).to(torch.uint8).contiguous()
-    native().attention_fwd(qkv, m, out, batch, seq_len, heads, None)
+    native().attention_fwd(qkv, m, out, batch, seq_len, heads, None, None)
     count_launch()
     return out
 
@@ -181,20 +306,24 @@ def embedding_layernorm(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps=
     Out-of-range ids raise IndexError.  On CUDA the kernel never reads outside a table; it raises a device flag that is
     checked after the launch, except while a CUDA graph is being captured (a replay cannot raise: such a row is the
     LayerNorm of the embeddings whose ids are in range)."""
-    from . import native, count_launch
-
     if not word.is_cuda:
         return embedding_layernorm_reference(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps)
     if not embedding_layernorm_supported(word, pos, seg):
         _count("embedding_layernorm: no kernel for width %d %s: float32 math on the library" % (word.shape[1], word.dtype))
         return embedding_layernorm_reference(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps)
+    return _embedding_layernorm_kernel(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps, out, None)
+
+
+def _embedding_layernorm_kernel(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps, out, drop):
+    from . import native, count_launch
+
     rows = ids.numel()
     if out is None:
         out = torch.empty((rows, word.shape[1]), device=word.device, dtype=torch.bfloat16)
     err = torch.zeros(1, dtype=torch.int32, device=word.device)
     ids, pos_ids, seg_ids = (t.reshape(-1).to(word.device, torch.int64).contiguous() for t in (ids, pos_ids, seg_ids))
     native().embedding_layernorm_fwd(ids, pos_ids, seg_ids, word, pos, seg, gamma.float().contiguous(),
-                                     beta.float().contiguous(), out, float(eps), err)
+                                     beta.float().contiguous(), out, float(eps), err, drop)
     count_launch()
     if not torch.cuda.is_current_stream_capturing() and int(err.item()) != 0:
         for t, tab, what in ((ids, word, "input id"), (pos_ids, pos, "position id"), (seg_ids, seg, "segment id")):
@@ -270,8 +399,10 @@ def embedding_layernorm_e4m3(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta,
 # master parameters and casts the matrices to bf16 at every forward.  On CUDA the forward and backward run on the
 # package's kernels (attention.cu / attention_bwd.cu, layernorm.cu, the persistent GEMM with its GELU epilogues); on CPU,
 # and for shapes the kernels do not take (counted through ``count_fallback`` on CUDA), the float32 references run under
-# torch autograd.  Dropout is not implemented: the student trains with p = 0.  Nothing reads back to the host, so a
-# whole training step can be captured in a CUDA graph.
+# torch autograd.  Dropout (the ``*_dropout`` / ``dropout_p`` arguments, default 0): the attention probabilities in the
+# attention kernels, the two residual branches in the output-projection / FFN2 GEMM epilogues (D = x + Z o branch) and
+# the embedding-LayerNorm output in its kernel; each backward regenerates its mask.  At p = 0 nothing is drawn and the
+# p = 0 kernels run.  Nothing reads back to the host, so a whole training step can be captured in a CUDA graph.
 def _needs_grad(*ts):
     return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
 
@@ -306,25 +437,27 @@ def attention_train_supported(x, batch, seq_len, heads, head_dim=64) -> bool:
             and native().attention_supported(batch, seq_len, heads, head_dim))
 
 
-def attention_forward_saved(qkv, mask, batch, seq_len, heads):
-    """The kernel forward with the statistics the backward needs: (out bf16 [B * L, H * 64], lse fp32 [B, H, L])."""
+def attention_forward_saved(qkv, mask, batch, seq_len, heads, drop=None):
+    """The kernel forward with the statistics the backward needs: (out bf16 [B * L, H * 64], lse fp32 [B, H, L]).
+    ``drop``: a drawn dropout site (``_draw``) for the probabilities, element (b, h, i, j) at ((b H + h) L + i) L + j;
+    lse is that of the undropped softmax."""
     from . import native, count_launch
 
     out = torch.empty((batch * seq_len, heads * 64), device=qkv.device, dtype=torch.bfloat16)
     lse = torch.empty((batch, heads, seq_len), device=qkv.device, dtype=torch.float32)
-    native().attention_fwd(qkv, mask, out, batch, seq_len, heads, lse)
+    native().attention_fwd(qkv, mask, out, batch, seq_len, heads, lse, drop)
     count_launch()
     return out, lse
 
 
-def attention_backward(qkv, mask, out, lse, dout, batch, seq_len, heads):
+def attention_backward(qkv, mask, out, lse, dout, batch, seq_len, heads, drop=None):
     """dqkv bf16 [B * L, 3 * H * 64] (dQ | dK | dV in qkv's layout) of ``attention``, from the forward's ``out`` and
-    ``lse`` (``attention_forward_saved``) and the output gradient ``dout``."""
+    ``lse`` (``attention_forward_saved``, with the same ``drop``) and the output gradient ``dout``."""
     from . import native, count_launch
 
     dqkv = torch.empty_like(qkv)
     delta = torch.empty((batch, heads, seq_len), device=qkv.device, dtype=torch.float32)
-    native().attention_bwd(qkv, mask, out, lse, _bf16(dout).contiguous(), dqkv, delta, batch, seq_len, heads)
+    native().attention_bwd(qkv, mask, out, lse, _bf16(dout).contiguous(), dqkv, delta, batch, seq_len, heads, drop)
     count_launch(3)
     return dqkv
 
@@ -337,45 +470,56 @@ def _mask_u8(mask, device):
 
 class _AttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, mask, batch, seq_len, heads):
+    def forward(ctx, qkv, mask, batch, seq_len, heads, drop):
         qkv = _bf16(qkv).contiguous()
-        out, lse = attention_forward_saved(qkv, mask, batch, seq_len, heads)
+        out, lse = attention_forward_saved(qkv, mask, batch, seq_len, heads, drop)
         ctx.save_for_backward(qkv, mask, out, lse)
-        ctx.shape = (batch, seq_len, heads)
+        ctx.shape, ctx.drop = (batch, seq_len, heads), drop
         return out
 
     @staticmethod
     def backward(ctx, dout):
         qkv, mask, out, lse = ctx.saved_tensors
-        return attention_backward(qkv, mask, out, lse, dout, *ctx.shape), None, None, None, None
+        return attention_backward(qkv, mask, out, lse, dout, *ctx.shape, ctx.drop), None, None, None, None, None
 
 
-def attention_trainable(qkv, mask, batch, seq_len, heads, head_dim=64):
-    """``attention`` with a gradient: the kernel path saves lse and runs attention_bwd.cu in the backward."""
+def attention_trainable(qkv, mask, batch, seq_len, heads, head_dim=64, dropout_p=0.0):
+    """``attention`` with a gradient: the kernel path saves lse and runs attention_bwd.cu in the backward.
+    ``dropout_p``: dropout on the attention probabilities (one site, index ((b H + h) L + i) L + j)."""
+    p = _check_p(dropout_p)
     if qkv.is_cuda and attention_supported(_bf16(qkv).contiguous(), batch, seq_len, heads, head_dim):
-        return _AttentionFn.apply(qkv, _mask_u8(mask, qkv.device), batch, seq_len, heads)
+        return _AttentionFn.apply(qkv, _mask_u8(mask, qkv.device), batch, seq_len, heads,
+                                  _draw(qkv.device, p) if p > 0.0 else None)
     if qkv.is_cuda:
         _count("attention: no training kernel for B %d, L %d, H %d, head dim %d: float32 math on the library"
                % (batch, seq_len, heads, head_dim))
-    return attention_reference(qkv.float(), mask, batch, seq_len, heads, head_dim)
+    z = _site_z(qkv, p, (batch, heads, seq_len, seq_len))
+    return attention_reference(qkv.float(), mask, batch, seq_len, heads, head_dim, z)
 
 
 class _AttentionBlockFn(torch.autograd.Function):
     """h = attention(x W_qkv^T + b_qkv) W_o^T + b_o + x, the attention half of a post-LN encoder layer before its
     LayerNorm.  Backward: dctx = dh W_o, dqkv by attention_bwd.cu, and dx = dqkv W_qkv + dh as ONE dgrad GEMM with the
-    residual gradient as its fused addend; dW_qkv and dW_o through ``_wgrad``."""
+    residual gradient as its fused addend; dW_qkv and dW_o through ``_wgrad``.
+
+    ``drops`` = (attention-probability site, output-branch site), each None at p = 0.  With the branch dropout the output
+    projection's epilogue stores x + Z o (o W_o^T + b_o); the backward forms dh_b = Z o dh (dropout.cu) for dctx, dW_o
+    and db_o, while the residual still receives dh."""
 
     @staticmethod
-    def forward(ctx, x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, sinks):
-        from .gemm import gemm_bf16
+    def forward(ctx, x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, sinks, drops):
+        from .gemm import gemm_bf16, gemm_bf16_residual_dropout
 
         x = _bf16(x).contiguous()
         wq, wo = _bf16(qkv_w).contiguous(), _bf16(out_w).contiguous()
         qkv = gemm_bf16(x, wq, col_shift=qkv_b.float())
-        o, lse = attention_forward_saved(qkv, mask, batch, seq_len, heads)
-        h = gemm_bf16(o, wo, col_shift=out_b.float(), add=x)
+        o, lse = attention_forward_saved(qkv, mask, batch, seq_len, heads, drops[0])
+        if drops[1] is None:
+            h = gemm_bf16(o, wo, col_shift=out_b.float(), add=x)
+        else:
+            h = gemm_bf16_residual_dropout(o, wo, out_b, x, drops[1])
         ctx.save_for_backward(x, wq, wo, qkv, o, lse, mask, qkv_w, qkv_b, out_w, out_b)
-        ctx.shape, ctx.sinks = (batch, seq_len, heads), sinks
+        ctx.shape, ctx.sinks, ctx.drops = (batch, seq_len, heads), sinks, drops
         return h
 
     @staticmethod
@@ -384,8 +528,9 @@ class _AttentionBlockFn(torch.autograd.Function):
 
         x, wq, wo, qkv, o, lse, mask, qkv_w, qkv_b, out_w, out_b = ctx.saved_tensors
         dh = _bf16(dh).contiguous()
-        dctx = gemm_bf16(dh, wo, b_mn_major=True)
-        dqkv = attention_backward(qkv, mask, o, lse, dctx, *ctx.shape)
+        dhb = dh if ctx.drops[1] is None else _dropout_apply(dh, ctx.drops[1])
+        dctx = gemm_bf16(dhb, wo, b_mn_major=True)
+        dqkv = attention_backward(qkv, mask, o, lse, dctx, *ctx.shape, ctx.drops[0])
         dx = gemm_bf16(dqkv, wq, b_mn_major=True, add=dh) if ctx.needs_input_grad[0] else None
         s = ctx.sinks
         g = [None] * 4
@@ -394,52 +539,66 @@ class _AttentionBlockFn(torch.autograd.Function):
         if ctx.needs_input_grad[2]:
             g[1] = _bias_grad(dqkv.float().sum(0), qkv_b, s[1])
         if ctx.needs_input_grad[3]:
-            g[2] = _wgrad_to(dh, o, out_w, s[2])
+            g[2] = _wgrad_to(dhb, o, out_w, s[2])
         if ctx.needs_input_grad[4]:
-            g[3] = _bias_grad(dh.float().sum(0), out_b, s[3])
-        return (dx, *g, None, None, None, None, None)
+            g[3] = _bias_grad(dhb.float().sum(0), out_b, s[3])
+        return (dx, *g, None, None, None, None, None, None)
 
 
-def attention_block_reference(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads):
+def attention_block_reference(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, attn_z=None, hidden_z=None):
+    """Float32 math of ``attention_block``; ``attn_z`` [B, H, L, L] / ``hidden_z`` [B * L, C]: dropout (keep * scale)
+    on the probabilities and on the output branch."""
     f = torch.float32
     xf = x.float()
     qkv = torch.nn.functional.linear(xf, qkv_w.to(f), qkv_b.to(f))
-    o = attention_reference(qkv, mask, batch, seq_len, heads, qkv_w.shape[0] // (3 * heads))
-    return torch.nn.functional.linear(o, out_w.to(f), out_b.to(f)) + xf
+    o = attention_reference(qkv, mask, batch, seq_len, heads, qkv_w.shape[0] // (3 * heads), attn_z)
+    h = torch.nn.functional.linear(o, out_w.to(f), out_b.to(f))
+    return (h if hidden_z is None else hidden_z * h) + xf
 
 
-def attention_block(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads):
+def attention_block(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, attn_dropout=0.0, hidden_dropout=0.0):
     """Attention sub-layer with its residual: attention(x W_qkv^T + b_qkv) W_o^T + b_o + x, x [B * L, C] (bf16 on
     CUDA), the weights in any float dtype (cast to bf16 here), ``mask`` [B, L] (nonzero = attend) or None.  Returns
-    bf16 on the kernel path (the input of the following LayerNorm); differentiable in x and the four parameters."""
+    bf16 on the kernel path (the input of the following LayerNorm); differentiable in x and the four parameters.
+    ``attn_dropout`` drops attention probabilities, then ``hidden_dropout`` the output branch before the residual add
+    (two sites, in that order; branch index row * C + col)."""
     from .gemm import _grad_sink
 
+    pa, ph = _check_p(attn_dropout), _check_p(hidden_dropout)
     c = x.shape[-1]
     if x.is_cuda and c % 8 == 0 and c == heads * 64 and attention_train_supported(x, batch, seq_len, heads):
         sinks = tuple(_grad_sink(p) for p in (qkv_w, qkv_b, out_w, out_b))
+        drops = tuple(_draw(x.device, p) if p > 0.0 else None for p in (pa, ph))
         return _AttentionBlockFn.apply(x, qkv_w, qkv_b, out_w, out_b, _mask_u8(mask, x.device), batch, seq_len, heads,
-                                       sinks)
+                                       sinks, drops)
     if x.is_cuda:
         _count("attention_block: no kernel for B %d, L %d, H %d, width %d: float32 math on the library"
                % (batch, seq_len, heads, c))
-    return attention_block_reference(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads)
+    za = _site_z(x, pa, (batch, heads, seq_len, seq_len))
+    zh = _site_z(x, ph, (x.shape[0], c))
+    return attention_block_reference(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, za, zh)
 
 
 class _GeluFfnFn(torch.autograd.Function):
     """h = gelu(x W1^T + b1) W2^T + b2 + x, the feed-forward half of a post-LN encoder layer before its LayerNorm.
     FFN1 runs the GELU training epilogue (stores gelu(u) for FFN2 and u for the backward); FFN2's dgrad applies gelu'(u)
-    in its epilogue, so dU comes out of one GEMM; dx = dU W1 + dh is one dgrad GEMM with the residual gradient fused."""
+    in its epilogue, so dU comes out of one GEMM; dx = dU W1 + dh is one dgrad GEMM with the residual gradient fused.
+    ``drop``: the output-branch dropout site or None; FFN2's epilogue then stores x + Z o (y W2^T + b2) and the backward
+    takes dh_b = Z o dh for dU, dW2 and db2 (the residual receives dh)."""
 
     @staticmethod
-    def forward(ctx, x, w1, b1, w2, b2, sinks):
-        from .gemm import gemm_bf16, gemm_bf16_gelu_train
+    def forward(ctx, x, w1, b1, w2, b2, sinks, drop):
+        from .gemm import gemm_bf16, gemm_bf16_gelu_train, gemm_bf16_residual_dropout
 
         x = _bf16(x).contiguous()
         w1h, w2h = _bf16(w1).contiguous(), _bf16(w2).contiguous()
         y, u = gemm_bf16_gelu_train(x, w1h, b1.float())
-        h = gemm_bf16(y, w2h, col_shift=b2.float(), add=x)
+        if drop is None:
+            h = gemm_bf16(y, w2h, col_shift=b2.float(), add=x)
+        else:
+            h = gemm_bf16_residual_dropout(y, w2h, b2, x, drop)
         ctx.save_for_backward(x, w1h, w2h, y, u, w1, b1, w2, b2)
-        ctx.sinks = sinks
+        ctx.sinks, ctx.drop = sinks, drop
         return h
 
     @staticmethod
@@ -448,7 +607,8 @@ class _GeluFfnFn(torch.autograd.Function):
 
         x, w1h, w2h, y, u, w1, b1, w2, b2 = ctx.saved_tensors
         dh = _bf16(dh).contiguous()
-        du = gemm_bf16_gelu_grad(dh, w2h, u)
+        dhb = dh if ctx.drop is None else _dropout_apply(dh, ctx.drop)
+        du = gemm_bf16_gelu_grad(dhb, w2h, u)
         dx = gemm_bf16(du, w1h, b_mn_major=True, add=dh) if ctx.needs_input_grad[0] else None
         s = ctx.sinks
         g = [None] * 4
@@ -457,35 +617,39 @@ class _GeluFfnFn(torch.autograd.Function):
         if ctx.needs_input_grad[2]:
             g[1] = _bias_grad(du.float().sum(0), b1, s[1])
         if ctx.needs_input_grad[3]:
-            g[2] = _wgrad_to(dh, y, w2, s[2])
+            g[2] = _wgrad_to(dhb, y, w2, s[2])
         if ctx.needs_input_grad[4]:
-            g[3] = _bias_grad(dh.float().sum(0), b2, s[3])
-        return (dx, *g, None)
+            g[3] = _bias_grad(dhb.float().sum(0), b2, s[3])
+        return (dx, *g, None, None)
 
 
-def gelu_ffn_reference(x, w1, b1, w2, b2):
+def gelu_ffn_reference(x, w1, b1, w2, b2, drop_z=None):
+    """Float32 math of ``gelu_ffn``; ``drop_z`` [rows, C]: dropout (keep * scale) on the output branch."""
     f = torch.float32
     xf = x.float()
     u = torch.nn.functional.linear(xf, w1.to(f), b1.to(f))
-    return torch.nn.functional.linear(torch.nn.functional.gelu(u), w2.to(f), b2.to(f)) + xf
+    h = torch.nn.functional.linear(torch.nn.functional.gelu(u), w2.to(f), b2.to(f))
+    return (h if drop_z is None else drop_z * h) + xf
 
 
-def gelu_ffn(x, w1, b1, w2, b2):
+def gelu_ffn(x, w1, b1, w2, b2, dropout_p=0.0):
     """Feed-forward sub-layer with its residual: gelu(x W1^T + b1) W2^T + b2 + x (erf GELU), x [rows, C] (bf16 on
     CUDA), weights in any float dtype.  This is the trainable GELU linear: its backward needs FFN2's dgrad, which is
-    where gelu'(u) is applied.  Returns bf16 on the kernel path; differentiable in x and the four parameters."""
+    where gelu'(u) is applied.  Returns bf16 on the kernel path; differentiable in x and the four parameters.
+    ``dropout_p``: dropout on the output branch before the residual add (one site, index row * C + col)."""
     from .gemm import _grad_sink, _tma_compatible
     from . import native
 
+    p = _check_p(dropout_p)
     ffn, c = w1.shape
     if (x.is_cuda and x.dim() == 2 and c % 8 == 0 and ffn % 8 == 0 and native().persistent_gemm_enabled()
             and _tma_compatible(_bf16(x).contiguous(), _bf16(w1), None, ffn)):
-        sinks = tuple(_grad_sink(p) for p in (w1, b1, w2, b2))
-        return _GeluFfnFn.apply(x, w1, b1, w2, b2, sinks)
+        sinks = tuple(_grad_sink(t) for t in (w1, b1, w2, b2))
+        return _GeluFfnFn.apply(x, w1, b1, w2, b2, sinks, _draw(x.device, p) if p > 0.0 else None)
     if x.is_cuda:
         _count("gelu_ffn: no kernel for x %s, FFN %d (persistent GEMM on, widths % 8 == 0): float32 math on the library"
                % (tuple(x.shape), ffn))
-    return gelu_ffn_reference(x, w1, b1, w2, b2)
+    return gelu_ffn_reference(x, w1, b1, w2, b2, _site_z(x, p, (x.shape[0], c)))
 
 
 def _ln_part(rows, c, device):
@@ -544,12 +708,15 @@ def _table_grad(dE, idx, rows):
 
 class _EmbeddingLayerNormFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps):
+    def forward(ctx, ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps, drop):
         tabs = tuple(_bf16(t).contiguous() for t in (word, pos, seg))
         ids, pos_ids, seg_ids = (t.reshape(-1).to(word.device, torch.int64).contiguous() for t in (ids, pos_ids, seg_ids))
-        y = embedding_layernorm(ids, pos_ids, seg_ids, *tabs, gamma, beta, eps)
+        if drop is None:
+            y = embedding_layernorm(ids, pos_ids, seg_ids, *tabs, gamma, beta, eps)
+        else:
+            y = _embedding_layernorm_kernel(ids, pos_ids, seg_ids, *tabs, gamma, beta, eps, None, drop)
         ctx.save_for_backward(ids, pos_ids, seg_ids, *tabs, gamma, beta)
-        ctx.eps = eps
+        ctx.eps, ctx.drop = eps, drop
         ctx.dtypes = (word.dtype, pos.dtype, seg.dtype)
         return y
 
@@ -564,7 +731,7 @@ class _EmbeddingLayerNormFn(torch.autograd.Function):
         db = torch.empty_like(dg)
         native().embedding_layernorm_bwd(ids, pos_ids, seg_ids, word, pos, seg, _bf16(dy).contiguous(),
                                          gamma.float().contiguous(), dE, _ln_part(rows, c, word.device), dg, db,
-                                         float(ctx.eps))
+                                         float(ctx.eps), ctx.drop)
         count_launch(2)
         # the three table gradients, dE summed per table row.  The word table: the library's embedding backward, the
         # call nn.Embedding makes for the BiLSTM student.  The position and segment tables (at most _ONE_HOT_ROWS rows)
@@ -572,19 +739,24 @@ class _EmbeddingLayerNormFn(torch.autograd.Function):
         # one-hot GEMM, which is bitwise reproducible.
         grads = [None if not ctx.needs_input_grad[3 + i] else _table_grad(dE, idx, tab.shape[0]).to(dt)
                  for i, (idx, tab, dt) in enumerate(zip((ids, pos_ids, seg_ids), (word, pos, seg), ctx.dtypes))]
-        return None, None, None, *grads, dg.to(gamma.dtype), db.to(beta.dtype), None
+        return None, None, None, *grads, dg.to(gamma.dtype), db.to(beta.dtype), None, None
 
 
-def embedding_layernorm_trainable(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps=1e-12):
+def embedding_layernorm_trainable(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps=1e-12, dropout_p=0.0):
     """``embedding_layernorm`` with a gradient in the three tables and gamma / beta (tables in any float dtype, cast
-    to bf16 for the kernels).  Out-of-range ids raise as in ``embedding_layernorm``."""
+    to bf16 for the kernels).  Out-of-range ids raise as in ``embedding_layernorm``.  ``dropout_p``: dropout on the
+    output (one site, index row * C + col), applied by the same kernel."""
     c = word.shape[1]
     from . import native
 
+    p = _check_p(dropout_p)
     if word.is_cuda and all(t.is_cuda and t.dim() == 2 and t.shape[1] == c for t in (pos, seg)) \
             and native().layernorm_supported(c):
-        return _EmbeddingLayerNormFn.apply(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps)
+        return _EmbeddingLayerNormFn.apply(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps,
+                                           _draw(word.device, p) if p > 0.0 else None)
     if word.is_cuda:
         _count("embedding_layernorm: no training kernel for width %d: float32 math on the library" % c)
     f = torch.float32
-    return embedding_layernorm_reference(ids, pos_ids, seg_ids, word.to(f), pos.to(f), seg.to(f), gamma, beta, eps)
+    y = embedding_layernorm_reference(ids, pos_ids, seg_ids, word.to(f), pos.to(f), seg.to(f), gamma, beta, eps)
+    z = _site_z(word, p, (ids.numel(), c))
+    return y if z is None else y * z

@@ -33,6 +33,7 @@ def main():
     ap.add_argument("--T", type=float, default=2.0)
     ap.add_argument("--epochs", type=int, default=2)
     ap.add_argument("--vocab", type=int, default=2000)
+    ap.add_argument("--dropout", type=float, default=0.0, help="hidden and attention dropout of --model ernie")
     args = ap.parse_args()
     srv = None
     if not args.teachers:
@@ -43,7 +44,7 @@ def main():
     if args.model in ("lstm", "ernie"):  # these students run on the GPU when there is one
         dev = torch.device("cuda" if torch.cuda.is_available() else "cpu")
         # the Transformer student builds its four feeds from the ids (positions 0.., segment 0, mask ids != 0)
-        student = (BiLSTM(args.vocab) if args.model == "lstm" else ernie_student()).to(dev)
+        student = (BiLSTM(args.vocab) if args.model == "lstm" else ernie_student(dropout=args.dropout)).to(dev)
     else:
         student = BOW(args.vocab) if args.model == "bow" else TextCNN(args.vocab)
     opt = torch.optim.AdamW(student.parameters(), 1e-4 if args.model == "ernie" else 1e-3)   # a Transformer wants less

@@ -15,13 +15,13 @@ from paddle_edl.models.small import BOW, BiLSTM, TextCNN  # noqa: E402
 from paddle_edl.models.ernie import ernie_student  # noqa: E402
 
 
-def build_model(name, vocab):
+def build_model(name, vocab, dropout=0.0):
     """(model, device): the LSTM and Transformer students run on the GPU when there is one (csrc/lstm.cu, the encoder
     kernels), the others on the CPU.  The Transformer student has the teacher's 18000-id vocabulary and builds its four
-    feeds from the ids (positions 0.., segment 0, mask ids != 0)."""
+    feeds from the ids (positions 0.., segment 0, mask ids != 0); ``dropout`` is its hidden and attention dropout."""
     if name in ("lstm", "ernie"):
         dev = torch.device("cuda" if torch.cuda.is_available() else "cpu")
-        return (BiLSTM(vocab) if name == "lstm" else ernie_student()).to(dev), dev
+        return (BiLSTM(vocab) if name == "lstm" else ernie_student(dropout=dropout)).to(dev), dev
     return (BOW(vocab) if name == "bow" else TextCNN(vocab)), torch.device("cpu")
 
 
@@ -46,6 +46,7 @@ def main():
     ap.add_argument("--vocab", type=int, default=2000)
     ap.add_argument("--seq_len", type=int, default=64)
     ap.add_argument("--samples", type=int, default=1024)
+    ap.add_argument("--dropout", type=float, default=0.0, help="hidden and attention dropout of --model ernie")
     args = ap.parse_args()
     if args.train_tsv:
         tr = TsvReader(args.train_tsv, seq_len=args.seq_len)
@@ -57,7 +58,7 @@ def main():
         vocab = args.vocab
         train_iter = lambda ep: batches(synthetic_corpus(args.samples, vocab, args.seq_len, ep), 16)   # noqa: E731
         dev_data = list(batches(synthetic_corpus(256, vocab, args.seq_len, 10_000), 16))
-    model, dev = build_model(args.model, vocab)
+    model, dev = build_model(args.model, vocab, args.dropout)
     opt = torch.optim.AdamW(model.parameters(), 1e-4 if args.model == "ernie" else 1e-3)   # a Transformer wants less
     for ep in range(args.epochs):
         for ids, label in train_iter(ep):

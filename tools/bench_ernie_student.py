@@ -3,7 +3,9 @@
 AdamW) at B = 32, L = 128 with the student configuration (hidden 384, 4 layers, 6 heads, FFN 1536, vocabulary 18000)
 on the package's kernels, against the same bf16 model in torch (cuBLAS linears, F.scaled_dot_product_attention with
 the key mask, F.layer_norm, F.gelu), both as CUDA-graph replays; and the attention backward alone against SDPA's
-backward, eager.  All times come from CUDA events.  Prints the GPU name and power limit with the numbers."""
+backward, eager.  With ``--dropout p`` it times instead three training steps with hidden and attention dropout: ours at
+p, ours at 0, and the bf16 torch model with F.dropout at the same sites and SDPA's dropout_p = p.  All times come from
+CUDA events.  Prints the GPU name and power limit with the numbers."""
 import argparse
 import json
 import os
@@ -28,22 +30,25 @@ def gpu_info():
     return name, limit
 
 
-def torch_encoder(m, ids, keep):
-    """The student's layers in bf16 torch: cuBLAS linears, SDPA with the key mask, F.layer_norm, F.gelu."""
+def torch_encoder(m, ids, keep, p=0.0):
+    """The student's layers in bf16 torch: cuBLAS linears, SDPA with the key mask, F.layer_norm, F.gelu; with p > 0,
+    F.dropout at ErnieStudent's hidden sites and SDPA's dropout_p = p on the probabilities."""
     b, l = ids.shape
     c, nh = m.hidden, m.heads
+    d = (lambda t: F.dropout(t, p, True)) if p > 0 else (lambda t: t)
     pos = torch.arange(l, device=ids.device)
     x = F.embedding(ids, m.word_emb) + F.embedding(pos, m.pos_emb) + m.seg_emb[0]
-    x = F.layer_norm(x, (c,), m.emb_ln_g, m.emb_ln_b, m.eps)
+    x = d(F.layer_norm(x, (c,), m.emb_ln_g, m.emb_ln_b, m.eps))
     am = keep.view(b, 1, 1, l)
     for lyr in m.layers:
         q, k, v = F.linear(x, lyr.qkv_w, lyr.qkv_b).view(b, l, 3, nh, c // nh).unbind(2)
-        o = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), attn_mask=am)
-        x = F.layer_norm(F.linear(o.transpose(1, 2).reshape(b, l, c), lyr.out_w, lyr.out_b) + x, (c,), lyr.ln1_g,
+        o = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), attn_mask=am,
+                                           dropout_p=p)
+        x = F.layer_norm(d(F.linear(o.transpose(1, 2).reshape(b, l, c), lyr.out_w, lyr.out_b)) + x, (c,), lyr.ln1_g,
                          lyr.ln1_b, m.eps)
-        x = F.layer_norm(F.linear(F.gelu(F.linear(x, lyr.ffn1_w, lyr.ffn1_b)), lyr.ffn2_w, lyr.ffn2_b) + x, (c,),
+        x = F.layer_norm(d(F.linear(F.gelu(F.linear(x, lyr.ffn1_w, lyr.ffn1_b)), lyr.ffn2_w, lyr.ffn2_b)) + x, (c,),
                          lyr.ln2_g, lyr.ln2_b, m.eps)
-    return F.linear(torch.tanh(F.linear(x[:, 0], m.pool_w, m.pool_b)), m.cls_w, m.cls_b).float()
+    return F.linear(d(torch.tanh(F.linear(x[:, 0], m.pool_w, m.pool_b))), m.cls_w, m.cls_b).float()
 
 
 def graph_time(fn, warmup, iters):
@@ -87,6 +92,7 @@ def main():
     ap.add_argument("--seq", type=int, default=128)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--iters", type=int, default=50)
+    ap.add_argument("--dropout", type=float, default=None, help="time training steps with this dropout instead")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_ernie_student: needs a GPU")
@@ -114,6 +120,8 @@ def main():
         F.cross_entropy(torch_encoder(ref, ids, keep), label).backward()
         ropt.step()
 
+    if args.dropout is not None:
+        return bench_dropout(args, ours, opt, ref, ropt, ids, label, keep)
     ops.reset_fallbacks()
     t_ours = graph_time(step_ours, args.warmup, args.iters)
     fallbacks = ops.fallbacks()
@@ -137,6 +145,38 @@ def main():
                       "train_step_ms": {"ours": round(t_ours, 3), "torch_bf16": round(t_torch, 3)},
                       "attention_bwd_us": {"ours": round(t_abwd * 1e3, 1), "sdpa": round(t_sdpa * 1e3, 1)},
                       "fallbacks": fallbacks}))
+
+
+def bench_dropout(args, ours, opt, ref, ropt, ids, label, keep):
+    """Training steps with dropout p against the same steps at p = 0 and against torch with dropout, CUDA-graph
+    replays, the three alternated over five rounds (the median of each is printed)."""
+    p = args.dropout
+
+    def step_ours(q):
+        def fn():
+            ours.hidden_dropout = ours.attention_dropout = q
+            opt.zero_grad(set_to_none=False)
+            F.cross_entropy(ours(ids), label).backward()
+            opt.step()
+        return fn
+
+    def step_torch():
+        ropt.zero_grad(set_to_none=False)
+        F.cross_entropy(torch_encoder(ref, ids, keep, p), label).backward()
+        ropt.step()
+
+    ops.reset_fallbacks()
+    arms = {"ours_p": step_ours(p), "ours_0": step_ours(0.0), "torch_bf16_p": step_torch}
+    times = {k: [] for k in arms}
+    for _ in range(5):
+        for k, fn in arms.items():
+            times[k].append(graph_time(fn, args.warmup, args.iters))
+    med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
+    name, limit = gpu_info()
+    print(json.dumps({"gpu": name, "power_limit": limit, "batch": args.batch, "seq": args.seq, "dropout": p,
+                      "train_step_ms": {k: round(v, 3) for k, v in med.items()},
+                      "dropout_overhead": round(med["ours_p"] / med["ours_0"] - 1.0, 4),
+                      "fallbacks": ops.fallbacks()}))
 
 
 if __name__ == "__main__":
