@@ -1,4 +1,5 @@
-// Masked multi-head attention forward for sm_90a (the ERNIE / BERT encoder of the NLP teacher; inference only).
+// Masked multi-head attention forward for sm_90a (the ERNIE / BERT encoder of the NLP teacher and of the Transformer
+// student).
 //
 //   O[b, i, h, :] = sum_j softmax_j(Q[b, i, h, :] . K[b, j, h, :] / 8 + mask[b, j]) V[b, j, h, :],   head dim 64
 //
@@ -24,15 +25,22 @@
 // tensormap.cp_fenceproxy); the attention kernel acquires them and runs the same body with L = len_b.  A sequence's
 // output thus depends on its own rows only, whatever the others hold (NaN included), and nothing is stored outside it.
 //
-// Training (padded layout only): with lse != nullptr the kernel also stores, per (b, h, query), lse = m + log2(l) in the
-// log2 units of the scaled scores (m the row max of S / 8 * log2(e), l the row sum over the bf16-rounded probabilities), or
-// +inf for a row without a valid key; attention_bwd.cu recomputes P = exp2(S / 8 * log2(e) - lse) from it.  The store
-// sits after O is formed, so O does not depend on whether lse is given.
+// Training: with lse != nullptr the padded kernel also stores, per (b, h, query), lse = m + log2(l) in the log2 units of
+// the scaled scores (m the row max of S / 8 * log2(e), l the row sum over the bf16-rounded probabilities), or +inf for a
+// row without a valid key; attention_bwd.cu recomputes P = exp2(S / 8 * log2(e) - lse) from it.  The store sits after O
+// is formed, so O does not depend on whether lse is given.  The packed layout's training instantiation (Seq =
+// VarlenTrain, a separate type, so the inference kernel the teacher serves with is not touched) stores the same lse in
+// fp32 [H, T] at h * T + packed row: the 64 queries of a consumer group are contiguous.
 //
-// Dropout on the attention probabilities (padded training instantiation, kDrop): element (b, h, i, j) of P has the
-// flat index ((b H + h) L + i) L + j in the mask of philox.cuh.  A dropped probability is zeroed in the bf16 A fragment
-// after the row sum has taken it, so m, l and lse stay those of the undropped softmax (lse is bitwise the p = 0 lse) and
-// the scale 1 / (1 - p) is applied to the fp32 output together with 1 / l.
+// Budgets (ptxas -v, sm_90a, __launch_bounds__(384, 1)): padded 98 registers (167 with dropout), packed inference 98,
+// packed training 101 (164 with dropout), no spills.
+//
+// Dropout on the attention probabilities (training instantiations, kDrop): element (b, h, i, j) of P has the flat index
+// ((b H + h) L + i) L + j in the mask of philox.cuh in the padded layout, and ((b H + h) 512 + i) 512 + j in the packed
+// one (the fixed stride kAttnMaxLen keeps the index ranges of the sequences disjoint whatever their lengths).  A dropped
+// probability is zeroed in the bf16 A fragment after the row sum has taken it, so m, l and lse stay those of the
+// undropped softmax (lse is bitwise the p = 0 lse) and the scale 1 / (1 - p) is applied to the fp32 output together
+// with 1 / l.
 #include <cuda.h>
 
 #include <type_traits>
@@ -78,14 +86,22 @@ struct Varlen {
   const CUtensorMap* maps;
 };
 
-// Seq = int: the padded layout, seq = L for every sequence (tmQKV / tmO span the whole batch).  Seq = Varlen: packed.
-// kDrop: dropout on P with the mask of `drop` (padded layout only).
+// The packed layout in training: also stores lse [H, T] (T packed rows), and may drop probabilities
+struct VarlenTrain {
+  const int* cu_seqlens;
+  const CUtensorMap* maps;
+  int T;
+};
+
+// Seq = int: the padded layout, seq = L for every sequence (tmQKV / tmO span the whole batch).  Seq = Varlen: packed,
+// inference.  Seq = VarlenTrain: packed, training.  kDrop: dropout on P with the mask of `drop` (training only).
 template <typename Seq, bool kDrop = false>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO,
                      const uint8_t* __restrict__ mask, Seq seq, int H, float* __restrict__ lse, const PhiloxArgs drop) {
-  constexpr bool kVarlen = std::is_same<Seq, Varlen>::value;
-  static_assert(!(kVarlen && kDrop), "dropout: padded layout only");
+  constexpr bool kVarlenTrain = std::is_same<Seq, VarlenTrain>::value;
+  constexpr bool kVarlen = std::is_same<Seq, Varlen>::value || kVarlenTrain;
+  static_assert(!(kVarlen && kDrop) || kVarlenTrain, "dropout: training instantiations only");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -167,8 +183,9 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
     [[maybe_unused]] uint64_t nrow[2];                          // flat mask index of key 0 of this thread's two rows
     if constexpr (kDrop) {
       pk = philox_key(drop);
+      const int dl = kVarlen ? kAttnMaxLen : L;                  // the mask's row stride: L padded, 512 packed
 #pragma unroll
-      for (int r = 0; r < 2; ++r) nrow[r] = (((uint64_t)b * H + h) * L + (q0 + cw * 64 + row + 8 * r)) * (uint64_t)L;
+      for (int r = 0; r < 2; ++r) nrow[r] = (((uint64_t)b * H + h) * dl + (q0 + cw * 64 + row + 8 * r)) * (uint64_t)dl;
     }
     ptx::mbar_wait(q_bar, 0);
     const uint64_t dq = ptx::make_smem_desc(ptx::smem_u32(sq + cw * kHalfBytes), 16, 1024);
@@ -255,6 +272,15 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
       for (int r = 0; r < 2; ++r) {
         const int qi = q0 + cw * 64 + row + 8 * r;
         if (qi < L) lse[((int64_t)b * H + h) * L + qi] = l[r] > 0.f ? m[r] + log2f(l[r]) : INFINITY;
+      }
+    }
+    if constexpr (kVarlenTrain) {
+      if ((lane & 3) == 0) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int qi = q0 + cw * 64 + row + 8 * r;
+          if (qi < L) lse[(int64_t)h * seq.T + start + qi] = l[r] > 0.f ? m[r] + log2f(l[r]) : INFINITY;
+        }
       }
     }
     uint8_t* st = sq + cw * kHalfBytes;
@@ -359,17 +385,24 @@ bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim) 
 }
 
 const char* attention_varlen_fwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, void* out, void* maps,
-                                 int T, int B, int max_len, int H, cudaStream_t stream) {
+                                 int T, int B, int max_len, int H, cudaStream_t stream, float* lse,
+                                 const PhiloxArgs* drop) {
   if (!attention_varlen_supported(T, B, max_len, H, 64))
     return "attention_varlen_fwd: unsupported shape (head dim 64, T >= 1, 1 <= max_len <= 512)";
+  if (drop != nullptr && lse == nullptr) return "attention_varlen_fwd: dropout is a training feature (give lse)";
   // templates over the whole buffer; the prologue replaces the address and the row count per sequence
   alignas(64) CUtensorMap tmQKV, tmO;
   if (const char* e = encode_attention_maps(&tmQKV, &tmO, qkv, out, T, 1, H)) return e;
   CUtensorMap* m = static_cast<CUtensorMap*>(maps);
   attention_varlen_maps_kernel<<<(B + 3) / 4, 128, 0, stream>>>(tmQKV, tmO, qkv, out, cu_seqlens, m, B, H);
   if (cudaError_t e = cudaGetLastError(); e != cudaSuccess) return cudaGetErrorString(e);
-  return launch_attention<Varlen>(tmQKV, tmO, key_mask, Varlen{cu_seqlens, m}, H, dim3((max_len + 127) / 128, H, B),
-                                  stream);
+  const dim3 grid((max_len + 127) / 128, H, B);
+  if (lse != nullptr) {
+    const VarlenTrain seq{cu_seqlens, m, T};
+    if (drop != nullptr) return launch_attention<VarlenTrain, true>(tmQKV, tmO, key_mask, seq, H, grid, stream, lse, *drop);
+    return launch_attention<VarlenTrain>(tmQKV, tmO, key_mask, seq, H, grid, stream, lse);
+  }
+  return launch_attention<Varlen>(tmQKV, tmO, key_mask, Varlen{cu_seqlens, m}, H, grid, stream);
 }
 
 }  // namespace edl

@@ -20,8 +20,17 @@
 // (philox.cuh; the mask does not depend on the tile order), dV = (Z o P)^T dO and dS = P o (Z o dP - D), D taken over the
 // stored, dropped O as before (FlashAttention-2's identity).  A row without a valid key still gets zero gradients.
 //
+// Packed sequences (kVarlen, attention_varlen_bwd): qkv / dqkv [T, 3 * H * 64], O / dO [T, H * 64], sequence b in rows
+// [cu_seqlens[b], cu_seqlens[b + 1]); lse and D are fp32 [H, T] at h * T + packed row (attention.cu's VarlenTrain), and
+// the dropout index of (b, h, i, j) is ((b H + h) 512 + i) 512 + j.  The grid spans the longest sequence; a CTA reads its
+// sequence's start and length L, exits when its tile starts at or past L, and otherwise runs the padded body with that
+// L on the rows from the start: the same tiles and bounds, so no row outside the sequence is read as its data and the
+// bits are those of the padded kernels at B = 1 (up to the dropout index).  A key is valid iff key < L and key_mask of
+// its packed row is set.  D is the padded delta pass over T rows as one sequence (B = 1, L = T).
+//
 // Budgets (ptxas -v, sm_90a, 128 threads): attn_bwd_dkdv 175 registers (228 with dropout), attn_bwd_dq 134 (242),
-// attn_bwd_delta 40, no spills;
+// attn_bwd_delta 40, no spills; packed: attn_bwd_dkdv 173 registers (220 with dropout), attn_bwd_dq 136 (175), no
+// spills;
 // static shared memory 36.5 KB (dkdv: Q, Q^T, dO, dO^T tiles + lse / D) and 27.1 KB (dq: K, K^T, V tiles + key flags).
 #include "common.cuh"
 #include "kernels.h"
@@ -127,18 +136,28 @@ attn_bwd_delta(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __res
   }
 }
 
-template <bool kDrop>
+template <bool kDrop, bool kVarlen = false>
 __global__ void __launch_bounds__(128)
 attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ mask,
               const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse, const float* __restrict__ delta,
-              __nv_bfloat16* __restrict__ dqkv, int L, int H, const PhiloxArgs drop) {
+              __nv_bfloat16* __restrict__ dqkv, int L, int H, const PhiloxArgs drop,
+              const int* __restrict__ cu_seqlens = nullptr, int T = 0) {
   __shared__ alignas(16) __nv_bfloat16 sQ[kT * kP], sQt[kT * kP], sO[kT * kP], sOt[kT * kP];
   __shared__ float sL[kT], sD[kT];
   const int k0 = blockIdx.x * kT, h = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const int64_t ldq = (int64_t)3 * H * 64, ldo = (int64_t)H * 64;
-  const __nv_bfloat16* base = qkv + (int64_t)b * L * ldq;
-  const int64_t sh = ((int64_t)b * H + h) * L;
+  int64_t r0 = (int64_t)b * L;                                  // the sequence's first row
+  if constexpr (kVarlen) {
+    r0 = cu_seqlens[b];
+    L = cu_seqlens[b + 1] - (int)r0;
+    if (k0 >= L) return;                                        // the grid spans the longest sequence
+  }
+  const __nv_bfloat16* base = qkv + r0 * ldq;
+  // lse / D of head h and row i at sh + i; the dropout index of (i, j) is (dsh + i) dl + j
+  const int64_t sh = kVarlen ? (int64_t)h * T + r0 : ((int64_t)b * H + h) * L;
+  const int dl = kVarlen ? kAttnMaxLen : L;
+  const uint64_t dsh = kVarlen ? ((uint64_t)b * H + h) * kAttnMaxLen : (uint64_t)sh;
   // this warp's 16 keys of K and V as A fragments (staged through the Q / dO tiles)
   load_tile(base + (H + h) * 64, ldq, k0, L, sQ, nullptr);
   load_tile(base + (2 * H + h) * 64, ldq, k0, L, sO, nullptr);
@@ -151,7 +170,7 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     const int key = key0 + 8 * e;
-    kv[e] = key < L && (mask == nullptr || mask[(int64_t)b * L + key] != 0);
+    kv[e] = key < L && (mask == nullptr || mask[r0 + key] != 0);
   }
   float dk[8][4], dv[8][4];
 #pragma unroll
@@ -164,7 +183,7 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
   for (int q0 = 0; q0 < L; q0 += kT) {
     __syncthreads();                                        // the previous tiles (or the K / V staging) are consumed
     load_tile(base + h * 64, ldq, q0, L, sQ, sQt);
-    load_tile(dout + (int64_t)b * L * ldo + h * 64, ldo, q0, L, sO, sOt);
+    load_tile(dout + r0 * ldo + h * 64, ldo, q0, L, sO, sOt);
     if (threadIdx.x < kT) {
       const int q = q0 + threadIdx.x;
       sL[threadIdx.x] = q < L ? lse[sh + q] : INFINITY;
@@ -178,7 +197,7 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
 #pragma unroll 1
       for (int i = 0; i < 32; ++i) {
         const int qc = (i >> 2) * 8 + 2 * t + (i & 1);
-        const uint64_t n = ((uint64_t)sh + (q0 + qc)) * (uint64_t)L + (key0 + 8 * ((i >> 1) & 1));
+        const uint64_t n = (dsh + (q0 + qc)) * (uint64_t)dl + (key0 + 8 * ((i >> 1) & 1));
         km |= dropout_keep(pk, n) ? 1u << i : 0u;
       }
     }
@@ -219,26 +238,36 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
         mma16816(dk[j], sa[k], lds(rq), lds(rq + 8));
       }
   }
-  __nv_bfloat16* drow = dqkv + (int64_t)b * L * ldq;
+  __nv_bfloat16* drow = dqkv + r0 * ldq;
   store_rows(dk, drow + (H + h) * 64, ldq, key0, L, t, 0.125f);
   store_rows(dv, drow + (2 * H + h) * 64, ldq, key0, L, t, 1.f);
 }
 
-template <bool kDrop>
+template <bool kDrop, bool kVarlen = false>
 __global__ void __launch_bounds__(128)
 attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ mask,
             const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse, const float* __restrict__ delta,
-            __nv_bfloat16* __restrict__ dqkv, int L, int H, const PhiloxArgs drop) {
+            __nv_bfloat16* __restrict__ dqkv, int L, int H, const PhiloxArgs drop,
+            const int* __restrict__ cu_seqlens = nullptr, int T = 0) {
   __shared__ alignas(16) __nv_bfloat16 sK[kT * kP], sKt[kT * kP], sV[kT * kP];
   __shared__ uint8_t sM[kT];
   const int q0 = blockIdx.x * kT, h = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const int64_t ldq = (int64_t)3 * H * 64, ldo = (int64_t)H * 64;
-  const __nv_bfloat16* base = qkv + (int64_t)b * L * ldq;
-  const int64_t sh = ((int64_t)b * H + h) * L;
+  int64_t r0 = (int64_t)b * L;                                  // the sequence's first row
+  if constexpr (kVarlen) {
+    r0 = cu_seqlens[b];
+    L = cu_seqlens[b + 1] - (int)r0;
+    if (q0 >= L) return;                                        // the grid spans the longest sequence
+  }
+  const __nv_bfloat16* base = qkv + r0 * ldq;
+  // lse / D of head h and row i at sh + i; the dropout index of (i, j) is (dsh + i) dl + j
+  const int64_t sh = kVarlen ? (int64_t)h * T + r0 : ((int64_t)b * H + h) * L;
+  const int dl = kVarlen ? kAttnMaxLen : L;
+  const uint64_t dsh = kVarlen ? ((uint64_t)b * H + h) * kAttnMaxLen : (uint64_t)sh;
   // this warp's 16 queries of Q and dO as A fragments (staged through the K / V tiles)
   load_tile(base + h * 64, ldq, q0, L, sK, nullptr);
-  load_tile(dout + (int64_t)b * L * ldo + h * 64, ldo, q0, L, sV, nullptr);
+  load_tile(dout + r0 * ldo + h * 64, ldo, q0, L, sV, nullptr);
   __syncthreads();
   uint32_t qf[4][4], of[4][4];
   load_afrag(sK, warp * 16, g, t, qf);
@@ -265,7 +294,7 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
     load_tile(base + (2 * H + h) * 64, ldq, kb, L, sV, nullptr);
     if (threadIdx.x < kT) {
       const int key = kb + threadIdx.x;
-      sM[threadIdx.x] = (key < L && (mask == nullptr || mask[(int64_t)b * L + key] != 0)) ? 1 : 0;
+      sM[threadIdx.x] = (key < L && (mask == nullptr || mask[r0 + key] != 0)) ? 1 : 0;
     }
     __syncthreads();
     float s[8][4], dp[8][4];
@@ -281,7 +310,7 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
       if constexpr (kDrop) {
 #pragma unroll
         for (int r = 0; r < 2; ++r)
-          keep[r] = dropout_keep2(pk, ((uint64_t)sh + (qr + 8 * r)) * (uint64_t)L + (kb + j * 8 + 2 * t));
+          keep[r] = dropout_keep2(pk, (dsh + (qr + 8 * r)) * (uint64_t)dl + (kb + j * 8 + 2 * t));
       }
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
@@ -305,7 +334,7 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
         mma16816(dq[j], sa[k], lds(rk), lds(rk + 8));
       }
   }
-  store_rows(dq, dqkv + (int64_t)b * L * ldq + h * 64, ldq, qr, L, t, 0.125f);
+  store_rows(dq, dqkv + r0 * ldq + h * 64, ldq, qr, L, t, 0.125f);
 }
 
 }  // namespace
@@ -326,6 +355,30 @@ const char* attention_bwd(const void* qkv, const uint8_t* mask, const void* out,
   } else {
     attn_bwd_dkdv<false><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, PhiloxArgs{});
     attn_bwd_dq<false><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, PhiloxArgs{});
+  }
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
+const char* attention_varlen_bwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, const void* out,
+                                 const float* lse, const void* dout, void* dqkv, float* delta, int T, int B, int max_len,
+                                 int H, cudaStream_t stream, const PhiloxArgs* drop) {
+  if (!attention_varlen_supported(T, B, max_len, H, 64))
+    return "attention_varlen_bwd: unsupported shape (head dim 64, T >= 1, 1 <= max_len <= 512)";
+  const auto* q = reinterpret_cast<const __nv_bfloat16*>(qkv);
+  const auto* o = reinterpret_cast<const __nv_bfloat16*>(out);
+  const auto* d = reinterpret_cast<const __nv_bfloat16*>(dout);
+  auto* dq = reinterpret_cast<__nv_bfloat16*>(dqkv);
+  attn_bwd_delta<<<(unsigned)(((int64_t)T + 7) / 8), 256, 0, stream>>>(o, d, delta, 1, T, H);   // D [H, T]
+  const dim3 grid((max_len + kT - 1) / kT, H, B);
+  if (drop != nullptr) {
+    attn_bwd_dkdv<true, true><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, *drop, cu_seqlens, T);
+    attn_bwd_dq<true, true><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, *drop, cu_seqlens, T);
+  } else {
+    attn_bwd_dkdv<false, true><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, PhiloxArgs{},
+                                                         cu_seqlens, T);
+    attn_bwd_dq<false, true><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, PhiloxArgs{},
+                                                       cu_seqlens, T);
   }
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);

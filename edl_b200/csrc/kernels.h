@@ -241,8 +241,19 @@ bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim);
 // Packed sequences: qkv bf16 [T, 3 * H * 64], sequence b in rows [cu_seqlens[b], cu_seqlens[b + 1]) (int32 device
 // offsets, 1 <= length <= max_len <= 512), key_mask uint8 [T] (1 = attend; nullptr: all), out bf16 [T, H * 64];
 // maps: device workspace of 2 * B CUtensorMaps (64-byte aligned).  A sequence's output depends on its own rows only.
+// lse (training): nullptr, or fp32 [H, T] that receives lse at h * T + packed row (a separate kernel instantiation; the
+// inference one is unchanged).  drop (training, with lse): dropout on the probabilities, element (b, h, i, j) at flat
+// index ((b H + h) 512 + i) 512 + j of the mask: the fixed stride kAttnMaxLen keeps the sequences' ranges disjoint.
 const char* attention_varlen_fwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, void* out, void* maps,
-                                 int T, int B, int max_len, int H, cudaStream_t stream);
+                                 int T, int B, int max_len, int H, cudaStream_t stream, float* lse = nullptr,
+                                 const PhiloxArgs* drop = nullptr);
+// Backward of the packed training forward (attention_bwd.cu): from qkv, out and lse [H, T] of attention_varlen_fwd and
+// dout bf16 [T, H * 64], writes the rows of every sequence of dqkv bf16 [T, 3 * H * 64] (rows outside all sequences are
+// not written).  delta: fp32 [H, T] workspace.  drop: the forward's dropout.  A sequence's gradients depend on its own
+// rows only.  Deterministic, no atomics, no host synchronisation.
+const char* attention_varlen_bwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, const void* out,
+                                 const float* lse, const void* dout, void* dqkv, float* delta, int T, int B, int max_len,
+                                 int H, cudaStream_t stream, const PhiloxArgs* drop = nullptr);
 constexpr int kLnMaxC = 1024;
 bool layernorm_supported(int C);
 // y[r] = (x[r] - mean) * rsqrt(var + eps) * gamma + beta over the C columns of each row; x, y bf16 [rows, C] (row pitch

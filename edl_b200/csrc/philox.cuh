@@ -2,6 +2,11 @@
 // numbers: as easy as 1, 2, 3", SC 2011) keyed by the site's seed, counter (n / 4, offset), word n % 4.  The mask of an
 // element is a pure function of (seed, offset, n), so a backward kernel regenerates exactly the forward's mask whatever
 // order it visits the elements in.  ops.transformer.dropout_keep_reference is the same rule in torch arithmetic.
+//
+// The flat index n of each site's elements (kernels.h states it per entry point):
+//   attention probabilities (b, h, i, j)   ((b H + h) L + i) L + j padded [B, L]; ((b H + h) 512 + i) 512 + j packed
+//                                           (attention_varlen_*: the fixed stride keeps the sequences' ranges disjoint)
+//   residual branches, embedding-LN output  row * C + col, padded or packed rows alike
 #pragma once
 #include "common.cuh"
 #include "kernels.h"

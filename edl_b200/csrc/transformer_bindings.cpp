@@ -104,31 +104,72 @@ void attention_bwd(const Tensor& qkv, const c10::optional<Tensor>& mask, const T
   TORCH_CHECK(err == nullptr, "edl attention_bwd failed: ", err);
 }
 
-// qkv [T, 3 * H * 64], cu_seqlens int32 [B + 1], key_mask uint8 [T] or None, out [T, H * 64], maps uint8 [B * 256]
-void attention_varlen_fwd(const Tensor& qkv, const Tensor& cu_seqlens, const c10::optional<Tensor>& key_mask,
-                          Tensor& out, Tensor& maps, int64_t max_len, int64_t H) {
-  check_bf16_2d(qkv, "qkv");
-  check_bf16_2d(out, "out");
-  const int64_t T = qkv.size(0), B = cu_seqlens.numel() - 1;
-  TORCH_CHECK(qkv.size(1) == 3 * H * 64, "qkv must be [T, 3 * H * 64]");
-  TORCH_CHECK(out.size(0) == T && out.size(1) == H * 64, "out must be [T, H * 64]");
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0);
+// cu_seqlens int32 [B + 1] and key_mask uint8 [T] or None of a packed batch of T rows; returns B
+int64_t check_varlen(const Tensor& cu_seqlens, const c10::optional<Tensor>& key_mask, int64_t T, const uint8_t** mp) {
+  const int64_t B = cu_seqlens.numel() - 1;
   TORCH_CHECK(cu_seqlens.is_cuda() && cu_seqlens.scalar_type() == at::kInt && cu_seqlens.dim() == 1 &&
               cu_seqlens.is_contiguous() && B >= 1, "cu_seqlens must be a contiguous int32 [B + 1] CUDA tensor");
-  TORCH_CHECK(maps.is_cuda() && maps.scalar_type() == at::kByte && maps.is_contiguous() && maps.numel() >= B * 256 &&
-              reinterpret_cast<uintptr_t>(maps.data_ptr()) % 64 == 0, "maps: 64-byte aligned uint8 [B * 256] workspace");
-  TORCH_CHECK(T < (int64_t{1} << 31) && B <= 65535, "attention_varlen_fwd: T < 2^31 rows, B <= 65535 sequences");
-  const uint8_t* mp = nullptr;
+  TORCH_CHECK(T < (int64_t{1} << 31) && B <= 65535, "attention_varlen: T < 2^31 rows, B <= 65535 sequences");
+  *mp = nullptr;
   if (key_mask.has_value() && key_mask->defined()) {
     TORCH_CHECK(key_mask->is_cuda() && key_mask->scalar_type() == at::kByte && key_mask->is_contiguous() &&
                 key_mask->numel() == T, "key_mask must be a contiguous uint8 [T] CUDA tensor");
-    mp = key_mask->data_ptr<uint8_t>();
+    *mp = key_mask->data_ptr<uint8_t>();
+  }
+  return B;
+}
+
+// qkv [T, 3 * H * 64], cu_seqlens int32 [B + 1], key_mask uint8 [T] or None, out [T, H * 64], maps uint8 [B * 256];
+// training: lse fp32 [H, T] (and drop, with lse) or None
+void attention_varlen_fwd(const Tensor& qkv, const Tensor& cu_seqlens, const c10::optional<Tensor>& key_mask,
+                          Tensor& out, Tensor& maps, int64_t max_len, int64_t H, const c10::optional<Tensor>& lse,
+                          const edl::PhiloxArgs* drop) {
+  check_bf16_2d(qkv, "qkv");
+  check_bf16_2d(out, "out");
+  const int64_t T = qkv.size(0);
+  TORCH_CHECK(qkv.size(1) == 3 * H * 64, "qkv must be [T, 3 * H * 64]");
+  TORCH_CHECK(out.size(0) == T && out.size(1) == H * 64, "out must be [T, H * 64]");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0);
+  const uint8_t* mp;
+  const int64_t B = check_varlen(cu_seqlens, key_mask, T, &mp);
+  TORCH_CHECK(maps.is_cuda() && maps.scalar_type() == at::kByte && maps.is_contiguous() && maps.numel() >= B * 256 &&
+              reinterpret_cast<uintptr_t>(maps.data_ptr()) % 64 == 0, "maps: 64-byte aligned uint8 [B * 256] workspace");
+  float* lp = nullptr;
+  if (lse.has_value() && lse->defined()) {
+    TORCH_CHECK(lse->is_cuda() && lse->scalar_type() == at::kFloat && lse->is_contiguous() && lse->numel() == H * T &&
+                lse->device() == qkv.device(), "lse must be a contiguous fp32 [H, T] CUDA tensor");
+    lp = lse->data_ptr<float>();
   }
   c10::cuda::CUDAGuard guard(qkv.device());
   const char* err = edl::attention_varlen_fwd(qkv.data_ptr(), cu_seqlens.data_ptr<int>(), mp, out.data_ptr(),
                                               maps.data_ptr(), (int)T, (int)B, (int)max_len, (int)H,
-                                              at::cuda::getCurrentCUDAStream().stream());
+                                              at::cuda::getCurrentCUDAStream().stream(), lp, drop);
   TORCH_CHECK(err == nullptr, "edl attention_varlen_fwd failed: ", err);
+}
+
+// dqkv [T, 3 * H * 64] (the rows of every sequence) from qkv, the packed forward's out and lse [H, T], dout [T, H * 64];
+// delta fp32 [H, T]
+void attention_varlen_bwd(const Tensor& qkv, const Tensor& cu_seqlens, const c10::optional<Tensor>& key_mask,
+                          const Tensor& out, const Tensor& lse, const Tensor& dout, Tensor& dqkv, Tensor& delta,
+                          int64_t max_len, int64_t H, const edl::PhiloxArgs* drop) {
+  for (const Tensor* t : {&qkv, &out, &dout, static_cast<const Tensor*>(&dqkv)})
+    check_bf16_2d(*t, "attention_varlen_bwd operand");
+  const int64_t T = qkv.size(0);
+  TORCH_CHECK(qkv.size(1) == 3 * H * 64 && dqkv.sizes() == qkv.sizes(), "qkv / dqkv must be [T, 3 * H * 64]");
+  TORCH_CHECK(out.size(0) == T && out.size(1) == H * 64 && dout.sizes() == out.sizes(), "out / dout: [T, H * 64]");
+  for (const Tensor* t : {&lse, static_cast<const Tensor*>(&delta)})
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() == H * T &&
+                t->device() == qkv.device(), "lse / delta must be contiguous fp32 [H, T] CUDA tensors");
+  for (const Tensor* t : {&qkv, &out, &dout, static_cast<const Tensor*>(&dqkv)})
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0 && t->device() == qkv.device());
+  const uint8_t* mp;
+  const int64_t B = check_varlen(cu_seqlens, key_mask, T, &mp);
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const char* err = edl::attention_varlen_bwd(qkv.data_ptr(), cu_seqlens.data_ptr<int>(), mp, out.data_ptr(),
+                                              lse.data_ptr<float>(), dout.data_ptr(), dqkv.data_ptr(),
+                                              delta.data_ptr<float>(), (int)T, (int)B, (int)max_len, (int)H,
+                                              at::cuda::getCurrentCUDAStream().stream(), drop);
+  TORCH_CHECK(err == nullptr, "edl attention_varlen_bwd failed: ", err);
 }
 
 void check_affine(const Tensor& g, const Tensor& b, int64_t C) {
@@ -278,6 +319,7 @@ void register_transformer_bindings(pybind11::module_& m) {
   m.def("attention_supported", &edl::attention_supported);
   m.def("attention_varlen_fwd", &attention_varlen_fwd);
   m.def("attention_varlen_supported", &edl::attention_varlen_supported);
+  m.def("attention_varlen_bwd", &attention_varlen_bwd);
   m.def("layernorm_fwd", &layernorm_fwd);
   m.def("layernorm_supported", &edl::layernorm_supported);
   m.def("attention_bwd", &attention_bwd);

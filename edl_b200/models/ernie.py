@@ -13,6 +13,7 @@ PyTorch math (the reference the GPU path is tested against).
 
 ``forward_packed`` runs the same layers on a batch packed to its real tokens (``pack_sequences``) with the
 variable-length attention kernel; ``forward_requests`` packs requests of different lengths for the teacher server.
+``ErnieStudent.forward_packed`` is its training form.
 
 ``enable_fp8()`` switches the four linear layers of every encoder layer to the block-scaled e4m3 GEMM (ops/fp8.py):
 the LayerNorms write the next GEMM's quantised operand themselves, FFN1's epilogue quantises its GELU output for FFN2,
@@ -333,7 +334,15 @@ class ErnieStudent(ErnieEncoder):
     A step thus advances the generator offset by 4 * (2 + 3 * layers).  A site with p = 0 draws nothing and runs the
     p = 0 kernels; on CPU the sites are ``F.dropout``.  Dropout adds no parameters or buffers.
 
-    ``forward`` also takes the token ids alone: positions are then 0 .. L - 1, segments 0 and the mask ``ids != 0``."""
+    ``forward`` also takes the token ids alone: positions are then 0 .. L - 1, segments 0 and the mask ``ids != 0``.
+
+    ``forward_packed`` trains on a batch packed to its real tokens (``pack_sequences``): every GEMM, LayerNorm and
+    attention tile runs on the T real rows only, and the [CLS] rows are rows cu_seqlens[:-1].  Its dropout sites and
+    their order are those above, with packed indices: the hidden sites (1, 3, 4) at packed row * C + col, the attention
+    probabilities (2) at ((b H + h) 512 + i) 512 + j (a fixed stride, so the sequences' index ranges are disjoint), the
+    pooled features (5) at b * C + col; a step advances the offset by the same 4 * (2 + 3 * layers).  The padded
+    ``forward`` is the shape-stable entry point: one graph per (B, L), where a packed step's graph is fixed to its T and
+    cu_seqlens."""
 
     def __init__(self, *args, hidden_dropout=0.0, attention_dropout=0.0, **kwargs):
         super().__init__(*args, **kwargs)
@@ -379,6 +388,36 @@ class ErnieStudent(ErnieEncoder):
         logits = ops.linear_bf16(pooled, F.pad(self.cls_w, (0, 0, 0, pad)).to(bf), F.pad(self.cls_b, (0, pad)))
         return logits[:, :n].float()
 
+
+    def forward_packed(self, ids, pos, seg, cu_seqlens, max_len, key_mask=None):
+        """The training forward over packed sequences, with the arguments ``pack_sequences`` returns: ids / pos / seg
+        int64 [T], ``cu_seqlens`` int32 [B + 1], ``max_len`` (host int) the longest length, ``key_mask`` uint8 [T] or
+        None.  Returns fp32 logits [B, num_labels] with a gradient; the padded ``forward`` of the same batch up to the
+        order of floating-point sums.  On CUDA the inputs are expected on the model's device; nothing reads back to the
+        host under CUDA-graph capture, so a step can be captured for a fixed T and cu_seqlens.  Under
+        ``torch.no_grad()`` at p = 0 the logits are those of ``ErnieEncoder.forward_packed``."""
+        dev = self.word_emb.device
+        ids, pos, seg, cu_seqlens = (t.to(dev) for t in (ids, pos, seg, cu_seqlens))
+        key_mask = None if key_mask is None else key_mask.to(dev)
+        hd, ad = (self.hidden_dropout, self.attention_dropout) if self.training else (0.0, 0.0)
+        x = ops.embedding_layernorm_trainable(ids, pos, seg, self.word_emb, self.pos_emb, self.seg_emb, self.emb_ln_g,
+                                              self.emb_ln_b, self.eps, dropout_p=hd)
+        for lyr in self.layers:
+            h = ops.attention_block_varlen(x, lyr.qkv_w, lyr.qkv_b, lyr.out_w, lyr.out_b, cu_seqlens, max_len,
+                                           self.heads, key_mask, attn_dropout=ad, hidden_dropout=hd)
+            x = ops.layer_norm_trainable(h, lyr.ln1_g, lyr.ln1_b, self.eps)
+            h = ops.gelu_ffn(x, lyr.ffn1_w, lyr.ffn1_b, lyr.ffn2_w, lyr.ffn2_b, dropout_p=hd)
+            x = ops.layer_norm_trainable(h, lyr.ln2_g, lyr.ln2_b, self.eps)
+        cls = x.index_select(0, cu_seqlens[:-1].long())
+        if not self.word_emb.is_cuda:
+            pooled = ops.dropout(torch.tanh(F.linear(cls, self.pool_w, self.pool_b)), hd)
+            return F.linear(pooled, self.cls_w, self.cls_b)
+        bf = torch.bfloat16
+        pooled = ops.dropout(torch.tanh(ops.linear_bf16(cls, self.pool_w.to(bf), self.pool_b)), hd)
+        n = self.num_labels
+        pad = max(CLS_PAD, -(-n // CLS_PAD) * CLS_PAD) - n
+        logits = ops.linear_bf16(pooled, F.pad(self.cls_w, (0, 0, 0, pad)).to(bf), F.pad(self.cls_b, (0, pad)))
+        return logits[:, :n].float()
 
     def _forward_dropout_cpu(self, ids, pos, seg, keep, hd, ad):
         """The float32 training forward on CPU with dropout at the documented sites (F.dropout masks)."""

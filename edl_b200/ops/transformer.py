@@ -28,6 +28,7 @@ def _count(reason):
 # (floor(n / 4)_lo, floor(n / 4)_hi, offset_lo, offset_hi) is >= floor(p * 2^32); kept elements are scaled by
 # fp32(1 / (1 - p)).  The kernels evaluate the same rule (csrc/philox.cuh).  On CPU the sites use F.dropout.
 _M32 = 0xFFFFFFFF
+_ATTN_MAX_LEN = 512            # kAttnMaxLen: the row stride of the packed attention-probability index
 _PHILOX_M = (0xD2511F53, 0xCD9E8D57)
 _PHILOX_W = (0x9E3779B9, 0xBB67AE85)
 
@@ -70,7 +71,13 @@ def _keep(seed, offset, index, threshold):
 def dropout_keep_reference(seed, offset, index, p):
     """The keep mask (bool, index's shape and device) of a dropout site with generator state (seed, offset) at the flat
     element indices ``index`` (int64 tensor), in torch int64 arithmetic on any device.  The single host-side statement
-    of the rule the kernels use; the scale of a kept element is ``fp32(1 / (1 - p))``."""
+    of the rule the kernels use; the scale of a kept element is ``fp32(1 / (1 - p))``.
+
+    The flat index of each site: attention probability (b, h, i, j) at ((b H + h) L + i) L + j in the padded layout
+    [B, L], and at ((b H + h) 512 + i) 512 + j for packed sequences (the fixed stride 512, the longest sequence the
+    kernels take, keeps the sequences' index ranges disjoint whatever their lengths); a row-wise site (residual
+    branches, embedding-LayerNorm output) at row * C + col, padded or packed rows alike; the pooled features at
+    b * C + col."""
     p = _check_p(p)
     return _keep(int(seed), int(offset), index, int(p * 4294967296.0))
 
@@ -102,6 +109,30 @@ def _site_z(t, p, shape):
     if not t.is_cuda:
         return torch.nn.functional.dropout(torch.ones(shape, dtype=torch.float32), p, True)
     return _fallback_z(_draw(t.device, p), shape, t.device)
+
+
+def _varlen_site_z(t, p, cu_seqlens, max_len, heads):
+    """Z of the attention-probability site of a packed batch on the float32 reference path, as a list of per-sequence
+    [1, H, len_b, len_b] tensors: None at p = 0; on CUDA the kernels' mask (one generator draw), element (b, h, i, j)
+    at ((b H + h) 512 + i) 512 + j; on CPU the blocks [b, :, :len_b, :len_b] of one F.dropout mask of
+    [B, H, max_len, max_len]."""
+    if p == 0.0:
+        return None
+    cu = [int(v) for v in cu_seqlens.tolist()]
+    lens = [e - s for s, e in zip(cu[:-1], cu[1:])]
+    if not t.is_cuda:
+        z = torch.nn.functional.dropout(torch.ones((len(lens), heads, max_len, max_len)), p, True)
+        return [z[b:b + 1, :, :n, :n] for b, n in enumerate(lens)]
+    drop = _draw(t.device, p)
+    if drop.captured:
+        raise RuntimeError("dropout: the float32 fallback cannot be captured in a CUDA graph")
+    out = []
+    for b, n in enumerate(lens):
+        i = torch.arange(n, device=t.device, dtype=torch.int64)
+        h = torch.arange(heads, device=t.device, dtype=torch.int64)
+        idx = (((b * heads + h).view(-1, 1, 1) * _ATTN_MAX_LEN + i.view(1, -1, 1)) * _ATTN_MAX_LEN + i.view(1, 1, -1))
+        out.append((_keep(drop.seed, drop.offset, idx, drop.threshold).float() * drop.scale).unsqueeze(0))
+    return out
 
 
 def _dropout_apply(x, drop):
@@ -191,16 +222,18 @@ def attention(qkv, mask, batch, seq_len, heads, head_dim=64, out=None):
 
 
 # ----------------------------------------------------------------------------------------- variable-length attention
-def attention_varlen_reference(qkv, cu_seqlens, max_len, heads, key_mask=None):
+def attention_varlen_reference(qkv, cu_seqlens, max_len, heads, key_mask=None, drop_z=None):
     """Float32 math of ``attention_varlen``: ``attention_reference`` on each packed sequence.  Rows outside every
-    sequence are 0 (the kernel does not write them)."""
+    sequence are 0 (the kernel does not write them).  ``drop_z``: per sequence b a [1, H, len_b, len_b] dropout
+    (keep * scale) on its probabilities, or None."""
     d = qkv.shape[1] // (3 * heads)
     cu = [int(v) for v in cu_seqlens.tolist()]
     out = torch.zeros((qkv.shape[0], heads * d), device=qkv.device, dtype=qkv.dtype)
-    for s, e in zip(cu[:-1], cu[1:]):
+    for b, (s, e) in enumerate(zip(cu[:-1], cu[1:])):
         if e > s:
             m = None if key_mask is None else key_mask[s:e].view(1, e - s)
-            out[s:e] = attention_reference(qkv[s:e], m, 1, e - s, heads, d)
+            z = None if drop_z is None else drop_z[b]
+            out[s:e] = attention_reference(qkv[s:e], m, 1, e - s, heads, d, z)
     return out
 
 
@@ -241,7 +274,7 @@ def attention_varlen(qkv, cu_seqlens, max_len, heads, key_mask=None, out=None):
         km = key_mask if (key_mask.dtype == torch.uint8 and key_mask.is_contiguous()) else \
             (key_mask != 0).to(torch.uint8).contiguous()
     maps = torch.empty(b * 256, device=qkv.device, dtype=torch.uint8)        # two 128-byte tensor maps per sequence
-    native().attention_varlen_fwd(qkv, cu, km, out, maps, int(max_len), heads)
+    native().attention_varlen_fwd(qkv, cu, km, out, maps, int(max_len), heads, None, None)
     count_launch(2)
     return out
 
@@ -462,10 +495,72 @@ def attention_backward(qkv, mask, out, lse, dout, batch, seq_len, heads, drop=No
     return dqkv
 
 
+def attention_varlen_forward_saved(qkv, cu_seqlens, max_len, heads, key_mask=None, drop=None):
+    """The packed kernel forward with the statistics the backward needs: (out bf16 [T, H * 64], lse fp32 [H, T], lse
+    of head h and packed row r at [h, r]).  ``drop``: a drawn dropout site for the probabilities, element (b, h, i, j) at
+    ((b H + h) 512 + i) 512 + j; lse is that of the undropped softmax.  ``cu_seqlens`` int32 and ``key_mask`` uint8 (or
+    None), contiguous, on qkv's device."""
+    from . import native, count_launch
+
+    t = qkv.shape[0]
+    out = torch.empty((t, heads * 64), device=qkv.device, dtype=torch.bfloat16)
+    lse = torch.empty((heads, t), device=qkv.device, dtype=torch.float32)
+    maps = torch.empty((cu_seqlens.numel() - 1) * 256, device=qkv.device, dtype=torch.uint8)
+    native().attention_varlen_fwd(qkv, cu_seqlens, key_mask, out, maps, int(max_len), heads, lse, drop)
+    count_launch(2)
+    return out, lse
+
+
+def attention_varlen_backward(qkv, cu_seqlens, max_len, heads, key_mask, out, lse, dout, drop=None):
+    """dqkv bf16 [T, 3 * H * 64] of ``attention_varlen`` from the forward's ``out`` and ``lse``
+    (``attention_varlen_forward_saved``, with the same ``drop``) and the output gradient ``dout``.  Every row must
+    belong to a sequence (cu_seqlens[-1] == T, as ``pack_sequences`` makes it): rows outside all sequences are not
+    written."""
+    from . import native, count_launch
+
+    dqkv = torch.empty_like(qkv)
+    delta = torch.empty((heads, qkv.shape[0]), device=qkv.device, dtype=torch.float32)
+    native().attention_varlen_bwd(qkv, cu_seqlens, key_mask, out, lse, _bf16(dout).contiguous(), dqkv, delta,
+                                  int(max_len), heads, drop)
+    count_launch(3)
+    return dqkv
+
+
 def _mask_u8(mask, device):
     if mask is None:
         return None
     return mask if (mask.dtype == torch.uint8 and mask.is_contiguous()) else (mask != 0).to(torch.uint8).contiguous()
+
+
+def _cu_i32(cu_seqlens):
+    return cu_seqlens if (cu_seqlens.dtype == torch.int32 and cu_seqlens.is_contiguous()) else \
+        cu_seqlens.to(torch.int32).contiguous()
+
+
+class _Padded:
+    """The padded layout of the attention kernels: ``mask`` uint8 [B, L] or None, rows b * L + i."""
+
+    def __init__(self, mask, batch, seq_len):
+        self.mask, self.batch, self.seq_len = mask, batch, seq_len
+
+    def forward(self, qkv, heads, drop):
+        return attention_forward_saved(qkv, self.mask, self.batch, self.seq_len, heads, drop)
+
+    def backward(self, qkv, out, lse, dout, heads, drop):
+        return attention_backward(qkv, self.mask, out, lse, dout, self.batch, self.seq_len, heads, drop)
+
+
+class _Packed:
+    """Sequences packed back to back: ``cu_seqlens`` int32 [B + 1], host ``max_len``, ``key_mask`` uint8 [T] or None."""
+
+    def __init__(self, cu_seqlens, max_len, key_mask):
+        self.cu_seqlens, self.max_len, self.key_mask = cu_seqlens, int(max_len), key_mask
+
+    def forward(self, qkv, heads, drop):
+        return attention_varlen_forward_saved(qkv, self.cu_seqlens, self.max_len, heads, self.key_mask, drop)
+
+    def backward(self, qkv, out, lse, dout, heads, drop):
+        return attention_varlen_backward(qkv, self.cu_seqlens, self.max_len, heads, self.key_mask, out, lse, dout, drop)
 
 
 class _AttentionFn(torch.autograd.Function):
@@ -481,6 +576,39 @@ class _AttentionFn(torch.autograd.Function):
     def backward(ctx, dout):
         qkv, mask, out, lse = ctx.saved_tensors
         return attention_backward(qkv, mask, out, lse, dout, *ctx.shape, ctx.drop), None, None, None, None, None
+
+
+class _AttentionVarlenFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, qkv, layout, heads, drop):
+        qkv = _bf16(qkv).contiguous()
+        out, lse = layout.forward(qkv, heads, drop)
+        ctx.save_for_backward(qkv, out, lse)
+        ctx.layout, ctx.heads, ctx.drop = layout, heads, drop
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        qkv, out, lse = ctx.saved_tensors
+        return ctx.layout.backward(qkv, out, lse, dout, ctx.heads, ctx.drop), None, None, None
+
+
+def attention_varlen_trainable(qkv, cu_seqlens, max_len, heads, key_mask=None, dropout_p=0.0):
+    """``attention_varlen`` with a gradient, the packed sibling of ``attention_trainable``: the kernel path saves lse
+    [H, T] and runs the packed backward of attention_bwd.cu.  ``qkv`` [T, 3 * H * 64] with every row inside a sequence
+    (cu_seqlens[-1] == T).  ``dropout_p``: dropout on the attention probabilities (one site, index
+    ((b H + h) 512 + i) 512 + j).  On CPU, and for a shape the kernels do not take, ``attention_varlen_reference`` runs
+    under autograd (counted through ``count_fallback`` on CUDA)."""
+    p = _check_p(dropout_p)
+    if qkv.is_cuda and attention_varlen_supported(_bf16(qkv).contiguous(), cu_seqlens, max_len, heads) \
+            and qkv.shape[1] == 3 * heads * 64:
+        layout = _Packed(_cu_i32(cu_seqlens), max_len, _mask_u8(key_mask, qkv.device))
+        return _AttentionVarlenFn.apply(qkv, layout, heads, _draw(qkv.device, p) if p > 0.0 else None)
+    if qkv.is_cuda:
+        _count("attention_varlen: no training kernel for T %d, B %d, max_len %d, H %d, width %d: float32 math on the "
+               "library" % (qkv.shape[0], cu_seqlens.numel() - 1, max_len, heads, qkv.shape[-1]))
+    z = _varlen_site_z(qkv, p, cu_seqlens, max_len, heads)
+    return attention_varlen_reference(qkv.float(), cu_seqlens, max_len, heads, key_mask, z)
 
 
 def attention_trainable(qkv, mask, batch, seq_len, heads, head_dim=64, dropout_p=0.0):
@@ -500,37 +628,38 @@ def attention_trainable(qkv, mask, batch, seq_len, heads, head_dim=64, dropout_p
 class _AttentionBlockFn(torch.autograd.Function):
     """h = attention(x W_qkv^T + b_qkv) W_o^T + b_o + x, the attention half of a post-LN encoder layer before its
     LayerNorm.  Backward: dctx = dh W_o, dqkv by attention_bwd.cu, and dx = dqkv W_qkv + dh as ONE dgrad GEMM with the
-    residual gradient as its fused addend; dW_qkv and dW_o through ``_wgrad``.
+    residual gradient as its fused addend; dW_qkv and dW_o through ``_wgrad``.  ``layout`` (``_Padded`` or ``_Packed``)
+    picks the attention forward / backward pair; everything else is row-wise and the same for both.
 
     ``drops`` = (attention-probability site, output-branch site), each None at p = 0.  With the branch dropout the output
     projection's epilogue stores x + Z o (o W_o^T + b_o); the backward forms dh_b = Z o dh (dropout.cu) for dctx, dW_o
     and db_o, while the residual still receives dh."""
 
     @staticmethod
-    def forward(ctx, x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, sinks, drops):
+    def forward(ctx, x, qkv_w, qkv_b, out_w, out_b, layout, heads, sinks, drops):
         from .gemm import gemm_bf16, gemm_bf16_residual_dropout
 
         x = _bf16(x).contiguous()
         wq, wo = _bf16(qkv_w).contiguous(), _bf16(out_w).contiguous()
         qkv = gemm_bf16(x, wq, col_shift=qkv_b.float())
-        o, lse = attention_forward_saved(qkv, mask, batch, seq_len, heads, drops[0])
+        o, lse = layout.forward(qkv, heads, drops[0])
         if drops[1] is None:
             h = gemm_bf16(o, wo, col_shift=out_b.float(), add=x)
         else:
             h = gemm_bf16_residual_dropout(o, wo, out_b, x, drops[1])
-        ctx.save_for_backward(x, wq, wo, qkv, o, lse, mask, qkv_w, qkv_b, out_w, out_b)
-        ctx.shape, ctx.sinks, ctx.drops = (batch, seq_len, heads), sinks, drops
+        ctx.save_for_backward(x, wq, wo, qkv, o, lse, qkv_w, qkv_b, out_w, out_b)
+        ctx.layout, ctx.heads, ctx.sinks, ctx.drops = layout, heads, sinks, drops
         return h
 
     @staticmethod
     def backward(ctx, dh):
         from .gemm import gemm_bf16
 
-        x, wq, wo, qkv, o, lse, mask, qkv_w, qkv_b, out_w, out_b = ctx.saved_tensors
+        x, wq, wo, qkv, o, lse, qkv_w, qkv_b, out_w, out_b = ctx.saved_tensors
         dh = _bf16(dh).contiguous()
         dhb = dh if ctx.drops[1] is None else _dropout_apply(dh, ctx.drops[1])
         dctx = gemm_bf16(dhb, wo, b_mn_major=True)
-        dqkv = attention_backward(qkv, mask, o, lse, dctx, *ctx.shape, ctx.drops[0])
+        dqkv = ctx.layout.backward(qkv, o, lse, dctx, ctx.heads, ctx.drops[0])
         dx = gemm_bf16(dqkv, wq, b_mn_major=True, add=dh) if ctx.needs_input_grad[0] else None
         s = ctx.sinks
         g = [None] * 4
@@ -542,18 +671,32 @@ class _AttentionBlockFn(torch.autograd.Function):
             g[2] = _wgrad_to(dhb, o, out_w, s[2])
         if ctx.needs_input_grad[4]:
             g[3] = _bias_grad(dhb.float().sum(0), out_b, s[3])
-        return (dx, *g, None, None, None, None, None, None)
+        return (dx, *g, None, None, None, None)
+
+
+def _block_reference(x, qkv_w, qkv_b, out_w, out_b, attend, hidden_z):
+    f = torch.float32
+    xf = x.float()
+    qkv = torch.nn.functional.linear(xf, qkv_w.to(f), qkv_b.to(f))
+    h = torch.nn.functional.linear(attend(qkv), out_w.to(f), out_b.to(f))
+    return (h if hidden_z is None else hidden_z * h) + xf
 
 
 def attention_block_reference(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, attn_z=None, hidden_z=None):
     """Float32 math of ``attention_block``; ``attn_z`` [B, H, L, L] / ``hidden_z`` [B * L, C]: dropout (keep * scale)
     on the probabilities and on the output branch."""
-    f = torch.float32
-    xf = x.float()
-    qkv = torch.nn.functional.linear(xf, qkv_w.to(f), qkv_b.to(f))
-    o = attention_reference(qkv, mask, batch, seq_len, heads, qkv_w.shape[0] // (3 * heads), attn_z)
-    h = torch.nn.functional.linear(o, out_w.to(f), out_b.to(f))
-    return (h if hidden_z is None else hidden_z * h) + xf
+    d = qkv_w.shape[0] // (3 * heads)
+    return _block_reference(x, qkv_w, qkv_b, out_w, out_b,
+                            lambda qkv: attention_reference(qkv, mask, batch, seq_len, heads, d, attn_z), hidden_z)
+
+
+def attention_block_varlen_reference(x, qkv_w, qkv_b, out_w, out_b, cu_seqlens, max_len, heads, key_mask=None,
+                                     attn_z=None, hidden_z=None):
+    """Float32 math of ``attention_block_varlen``; ``attn_z``: per-sequence probability dropout as in
+    ``attention_varlen_reference``, ``hidden_z`` [T, C]: the output-branch dropout."""
+    return _block_reference(x, qkv_w, qkv_b, out_w, out_b,
+                            lambda qkv: attention_varlen_reference(qkv, cu_seqlens, max_len, heads, key_mask, attn_z),
+                            hidden_z)
 
 
 def attention_block(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, attn_dropout=0.0, hidden_dropout=0.0):
@@ -569,14 +712,47 @@ def attention_block(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, 
     if x.is_cuda and c % 8 == 0 and c == heads * 64 and attention_train_supported(x, batch, seq_len, heads):
         sinks = tuple(_grad_sink(p) for p in (qkv_w, qkv_b, out_w, out_b))
         drops = tuple(_draw(x.device, p) if p > 0.0 else None for p in (pa, ph))
-        return _AttentionBlockFn.apply(x, qkv_w, qkv_b, out_w, out_b, _mask_u8(mask, x.device), batch, seq_len, heads,
-                                       sinks, drops)
+        return _AttentionBlockFn.apply(x, qkv_w, qkv_b, out_w, out_b,
+                                       _Padded(_mask_u8(mask, x.device), batch, seq_len), heads, sinks, drops)
     if x.is_cuda:
         _count("attention_block: no kernel for B %d, L %d, H %d, width %d: float32 math on the library"
                % (batch, seq_len, heads, c))
     za = _site_z(x, pa, (batch, heads, seq_len, seq_len))
     zh = _site_z(x, ph, (x.shape[0], c))
     return attention_block_reference(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, za, zh)
+
+
+def attention_block_varlen(x, qkv_w, qkv_b, out_w, out_b, cu_seqlens, max_len, heads, key_mask=None,
+                           attn_dropout=0.0, hidden_dropout=0.0):
+    """``attention_block`` on sequences packed back to back: x [T, C] holds the real tokens only, sequence b in rows
+    [cu_seqlens[b], cu_seqlens[b + 1]) (every row inside a sequence, as ``pack_sequences`` makes them), ``max_len``
+    (host int) at least the longest length, ``key_mask`` [T] (nonzero = attend) or None.  The same GEMMs, fused residual
+    gradient and weight-gradient hand-off as the padded form; attention runs the packed kernels.  Dropout sites as in
+    ``attention_block``: the probabilities at ((b H + h) 512 + i) 512 + j, then the output branch at row * C + col.
+    Nothing reads back to the host on the kernel path."""
+    from .gemm import _grad_sink
+
+    pa, ph = _check_p(attn_dropout), _check_p(hidden_dropout)
+    c = x.shape[-1]
+    if (x.is_cuda and x.dim() == 2 and c % 8 == 0 and c == heads * 64 and cu_seqlens.is_cuda
+            and cu_seqlens.dim() == 1 and cu_seqlens.numel() >= 2):
+        from . import native
+
+        ok = native().attention_varlen_supported(x.shape[0], cu_seqlens.numel() - 1, int(max_len), heads, 64)
+    else:
+        ok = False
+    if ok:
+        sinks = tuple(_grad_sink(p) for p in (qkv_w, qkv_b, out_w, out_b))
+        drops = tuple(_draw(x.device, p) if p > 0.0 else None for p in (pa, ph))
+        layout = _Packed(_cu_i32(cu_seqlens), max_len, _mask_u8(key_mask, x.device))
+        return _AttentionBlockFn.apply(x, qkv_w, qkv_b, out_w, out_b, layout, heads, sinks, drops)
+    if x.is_cuda:
+        _count("attention_block_varlen: no kernel for T %d, B %d, max_len %d, H %d, width %d: float32 math on the "
+               "library" % (x.shape[0], cu_seqlens.numel() - 1, max_len, heads, c))
+    za = _varlen_site_z(x, pa, cu_seqlens, max_len, heads)
+    zh = _site_z(x, ph, (x.shape[0], c))
+    return attention_block_varlen_reference(x, qkv_w, qkv_b, out_w, out_b, cu_seqlens, max_len, heads, key_mask, za,
+                                            zh)
 
 
 class _GeluFfnFn(torch.autograd.Function):

@@ -16,6 +16,9 @@ from paddle_edl.distill.teacher_server import TeacherServer  # noqa: E402
 from paddle_edl.models.small import BOW, BiLSTM, TextCNN, kl_distill_loss  # noqa: E402
 from paddle_edl.models.ernie import ernie_student  # noqa: E402
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from train import student_logits  # noqa: E402
+
 
 def corpus(n, vocab, seq, seed):
     rng = np.random.RandomState(seed)
@@ -34,7 +37,12 @@ def main():
     ap.add_argument("--epochs", type=int, default=2)
     ap.add_argument("--vocab", type=int, default=2000)
     ap.add_argument("--dropout", type=float, default=0.0, help="hidden and attention dropout of --model ernie")
+    ap.add_argument("--packed", action="store_true",
+                    help="--model ernie: the student trains on each batch packed to its real tokens (the teacher still "
+                         "receives the padded feeds)")
     args = ap.parse_args()
+    if args.packed and args.model != "ernie":
+        ap.error("--packed needs --model ernie")
     srv = None
     if not args.teachers:
         teacher = TextCNN(args.vocab).eval()
@@ -63,7 +71,7 @@ def main():
     reader = dr.set_batch_generator(batch_gen)
     for epoch in range(args.epochs):
         for i, (ids, label, t_logits) in enumerate(reader()):
-            logits = student(torch.from_numpy(ids).to(dev))
+            logits = student_logits(student, ids, dev, args.packed)
             loss = kl_distill_loss(logits, torch.from_numpy(t_logits).to(dev), args.T) + \
                 torch.nn.functional.cross_entropy(logits, torch.from_numpy(label[:, 0]).to(dev))
             opt.zero_grad()

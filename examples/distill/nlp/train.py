@@ -12,7 +12,7 @@ sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.abspath(os.path.join(HERE, "..", "..", "..")))
 from reader import TsvReader, batches, synthetic_corpus  # noqa: E402
 from paddle_edl.models.small import BOW, BiLSTM, TextCNN  # noqa: E402
-from paddle_edl.models.ernie import ernie_student  # noqa: E402
+from paddle_edl.models.ernie import ernie_student, pack_sequences  # noqa: E402
 
 
 def build_model(name, vocab, dropout=0.0):
@@ -23,6 +23,19 @@ def build_model(name, vocab, dropout=0.0):
         dev = torch.device("cuda" if torch.cuda.is_available() else "cpu")
         return (BiLSTM(vocab) if name == "lstm" else ernie_student(dropout=dropout)).to(dev), dev
     return (BOW(vocab) if name == "bow" else TextCNN(vocab)), torch.device("cpu")
+
+
+def student_logits(model, ids, dev, packed=False):
+    """The student's logits for a padded id batch.  ``packed`` (Transformer student only): pack the batch to its real
+    tokens (``pack_sequences`` of the feeds built from the ids: positions 0.., segment 0, mask ids != 0) and run
+    ``forward_packed``, so no GEMM, LayerNorm or attention tile works on padding."""
+    t = torch.from_numpy(ids)
+    if not packed:
+        return model(t.to(dev))
+    b, l = t.shape
+    ids_p, pos, seg, cu, max_len, key_mask = pack_sequences(t, torch.arange(l).expand(b, l), torch.zeros_like(t), t != 0)
+    return model.forward_packed(ids_p.to(dev), pos.to(dev), seg.to(dev), cu.to(dev), max_len,
+                                None if key_mask is None else key_mask.to(dev))
 
 
 def evaluate(model, data, dev=torch.device("cpu")):
@@ -47,7 +60,11 @@ def main():
     ap.add_argument("--seq_len", type=int, default=64)
     ap.add_argument("--samples", type=int, default=1024)
     ap.add_argument("--dropout", type=float, default=0.0, help="hidden and attention dropout of --model ernie")
+    ap.add_argument("--packed", action="store_true",
+                    help="--model ernie: train on each batch packed to its real tokens (forward_packed)")
     args = ap.parse_args()
+    if args.packed and args.model != "ernie":
+        ap.error("--packed needs --model ernie")
     if args.train_tsv:
         tr = TsvReader(args.train_tsv, seq_len=args.seq_len)
         dev = TsvReader(args.dev_tsv or args.train_tsv, vocab=tr.vocab, seq_len=args.seq_len)
@@ -62,7 +79,7 @@ def main():
     opt = torch.optim.AdamW(model.parameters(), 1e-4 if args.model == "ernie" else 1e-3)   # a Transformer wants less
     for ep in range(args.epochs):
         for ids, label in train_iter(ep):
-            loss = torch.nn.functional.cross_entropy(model(torch.from_numpy(ids).to(dev)),
+            loss = torch.nn.functional.cross_entropy(student_logits(model, ids, dev, args.packed),
                                                      torch.from_numpy(label[:, 0]).to(dev))
             opt.zero_grad()
             loss.backward()

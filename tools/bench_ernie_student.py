@@ -4,20 +4,24 @@ AdamW) at B = 32, L = 128 with the student configuration (hidden 384, 4 layers, 
 on the package's kernels, against the same bf16 model in torch (cuBLAS linears, F.scaled_dot_product_attention with
 the key mask, F.layer_norm, F.gelu), both as CUDA-graph replays; and the attention backward alone against SDPA's
 backward, eager.  With ``--dropout p`` it times instead three training steps with hidden and attention dropout: ours at
-p, ours at 0, and the bf16 torch model with F.dropout at the same sites and SDPA's dropout_p = p.  All times come from
-CUDA events.  Prints the GPU name and power limit with the numbers."""
+p, ours at 0, and the bf16 torch model with F.dropout at the same sites and SDPA's dropout_p = p.  With ``--packed
+MIN_LEN`` the sample lengths are drawn uniformly from [MIN_LEN, seq] (fixed seed) and it times three steps on that
+batch and the same weights: ours padded (``forward``), ours packed (``forward_packed`` on ``pack_sequences`` of the
+batch) and torch padded; it also reports the real-token fraction and the host time of ``pack_sequences`` per batch.
+All GPU times come from CUDA events.  Prints the GPU name and power limit with the numbers."""
 import argparse
 import json
 import os
 import subprocess
 import sys
+import time
 
 import torch
 import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from edl_b200 import ops  # noqa: E402
-from edl_b200.models.ernie import ernie_student  # noqa: E402
+from edl_b200.models.ernie import ernie_student, pack_sequences  # noqa: E402
 
 
 def gpu_info():
@@ -93,14 +97,22 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--dropout", type=float, default=None, help="time training steps with this dropout instead")
+    ap.add_argument("--packed", type=int, default=None, metavar="MIN_LEN",
+                    help="lengths uniform in [MIN_LEN, seq]: time the padded step, the packed step and torch")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_ernie_student: needs a GPU")
+    if args.packed is not None and not 1 <= args.packed <= args.seq:
+        sys.exit("bench_ernie_student: --packed MIN_LEN needs 1 <= MIN_LEN <= --seq")
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
     b, l = args.batch, args.seq
     ids = torch.randint(1, 18000, (b, l), device=dev)
-    ids[torch.arange(l, device=dev).unsqueeze(0) >= torch.randint(l // 2, l + 1, (b, 1), device=dev)] = 0
+    if args.packed is None:
+        lens = torch.randint(l // 2, l + 1, (b, 1), device=dev)
+    else:                                                # a fixed batch whatever the device's RNG state
+        lens = torch.randint(args.packed, l + 1, (b, 1), generator=torch.Generator().manual_seed(1234)).to(dev)
+    ids[torch.arange(l, device=dev).unsqueeze(0) >= lens] = 0
     label = torch.randint(0, 2, (b,), device=dev)
     keep = ids != 0
 
@@ -122,6 +134,8 @@ def main():
 
     if args.dropout is not None:
         return bench_dropout(args, ours, opt, ref, ropt, ids, label, keep)
+    if args.packed is not None:
+        return bench_packed(args, ours, opt, step_ours, step_torch, ids, label)
     ops.reset_fallbacks()
     t_ours = graph_time(step_ours, args.warmup, args.iters)
     fallbacks = ops.fallbacks()
@@ -177,6 +191,40 @@ def bench_dropout(args, ours, opt, ref, ropt, ids, label, keep):
                       "train_step_ms": {k: round(v, 3) for k, v in med.items()},
                       "dropout_overhead": round(med["ours_p"] / med["ours_0"] - 1.0, 4),
                       "fallbacks": ops.fallbacks()}))
+
+
+def bench_packed(args, ours, opt, step_ours, step_torch, ids, label):
+    """The padded step, the packed step and torch's padded step on one batch, CUDA-graph replays alternated over five
+    rounds (medians); the packed step's graph is fixed to this batch's T and cu_seqlens."""
+    b, l = ids.shape
+    feeds = (ids.cpu(), torch.arange(l).expand(b, l), torch.zeros(b, l, dtype=torch.int64), (ids != 0).cpu())
+    n_pack = 200
+    t0 = time.perf_counter()
+    for _ in range(n_pack):
+        pk = pack_sequences(*feeds)
+    pack_ms = (time.perf_counter() - t0) * 1e3 / n_pack
+    dev = ids.device
+    pk = tuple(t.to(dev) if torch.is_tensor(t) else t for t in pk)
+    tokens = pk[0].numel()
+
+    def step_packed():
+        opt.zero_grad(set_to_none=False)
+        F.cross_entropy(ours.forward_packed(*pk), label).backward()
+        opt.step()
+
+    ops.reset_fallbacks()
+    arms = {"ours_padded": step_ours, "ours_packed": step_packed, "torch_bf16_padded": step_torch}
+    times = {k: [] for k in arms}
+    for _ in range(5):
+        for k, fn in arms.items():
+            times[k].append(graph_time(fn, args.warmup, args.iters))
+    med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
+    name, limit = gpu_info()
+    print(json.dumps({"gpu": name, "power_limit": limit, "batch": b, "seq": l, "min_len": args.packed,
+                      "tokens": tokens, "token_fraction": round(tokens / (b * l), 4),
+                      "train_step_ms": {k: round(v, 3) for k, v in med.items()},
+                      "packed_speedup_vs_padded": round(med["ours_padded"] / med["ours_packed"], 3),
+                      "pack_sequences_host_ms": round(pack_ms, 3), "fallbacks": ops.fallbacks()}))
 
 
 if __name__ == "__main__":
