@@ -215,8 +215,8 @@ def _deliver_wgrad(dy, x, sink, ready, compute):
 
 
 def _wgrad(dy2, x2, weight_shape, sink, ready):
-    """dW[Cout, Cin] = dy2[M, Cout]^T @ x2[M, Cin], written as bf16 straight into the (flat gradient bucket) sink --
-    no memset / cast / add kernels around it."""
+    """dW[Cout, Cin] = dy2[M, Cout]^T @ x2[M, Cin], written as bf16 straight into a bf16 (flat gradient bucket) sink --
+    no memset / cast / add kernels around it; a sink of another dtype gets the bf16 result added."""
     return _deliver_wgrad(dy2, x2, sink, ready, lambda s: _wgrad_impl(dy2, x2, weight_shape, s))
 
 
@@ -226,14 +226,20 @@ def _wgrad_impl(dy2, x2, weight_shape, sink, split_k: Optional[int] = None):
     cout, cin = dy2.shape[1], x2.shape[1]
     if dy2.is_cuda and _tma_compatible(dy2, x2, None, cin):
         split = split_k if split_k is not None else _split_k_for(cout, cin, dy2.shape[0])
-        out = sink.view(cout, cin) if sink is not None else torch.empty((cout, cin), device=dy2.device,
-                                                                        dtype=torch.bfloat16)
+        # a bf16 sink takes the kernel's accumulating store; any other sink (the fp32 master parameters of the
+        # Transformer student) receives the bf16 gradient the sink-less path returns, added in the sink's dtype
+        direct = sink is not None and sink.dtype == torch.bfloat16
+        out = sink.view(cout, cin) if direct else torch.empty((cout, cin), device=dy2.device, dtype=torch.bfloat16)
         block_n = 64 if cin <= 64 else 128      # the kernel's tile width (csrc/gemm.cu)
         tiles = ((cout + 127) // 128) * ((cin + block_n - 1) // block_n)
         partials = _splitk_partials(dy2.device, split * tiles * 128 * block_n) if split > 1 else None
-        native().gemm_wgrad_bf16(dy2, x2, out, split, sink is not None, partials)
+        native().gemm_wgrad_bf16(dy2, x2, out, split, direct, partials)
         count_launch()
-        return None if sink is not None else out.view(weight_shape)
+        if sink is None:
+            return out.view(weight_shape)
+        if not direct:
+            sink.view(cout, cin).add_(out)
+        return None
     if dy2.is_cuda:
         from . import count_fallback
         count_fallback("gemm_bf16: operand not TMA-describable (pitch / base not 16-byte aligned or not bf16): "

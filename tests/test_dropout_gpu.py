@@ -25,6 +25,7 @@ import torch.nn.functional as F
 from edl_b200 import ops
 from edl_b200.models.ernie import ErnieStudent
 from edl_b200.ops.transformer import _draw
+from student_oracle import attention_f64 as _attention_f64, ln_f64 as _ln_f64
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda", 0)
@@ -104,33 +105,6 @@ def test_residual_dropout_epilogue(M, N):
     assert torch.equal(out[~kept], add[~kept])                         # a dropped element stores the residual
 
 
-def _attention_f64(qkv, mask, do, b, l, h, z):
-    """O, dQ | dK | dV (float64) with dropout Z [B, H, L, L] on the probabilities, and the magnitudes of their errors."""
-    x = qkv.double().view(b, l, 3, h, 64)
-    q, k, v = (x[:, :, i].transpose(1, 2) for i in range(3))
-    dO = do.double().view(b, l, h, 64).transpose(1, 2)
-    keep = (mask != 0).view(b, 1, 1, l)
-    s = ((q @ k.transpose(-1, -2)) / 8).masked_fill(~keep, float("-inf"))
-    mx = s.amax(-1, keepdim=True)
-    e = torch.exp(s - torch.where(torch.isinf(mx), torch.zeros_like(mx), mx))
-    den = e.sum(-1, keepdim=True)
-    p = e / torch.where(den > 0, den, torch.ones_like(den))
-    pz = p * z
-    o = pz @ v
-    mo = pz @ v.abs()
-    dp = dO @ v.transpose(-1, -2)
-    ds = p * (z * dp - (dO * o).sum(-1, keepdim=True))
-    dq, dk, dv = ds @ k / 8, ds.transpose(-1, -2) @ q / 8, pz.transpose(-1, -2) @ dO
-    mds = p * (z * (dO.abs() @ v.abs().transpose(-1, -2)) + (dO.abs() * o.abs()).sum(-1, keepdim=True))
-    mq, mk, mv = mds @ k.abs() / 8, mds.transpose(-1, -2) @ q.abs() / 8, pz.transpose(-1, -2) @ dO.abs()
-
-    def flat(t):
-        return t.transpose(1, 2).reshape(b * l, h * 64)
-
-    return (flat(o), flat(mo), torch.cat([flat(dq), flat(dk), flat(dv)], 1),
-            torch.cat([flat(mq), flat(mk), flat(mv)], 1))
-
-
 @pytest.mark.parametrize("L", [1, 63, 64, 65, 128, 200, 512])
 def test_attention_dropout_f64_bounds(L):
     torch.manual_seed(L)
@@ -159,18 +133,6 @@ def test_attention_dropout_f64_bounds(L):
         o2, mo2, _, _ = _attention_f64(qkv, mask, do, b, L, h, zb)
         with pytest.raises(AssertionError):
             _check(out, o2, 2.0 ** -8 * o2.abs() + 2.0 ** -6 * mo2, "control")
-
-
-def _ln_f64(x, dy, gamma, eps):
-    x, dy, g = x.double(), dy.double(), gamma.double()
-    c = x.shape[1]
-    mean = x.mean(1, keepdim=True)
-    rstd = 1.0 / torch.sqrt(((x - mean) ** 2).mean(1, keepdim=True) + eps)
-    xh = (x - mean) * rstd
-    gg = dy * g
-    dx = rstd * (gg - gg.mean(1, keepdim=True) - xh * (gg * xh).mean(1, keepdim=True))
-    mag = rstd * (gg.abs() + gg.abs().mean(1, keepdim=True) + xh.abs() * (gg * xh).abs().mean(1, keepdim=True)) * c
-    return xh, dx, mag, (dy * xh).sum(0), (dy * xh).abs().sum(0), dy.sum(0), dy.abs().sum(0)
 
 
 @pytest.mark.parametrize("rows,C", [(5, 384), (4096, 384), (700, 768)])

@@ -37,6 +37,7 @@ import torch.nn.functional as F
 from edl_b200 import ops
 from edl_b200.models import ernie, teacher_zoo
 from f64_bounds import EPS32, check_bf16, gemm_ref, guarded, tau as gemm_tau
+from student_oracle import attention_ref, ln_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -47,28 +48,6 @@ DEV = torch.device("cuda", 0)
 
 
 # ------------------------------------------------------------------------------------------------------ attention
-def attention_ref(qkv, mask, b, l, h):
-    """(ref, slack) of the attention kernel's output [B * L, H * 64] in float64 (see the module docstring)."""
-    x = qkv.double().view(b, l, 3, h, 64)
-    q, k, v = (x[:, :, i].transpose(1, 2) for i in range(3))                       # [B, H, L, 64]
-    s = q @ k.transpose(-1, -2)
-    smag = q.abs() @ k.abs().transpose(-1, -2)
-    keep = (torch.ones(b, l, dtype=torch.bool, device=qkv.device) if mask is None else mask != 0).view(b, 1, 1, l)
-    c = math.log2(math.e) / 8
-    cs = (s * c).masked_fill(~keep, float("-inf"))
-    m = cs.amax(-1, keepdim=True)
-    w = torch.softmax((s / 8).masked_fill(~keep, float("-inf")), -1).nan_to_num(0.0)    # 2^(c s) = e^(s / 8)
-    ref = w @ v
-    wv = w @ v.abs()
-    delta = c * 5 * EPS32 * smag + EPS32 * (cs.abs() + (cs - m).abs())
-    eps_j = 2.0 ** -8 + 2.0 ** -21 + 1.01 * math.log(2) * delta
-    eps = eps_j.masked_fill(~keep, 0.0).amax(-1, keepdim=True)
-    n_tiles = -(-l // 64)
-    slack = (2 * eps / (1 - eps) + (8 * n_tiles + 32) * EPS32) * wv
-    flat = lambda t: t.transpose(1, 2).reshape(b * l, h * 64)                     # noqa: E731
-    return flat(ref), flat(slack)
-
-
 def _mask(kind, b, l, gen):
     if kind == "none":
         return None
@@ -112,21 +91,6 @@ def test_attention_vs_float64(batch, seq_len, heads):
 
 
 # ---------------------------------------------------------------------------------------------------- LayerNorm
-def ln_ref(x64, gamma, beta, eps, dx=None):
-    c = x64.shape[1]
-    mean = x64.mean(1, keepdim=True)
-    d = x64 - mean
-    rstd = torch.rsqrt(d.square().mean(1, keepdim=True) + eps)
-    g, b = gamma.double(), beta.double()
-    ref = d * rstd * g + b
-    dmu = c * EPS32 * x64.abs().mean(1, keepdim=True)
-    eps_r = (c + 2) * EPS32 / 2 + 2.0 ** -21 + (dmu * rstd).square() / 2
-    dxx = 0.0 if dx is None else dx
-    dxm = 0.0 if dx is None else dx.mean(1, keepdim=True)
-    slack = g.abs() * rstd * (dmu + dxm + dxx + d.abs() * eps_r) + 4 * EPS32 * (d.abs() * rstd * g.abs() + b.abs())
-    return ref, slack
-
-
 @pytest.mark.parametrize("c", [768, 40])
 @pytest.mark.parametrize("rows", [1, 13, 4099])
 def test_layer_norms_vs_float64(c, rows):

@@ -23,6 +23,7 @@ import torch
 
 from edl_b200 import ops
 from edl_b200.models.ernie import ErnieStudent
+from student_oracle import attention_f64, ln_f64
 from test_ernie_student_cpu import _functional_encoder
 
 pytestmark = pytest.mark.gpu
@@ -39,34 +40,6 @@ def _check(out, ref, bound, what):
     return ratio
 
 
-def _attention_f64(qkv, mask, do, b, l, h):
-    """dQ, dK, dV (float64) and the magnitudes of their rounding errors."""
-    x = qkv.double().view(b, l, 3, h, 64)
-    q, k, v = (x[:, :, i].transpose(1, 2) for i in range(3))           # [B, H, L, 64]
-    dO = do.double().view(b, l, h, 64).transpose(1, 2)
-    keep = (mask != 0).view(b, 1, 1, l)
-    s = (q @ k.transpose(-1, -2)) / 8
-    s = s.masked_fill(~keep, float("-inf"))
-    mx = s.amax(-1, keepdim=True)
-    mx = torch.where(torch.isinf(mx), torch.zeros_like(mx), mx)
-    e = torch.exp(s - mx)
-    den = e.sum(-1, keepdim=True)
-    p = e / torch.where(den > 0, den, torch.ones_like(den))
-    o = p @ v
-    dp = dO @ v.transpose(-1, -2)
-    dsum = (dO * o).sum(-1, keepdim=True)
-    ds = p * (dp - dsum)
-    dq, dk, dv = ds @ k / 8, ds.transpose(-1, -2) @ q / 8, p.transpose(-1, -2) @ dO
-    mds = p * (dO.abs() @ v.abs().transpose(-1, -2) + (dO.abs() * o.abs()).sum(-1, keepdim=True))
-    mq, mk = mds @ k.abs() / 8, mds.transpose(-1, -2) @ q.abs() / 8
-    mv = p.transpose(-1, -2) @ dO.abs()
-
-    def flat(t):
-        return t.transpose(1, 2).reshape(b * l, h * 64)
-
-    return torch.cat([flat(dq), flat(dk), flat(dv)], 1), torch.cat([flat(mq), flat(mk), flat(mv)], 1)
-
-
 @pytest.mark.parametrize("L", [1, 63, 64, 65, 128, 200, 512])
 def test_attention_backward_f64_bounds(L):
     torch.manual_seed(L)
@@ -80,7 +53,7 @@ def test_attention_backward_f64_bounds(L):
     out, lse = ops.transformer.attention_forward_saved(qkv, mask, b, L, h)
     assert torch.equal(out, ops.attention(qkv, mask, b, L, h))        # O bitwise unchanged by the saved statistics
     dqkv = ops.transformer.attention_backward(qkv, mask, out, lse, do, b, L, h)
-    ref, mag = _attention_f64(qkv, mask, do, b, L, h)
+    _, _, ref, mag = attention_f64(qkv, mask, do, b, L, h)
     _check(dqkv, ref, 2.0 ** -8 * ref.abs() + 2.0 ** -6 * mag, "attention dqkv L=%d" % L)
     has = (mask != 0).any(1)                                               # at L = 1 sample 1 has no valid key either
     assert (dqkv.view(b, L, -1)[~has] == 0).all()                     # no valid key: exactly zero gradients
@@ -100,21 +73,9 @@ def test_attention_backward_negative_control():
     dqkv = ops.transformer.attention_backward(qkv, mask, out, lse, do, b, L, h)
     bad = qkv.clone()
     bad[[3, 70]] = bad[[70, 3]]
-    ref, mag = _attention_f64(bad, mask, do, b, L, h)
+    _, _, ref, mag = attention_f64(bad, mask, do, b, L, h)
     with pytest.raises(AssertionError):
         _check(dqkv, ref, 2.0 ** -8 * ref.abs() + 2.0 ** -6 * mag, "control")
-
-
-def _ln_f64(x, dy, gamma, eps):
-    x, dy, g = x.double(), dy.double(), gamma.double()
-    c = x.shape[1]
-    mean = x.mean(1, keepdim=True)
-    rstd = 1.0 / torch.sqrt(((x - mean) ** 2).mean(1, keepdim=True) + eps)
-    xh = (x - mean) * rstd
-    gg = dy * g
-    dx = rstd * (gg - gg.mean(1, keepdim=True) - xh * (gg * xh).mean(1, keepdim=True))
-    mag = rstd * (gg.abs() + gg.abs().mean(1, keepdim=True) + xh.abs() * (gg * xh).abs().mean(1, keepdim=True)) * c
-    return dx, mag, (dy * xh).sum(0), (dy * xh).abs().sum(0), dy.sum(0), dy.abs().sum(0)
 
 
 @pytest.mark.parametrize("rows,C", [(1, 384), (77, 384), (4096, 384), (300, 1024), (33, 8), (2000, 136)])
@@ -129,7 +90,7 @@ def test_layernorm_backward_f64_bounds(rows, C):
     y = ops.layer_norm_trainable(xr, g, bt, 1e-12)
     assert torch.equal(y, ops.layer_norm(x, gamma, beta, 1e-12))
     y.backward(dy)
-    dx, mag, dg, mg, db, mb = _ln_f64(x, dy, gamma, 1e-12)
+    _, dx, mag, dg, mg, db, mb = ln_f64(x, dy, gamma, 1e-12)
     _check(xr.grad, dx, 2.0 ** -8 * dx.abs() + 2.0 ** -16 * mag, "LayerNorm dx")
     _check(g.grad, dg, 2.0 ** -12 * mg, "dgamma")
     _check(bt.grad, db, 2.0 ** -12 * mb, "dbeta")
@@ -151,7 +112,7 @@ def test_embedding_layernorm_backward_f64_bounds(rows, C):
     y.backward(dy)
     tb = [t.to(torch.bfloat16) for t in (word, pos, seg)]
     x = tb[0].double()[ids] + tb[1].double()[pid] + tb[2].double()[sid]
-    dE, mag, dg, mg, db, mb = _ln_f64(x, dy, gamma, 1e-12)
+    _, dE, mag, dg, mg, db, mb = ln_f64(x, dy, gamma, 1e-12)
     for t, idx, n, what in ((ps[0], ids, 500, "word"), (ps[1], pid, 130, "pos"), (ps[2], sid, 2, "seg")):
         ref = torch.zeros(n, C, device=DEV, dtype=torch.float64).index_add_(0, idx, dE)
         m = torch.zeros(n, C, device=DEV, dtype=torch.float64).index_add_(0, idx, mag + dE.abs())

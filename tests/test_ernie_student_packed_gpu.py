@@ -20,11 +20,11 @@ from edl_b200 import ops  # noqa: E402
 from edl_b200.models.ernie import ErnieEncoder, pack_sequences  # noqa: E402
 from edl_b200.ops.transformer import _draw  # noqa: E402
 from f64_bounds import guarded  # noqa: E402
-from test_dropout_gpu import (_attention_f64 as _attention_f64_z, _functional_encoder_dropout, _gen, _scale,  # noqa: E402
-                              _student)
+from student_oracle import attention_f64  # noqa: E402
+from test_dropout_gpu import _functional_encoder_dropout, _gen, _scale, _student  # noqa: E402
 from test_ernie_packed_gpu import _cu, _key_mask, _length_set  # noqa: E402
 from test_ernie_student_cpu import _functional_encoder  # noqa: E402
-from test_ernie_student_gpu import _attention_f64, _batch, _check  # noqa: E402
+from test_ernie_student_gpu import _batch, _check  # noqa: E402
 
 DEV = torch.device("cuda", 0)
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -72,7 +72,7 @@ def test_attention_varlen_backward_f64_bounds(lengths, masked):
     out, lse = T.attention_varlen_forward_saved(qkv.t, cu, ml, h, key_mask)
     assert torch.equal(out, ops.attention_varlen(qkv.t, cu, ml, h, key_mask))   # O bitwise the inference kernel's
     dqkv = T.attention_varlen_backward(qkv.t, cu, ml, h, key_mask, out, lse, do.t)
-    ref, mag = _seq_ref(lambda b, q, m, d, n: _attention_f64(q, m, d, 1, n, h), qkv.t, do.t, cu, key_mask, h)
+    ref, mag = _seq_ref(lambda b, q, m, d, n: attention_f64(q, m, d, 1, n, h)[2:], qkv.t, do.t, cu, key_mask, h)
     _check(dqkv, ref, 2.0 ** -8 * ref.abs() + 2.0 ** -6 * mag, "varlen dqkv %s masked %s" % (lengths, masked))
     assert torch.equal(T.attention_varlen_backward(qkv.t, cu, ml, h, key_mask, out, lse, do.t), dqkv)
     qkv.assert_untouched("qkv")
@@ -87,7 +87,7 @@ def test_attention_varlen_backward_negative_control():
     dqkv = T.attention_varlen_backward(qkv.t, cu, 96, h, None, out, lse, do.t)
     bad = qkv.t.clone()
     bad[[43, 110]] = bad[[110, 43]]
-    ref, mag = _seq_ref(lambda b, q, m, d, n: _attention_f64(q, m, d, 1, n, h), bad, do.t, cu, None, h)
+    ref, mag = _seq_ref(lambda b, q, m, d, n: attention_f64(q, m, d, 1, n, h)[2:], bad, do.t, cu, None, h)
     with pytest.raises(AssertionError):
         _check(dqkv, ref, 2.0 ** -8 * ref.abs() + 2.0 ** -6 * mag, "control")
 
@@ -130,7 +130,7 @@ def test_attention_varlen_dropout(lengths):
         c = cu.tolist()
         for b, (s, e) in enumerate(zip(c[:-1], c[1:])):
             m = key_mask[s:e].view(1, -1)
-            o, mo, r, g = _attention_f64_z(qkv.t[s:e], m, do.t[s:e], 1, e - s, h, zf(b, e - s))
+            o, mo, r, g = attention_f64(qkv.t[s:e], m, do.t[s:e], 1, e - s, h, zf(b, e - s))
             os_.append(o), mos.append(mo), rs.append(r), ms.append(g)
         return torch.cat(os_), torch.cat(mos), torch.cat(rs), torch.cat(ms)
 
