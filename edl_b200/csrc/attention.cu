@@ -1,16 +1,17 @@
 // Masked multi-head attention forward for sm_90a (the ERNIE / BERT encoder of the NLP teacher and of the Transformer
 // student).
 //
-//   O[b, i, h, :] = sum_j softmax_j(Q[b, i, h, :] . K[b, j, h, :] / 8 + mask[b, j]) V[b, j, h, :],   head dim 64
+//   O[b, i, h, :] = sum_j softmax_j(Q[b, i, h, :] . K[b, j, h, :] / sqrt(D) + mask[b, j]) V[b, j, h, :],   D = 64 or 32
 //
-// Q, K and V are read in place from the QKV projection's output [B * L, 3 * H * 64] (columns [0, H*64) are Q, then K,
-// then V) through ONE 4-D tensor map {64, 3H, L, B}: head h of Q / K / V is coordinate h / H + h / 2H of dimension 1.
-// O is written as [B * L, H * 64], the output projection's input.  mask is uint8 [B, L], 1 = attend; any pattern.
+// Q, K and V are read in place from the QKV projection's output [B * L, 3 * H * D] (columns [0, H*D) are Q, then K,
+// then V) through ONE 4-D tensor map {D, 3H, L, B}: head h of Q / K / V is coordinate h / H + h / 2H of dimension 1.
+// O is written as [B * L, H * D], the output projection's input.  mask is uint8 [B, L], 1 = attend; any pattern.
+// Text below speaks of D = 64; "Head dim 32" at the end lists what the D = 32 instantiations change.
 //
 // One CTA per (128-query tile, head, sequence):
 //   warp 0        TMA producer: the Q tile once, then 64-key K / V tiles through a kStages mbarrier ring
 //   warps 4..11   two consumer warpgroups of 64 query rows each:
-//                 S = Q K^T (four wgmma m64n64k16, both operands K-major) -> fp32 registers, masked keys -> -inf,
+//                 S = Q K^T (D / 16 wgmma m64n64k16, both operands K-major) -> fp32 registers, masked keys -> -inf,
 //                 online softmax in the fragment registers (exp2 with log2(e) / 8 folded into the scale),
 //                 P packed to bf16 in registers, O += P V (register-A wgmma, V MN-major),
 //                 O / rowsum -> bf16 -> swizzled staging (the group's own half of the Q tile) -> TMA store.
@@ -41,6 +42,18 @@
 // probability is zeroed in the bf16 A fragment after the row sum has taken it, so m, l and lse stay those of the
 // undropped softmax (lse is bitwise the p = 0 lse) and the scale 1 / (1 - p) is applied to the fp32 output together
 // with 1 / l.
+//
+// Head dim 32 (template parameter D; one kernel body, the D = 64 instantiations compile to the SASS they had before
+// the parameter existed).  A row of Q / K / V / O is 64 bytes, so the tiles use the 64-byte swizzle: tensor maps
+// {32, 3H | H, rows, batch} with CU_TENSOR_MAP_SWIZZLE_64B and wgmma descriptors of layout type 2 (8-row groups 512 B
+// apart), 16-byte chunk j of row r at chunk j ^ ((r / 2) % 4).  The 128B mode cannot describe a 64-byte box row, and a
+// row of 32 bf16 is exactly one 64B swizzle span, so the two k16 steps of S = Q K^T advance the descriptor start by
+// 32 bytes inside the span as the D = 64 steps do inside theirs; the swizzle also keeps the staging stores of the
+// epilogue (four 16-byte chunks per row) spread over the banks.  S = Q K^T is two m64n64k16 steps, O += P V four
+// register-A m64n32k16 (WgmmaBf16RegA32), the O accumulator 16 fp32 registers per thread, the scale log2(e) / sqrt(32),
+// the staging tile and TMA store 64 x 32.  Masks, lse, dropout indices and the packed layout are as above.  Budgets:
+// padded 80 registers (164 with dropout), packed inference 80, packed training 80 (168 with dropout), no spills;
+// dynamic shared memory 33.6 KB (65.6 KB at D = 64).
 #include <cuda.h>
 
 #include <type_traits>
@@ -55,13 +68,22 @@ namespace {
 
 constexpr int kAttnThreads = 384;
 constexpr int kAttnStages = 3;
-constexpr int kHalfBytes = 64 * 128;                            // 64 rows of 64 bf16
-constexpr int kQBytes = 2 * kHalfBytes;
-constexpr int kKVBytes = 2 * kHalfBytes;                        // K tile, then V tile
-constexpr int kMaskOffset = kQBytes + kAttnStages * kKVBytes;
-constexpr int kBarOffset = kMaskOffset + kAttnMaxLen;
-constexpr int kAttnSmem = kBarOffset + 128 + 1024;              // barriers + alignment slack
-constexpr float kScaleLog2 = 0.125f * 1.4426950408889634f;      // 1 / sqrt(64) * log2(e)
+
+// Shared-memory layout and constants of head dim D (64 or 32): rows of 2 D bytes, swizzled over the whole row
+template <int D>
+struct AttnCfg {
+  static_assert(D == 64 || D == 32, "head dim 64 or 32");
+  static constexpr int kRow = 2 * D;                             // bytes per row = the swizzle span
+  static constexpr int kHalfBytes = 64 * kRow;                   // 64 rows of D bf16
+  static constexpr int kQBytes = 2 * kHalfBytes;
+  static constexpr int kKVBytes = 2 * kHalfBytes;                // K tile, then V tile
+  static constexpr int kMaskOffset = kQBytes + kAttnStages * kKVBytes;
+  static constexpr int kBarOffset = kMaskOffset + kAttnMaxLen;
+  static constexpr int kSmem = kBarOffset + 128 + 1024;          // barriers + alignment slack
+  // 1 / sqrt(D) * log2(e)
+  static constexpr float kScaleLog2 =
+      D == 64 ? 0.125f * 1.4426950408889634f : (float)(1.4426950408889634 / 5.656854249492381);
+};
 
 EDL_DEVICE uint32_t pack_bf16(float a, float b) {
   const __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
@@ -95,10 +117,13 @@ struct VarlenTrain {
 
 // Seq = int: the padded layout, seq = L for every sequence (tmQKV / tmO span the whole batch).  Seq = Varlen: packed,
 // inference.  Seq = VarlenTrain: packed, training.  kDrop: dropout on P with the mask of `drop` (training only).
-template <typename Seq, bool kDrop = false>
+template <typename Seq, bool kDrop = false, int D = 64>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO,
                      const uint8_t* __restrict__ mask, Seq seq, int H, float* __restrict__ lse, const PhiloxArgs drop) {
+  using C = AttnCfg<D>;
+  constexpr int kHalfBytes = C::kHalfBytes, kQBytes = C::kQBytes, kKVBytes = C::kKVBytes;
+  constexpr int kSw = C::kRow;                                   // descriptor / tensor-map swizzle span
   constexpr bool kVarlenTrain = std::is_same<Seq, VarlenTrain>::value;
   constexpr bool kVarlen = std::is_same<Seq, Varlen>::value || kVarlenTrain;
   static_assert(!(kVarlen && kDrop) || kVarlenTrain, "dropout: training instantiations only");
@@ -106,8 +131,8 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* sq = smem;
-  uint8_t* smask = smem + kMaskOffset;
-  uint64_t* q_bar = reinterpret_cast<uint64_t*>(smem + kBarOffset);
+  uint8_t* smask = smem + C::kMaskOffset;
+  uint64_t* q_bar = reinterpret_cast<uint64_t*>(smem + C::kBarOffset);
   uint64_t* full_bar = q_bar + 1;
   uint64_t* empty_bar = full_bar + kAttnStages;
 
@@ -175,9 +200,9 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
     if (cw >= groups) return;                                   // every row of this half is past L
     const int row = (warp & 3) * 16 + (lane >> 2);              // first fragment row (the second: + 8)
     const int cq = (lane & 3) * 2;
-    float o[32];
+    float o[D / 2];                                             // the 64 x D output accumulator
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};      // running max (scaled, log2 units) and row sum
     [[maybe_unused]] PhiloxKey pk;
     [[maybe_unused]] uint64_t nrow[2];                          // flat mask index of key 0 of this thread's two rows
@@ -188,17 +213,18 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
       for (int r = 0; r < 2; ++r) nrow[r] = (((uint64_t)b * H + h) * dl + (q0 + cw * 64 + row + 8 * r)) * (uint64_t)dl;
     }
     ptx::mbar_wait(q_bar, 0);
-    const uint64_t dq = ptx::make_smem_desc(ptx::smem_u32(sq + cw * kHalfBytes), 16, 1024);
+    const uint64_t dq = ptx::make_smem_desc<kSw>(ptx::smem_u32(sq + cw * kHalfBytes), 16, 8 * C::kRow);
     for (int kt = 0; kt < n_kt; ++kt) {
       const int s = kt % kAttnStages;
       ptx::mbar_wait(&full_bar[s], (kt / kAttnStages) & 1);
       const uint32_t sk = ptx::smem_u32(smem + kQBytes + s * kKVBytes);
-      const uint64_t dk = ptx::make_smem_desc(sk, 16, 1024);
-      const uint64_t dv = ptx::make_smem_desc(sk + kHalfBytes, 8192, 1024);
+      const uint64_t dk = ptx::make_smem_desc<kSw>(sk, 16, 8 * C::kRow);
+      const uint64_t dv = ptx::make_smem_desc<kSw>(sk + kHalfBytes, 8192, 8 * C::kRow);   // N = D: one MN chunk
       float sc[32];
       ptx::wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k) ptx::WgmmaBf16<64, 0, 0>::mma(sc, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), k != 0 ? 1u : 0u);
+      for (int k = 0; k < D / 16; ++k)
+        ptx::WgmmaBf16<64, 0, 0>::mma(sc, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), k != 0 ? 1u : 0u);
       ptx::wgmma_commit();
       ptx::wgmma_wait<0>();
       // scale + mask, row maxima (a row's 64 columns live in the four lanes of a quad)
@@ -207,10 +233,10 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
       for (int j = 0; j < 8; ++j) {
         const int key = kt * 64 + j * 8 + cq;
         const bool v0 = smask[key] != 0, v1 = smask[key + 1] != 0;
-        sc[4 * j] = v0 ? sc[4 * j] * kScaleLog2 : -INFINITY;
-        sc[4 * j + 1] = v1 ? sc[4 * j + 1] * kScaleLog2 : -INFINITY;
-        sc[4 * j + 2] = v0 ? sc[4 * j + 2] * kScaleLog2 : -INFINITY;
-        sc[4 * j + 3] = v1 ? sc[4 * j + 3] * kScaleLog2 : -INFINITY;
+        sc[4 * j] = v0 ? sc[4 * j] * C::kScaleLog2 : -INFINITY;
+        sc[4 * j + 1] = v1 ? sc[4 * j + 1] * C::kScaleLog2 : -INFINITY;
+        sc[4 * j + 2] = v0 ? sc[4 * j + 2] * C::kScaleLog2 : -INFINITY;
+        sc[4 * j + 3] = v1 ? sc[4 * j + 3] * C::kScaleLog2 : -INFINITY;
         mx[0] = fmaxf(mx[0], fmaxf(sc[4 * j], sc[4 * j + 1]));
         mx[1] = fmaxf(mx[1], fmaxf(sc[4 * j + 2], sc[4 * j + 3]));
       }
@@ -248,13 +274,14 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
 #pragma unroll
       for (int r = 0; r < 2; ++r) l[r] = l[r] * alpha[r] + ls[r];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
+      for (int j = 0; j < D / 8; ++j) {
         o[4 * j] *= alpha[0]; o[4 * j + 1] *= alpha[0];
         o[4 * j + 2] *= alpha[1]; o[4 * j + 3] *= alpha[1];
       }
+      using PV = std::conditional_t<D == 64, ptx::WgmmaBf16RegA64<1>, ptx::WgmmaBf16RegA32<1>>;
       ptx::wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k) ptx::WgmmaBf16RegA64<1>::mma(o, pa[k], dv + (uint64_t)(128 * k), 1u);   // 16 V rows = 2 KB
+      for (int k = 0; k < 4; ++k) PV::mma(o, pa[k], dv + (uint64_t)(C::kRow * k), 1u);   // 16 V rows = 16 kRow bytes
       ptx::wgmma_commit();
       ptx::wgmma_wait<0>();
       if ((threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty_bar[s]);
@@ -285,10 +312,11 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
     }
     uint8_t* st = sq + cw * kHalfBytes;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      *reinterpret_cast<uint32_t*>(st + row * 128 + ((j ^ (row & 7)) << 4) + cq * 2) =
+    for (int j = 0; j < D / 8; ++j) {
+      *reinterpret_cast<uint32_t*>(st + row * C::kRow + ((j ^ (D == 64 ? (row & 7) : ((row >> 1) & 3))) << 4) + cq * 2) =
           pack_bf16(o[4 * j] * inv[0], o[4 * j + 1] * inv[0]);
-      *reinterpret_cast<uint32_t*>(st + (row + 8) * 128 + ((j ^ ((row + 8) & 7)) << 4) + cq * 2) =
+      *reinterpret_cast<uint32_t*>(st + (row + 8) * C::kRow +
+                                   ((j ^ (D == 64 ? ((row + 8) & 7) : (((row + 8) >> 1) & 3))) << 4) + cq * 2) =
           pack_bf16(o[4 * j + 2] * inv[1], o[4 * j + 3] * inv[1]);
     }
     ptx::fence_proxy_async_smem();
@@ -303,7 +331,8 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
 }
 
 // One warp per sequence: copy the template maps to shared memory, point them at the sequence's first row, set their
-// row count to its length, and publish them to maps[2 b], maps[2 b + 1] for the tensor-map proxy.
+// row count to its length, and publish them to maps[2 b], maps[2 b + 1] for the tensor-map proxy.  D: the head dim.
+template <int D = 64>
 __global__ void __launch_bounds__(128)
 attention_varlen_maps_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO,
                              const void* qkv, void* out, const int* __restrict__ cu_seqlens, CUtensorMap* maps, int B,
@@ -317,8 +346,8 @@ attention_varlen_maps_kernel(const __grid_constant__ CUtensorMap tmQKV, const __
     const int len = max(cu_seqlens[b + 1] - start, 1);          // a sequence with len < 1 launches no work
     s[0] = tmQKV;
     s[1] = tmO;
-    const uint64_t a0 = reinterpret_cast<uint64_t>(qkv) + (uint64_t)start * 3 * H * 128;
-    const uint64_t a1 = reinterpret_cast<uint64_t>(out) + (uint64_t)start * H * 128;
+    const uint64_t a0 = reinterpret_cast<uint64_t>(qkv) + (uint64_t)start * 3 * H * (2 * D);
+    const uint64_t a1 = reinterpret_cast<uint64_t>(out) + (uint64_t)start * H * (2 * D);
     asm volatile("tensormap.replace.tile.global_address.shared::cta.b1024.b64 [%0], %1;" ::"r"(ptx::smem_u32(s)),
                  "l"(a0) : "memory");
     asm volatile("tensormap.replace.tile.global_address.shared::cta.b1024.b64 [%0], %1;" ::"r"(ptx::smem_u32(s + 1)),
@@ -334,50 +363,82 @@ attention_varlen_maps_kernel(const __grid_constant__ CUtensorMap tmQKV, const __
                  ::"l"(reinterpret_cast<uint64_t>(maps + 2 * b + i)), "r"(ptx::smem_u32(s + i)) : "memory");
 }
 
-template <typename Seq, bool kDrop = false>
+template <int D, typename Seq, bool kDrop = false>
 const char* launch_attention(const CUtensorMap& tmQKV, const CUtensorMap& tmO, const uint8_t* mask, Seq seq, int H,
                              dim3 grid, cudaStream_t stream, float* lse = nullptr, const PhiloxArgs& drop = PhiloxArgs{}) {
+  constexpr int kSmem = AttnCfg<D>::kSmem;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attention_fwd_kernel<Seq, kDrop>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         kAttnSmem);
+    cudaError_t e = cudaFuncSetAttribute(attention_fwd_kernel<Seq, kDrop, D>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
     if (e != cudaSuccess) return cudaGetErrorString(e);
     attr_set = true;
   }
-  attention_fwd_kernel<Seq, kDrop><<<grid, kAttnThreads, kAttnSmem, stream>>>(tmQKV, tmO, mask, seq, H, lse, drop);
+  attention_fwd_kernel<Seq, kDrop, D><<<grid, kAttnThreads, kSmem, stream>>>(tmQKV, tmO, mask, seq, H, lse, drop);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
-// Q / K / V and O maps {64, 3H | H, rows, batch} of a [batch * rows, 3 * H * 64] / [batch * rows, H * 64] layout
+// Q / K / V and O maps {D, 3H | H, rows, batch} of a [batch * rows, 3 * H * D] / [batch * rows, H * D] layout, swizzled
+// over the 2 D-byte row (128B at D = 64, 64B at D = 32, the descriptors' mode)
+template <int D>
 const char* encode_attention_maps(CUtensorMap* tmQKV, CUtensorMap* tmO, const void* qkv, void* out, int rows, int batch,
                                   int H) {
-  const uint32_t box[4] = {64, 1, 64, 1};
+  constexpr uint64_t kRow = 2 * D;
+  const uint32_t box[4] = {D, 1, 64, 1};
   {
-    const uint64_t dims[4] = {64, (uint64_t)3 * H, (uint64_t)rows, (uint64_t)batch};
-    const uint64_t st[3] = {128, (uint64_t)3 * H * 128, (uint64_t)rows * 3 * H * 128};
-    if (const char* e = encode_tmap_bf16(tmQKV, qkv, 4, dims, st, box)) return e;
+    const uint64_t dims[4] = {D, (uint64_t)3 * H, (uint64_t)rows, (uint64_t)batch};
+    const uint64_t st[3] = {kRow, (uint64_t)3 * H * kRow, (uint64_t)rows * 3 * H * kRow};
+    if (const char* e = encode_tmap_strided(tmQKV, qkv, 4, dims, st, box, nullptr, 2, (int)kRow)) return e;
   }
-  const uint64_t dims[4] = {64, (uint64_t)H, (uint64_t)rows, (uint64_t)batch};
-  const uint64_t st[3] = {128, (uint64_t)H * 128, (uint64_t)rows * H * 128};
-  return encode_tmap_bf16(tmO, out, 4, dims, st, box);
+  const uint64_t dims[4] = {D, (uint64_t)H, (uint64_t)rows, (uint64_t)batch};
+  const uint64_t st[3] = {kRow, (uint64_t)H * kRow, (uint64_t)rows * H * kRow};
+  return encode_tmap_strided(tmO, out, 4, dims, st, box, nullptr, 2, (int)kRow);
+}
+
+template <int D>
+const char* attention_fwd_d(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream,
+                            float* lse, const PhiloxArgs* drop) {
+  alignas(64) CUtensorMap tmQKV, tmO;
+  if (const char* e = encode_attention_maps<D>(&tmQKV, &tmO, qkv, out, L, B, H)) return e;
+  const dim3 grid((L + 127) / 128, H, B);
+  if (drop != nullptr) return launch_attention<D, int, true>(tmQKV, tmO, mask, L, H, grid, stream, lse, *drop);
+  return launch_attention<D, int>(tmQKV, tmO, mask, L, H, grid, stream, lse);
+}
+
+template <int D>
+const char* attention_varlen_fwd_d(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, void* out,
+                                   void* maps, int T, int B, int max_len, int H, cudaStream_t stream, float* lse,
+                                   const PhiloxArgs* drop) {
+  // templates over the whole buffer; the prologue replaces the address and the row count per sequence
+  alignas(64) CUtensorMap tmQKV, tmO;
+  if (const char* e = encode_attention_maps<D>(&tmQKV, &tmO, qkv, out, T, 1, H)) return e;
+  CUtensorMap* m = static_cast<CUtensorMap*>(maps);
+  attention_varlen_maps_kernel<D><<<(B + 3) / 4, 128, 0, stream>>>(tmQKV, tmO, qkv, out, cu_seqlens, m, B, H);
+  if (cudaError_t e = cudaGetLastError(); e != cudaSuccess) return cudaGetErrorString(e);
+  const dim3 grid((max_len + 127) / 128, H, B);
+  if (lse != nullptr) {
+    const VarlenTrain seq{cu_seqlens, m, T};
+    if (drop != nullptr)
+      return launch_attention<D, VarlenTrain, true>(tmQKV, tmO, key_mask, seq, H, grid, stream, lse, *drop);
+    return launch_attention<D, VarlenTrain>(tmQKV, tmO, key_mask, seq, H, grid, stream, lse);
+  }
+  return launch_attention<D, Varlen>(tmQKV, tmO, key_mask, Varlen{cu_seqlens, m}, H, grid, stream);
 }
 
 }  // namespace
 
 bool attention_supported(int B, int L, int H, int head_dim) {
-  return B >= 1 && B <= 65535 && L >= 1 && L <= kAttnMaxLen && H >= 1 && H <= 65535 && head_dim == 64;
+  return B >= 1 && B <= 65535 && L >= 1 && L <= kAttnMaxLen && H >= 1 && H <= 65535 &&
+         (head_dim == 64 || head_dim == 32);
 }
 
-const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream,
-                          float* lse, const PhiloxArgs* drop) {
-  if (!attention_supported(B, L, H, 64)) return "attention_fwd: unsupported shape (head dim 64, 1 <= L <= 512)";
+const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, int D,
+                          cudaStream_t stream, float* lse, const PhiloxArgs* drop) {
+  if (!attention_supported(B, L, H, D)) return "attention_fwd: unsupported shape (head dim 32 or 64, 1 <= L <= 512)";
   if (drop != nullptr && lse == nullptr) return "attention_fwd: dropout is a training feature (give lse)";
-  alignas(64) CUtensorMap tmQKV, tmO;
-  if (const char* e = encode_attention_maps(&tmQKV, &tmO, qkv, out, L, B, H)) return e;
-  const dim3 grid((L + 127) / 128, H, B);
-  if (drop != nullptr) return launch_attention<int, true>(tmQKV, tmO, mask, L, H, grid, stream, lse, *drop);
-  return launch_attention<int>(tmQKV, tmO, mask, L, H, grid, stream, lse);
+  return D == 64 ? attention_fwd_d<64>(qkv, mask, out, B, L, H, stream, lse, drop)
+                 : attention_fwd_d<32>(qkv, mask, out, B, L, H, stream, lse, drop);
 }
 
 bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim) {
@@ -385,24 +446,13 @@ bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim) 
 }
 
 const char* attention_varlen_fwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, void* out, void* maps,
-                                 int T, int B, int max_len, int H, cudaStream_t stream, float* lse,
+                                 int T, int B, int max_len, int H, int D, cudaStream_t stream, float* lse,
                                  const PhiloxArgs* drop) {
-  if (!attention_varlen_supported(T, B, max_len, H, 64))
-    return "attention_varlen_fwd: unsupported shape (head dim 64, T >= 1, 1 <= max_len <= 512)";
+  if (!attention_varlen_supported(T, B, max_len, H, D))
+    return "attention_varlen_fwd: unsupported shape (head dim 32 or 64, T >= 1, 1 <= max_len <= 512)";
   if (drop != nullptr && lse == nullptr) return "attention_varlen_fwd: dropout is a training feature (give lse)";
-  // templates over the whole buffer; the prologue replaces the address and the row count per sequence
-  alignas(64) CUtensorMap tmQKV, tmO;
-  if (const char* e = encode_attention_maps(&tmQKV, &tmO, qkv, out, T, 1, H)) return e;
-  CUtensorMap* m = static_cast<CUtensorMap*>(maps);
-  attention_varlen_maps_kernel<<<(B + 3) / 4, 128, 0, stream>>>(tmQKV, tmO, qkv, out, cu_seqlens, m, B, H);
-  if (cudaError_t e = cudaGetLastError(); e != cudaSuccess) return cudaGetErrorString(e);
-  const dim3 grid((max_len + 127) / 128, H, B);
-  if (lse != nullptr) {
-    const VarlenTrain seq{cu_seqlens, m, T};
-    if (drop != nullptr) return launch_attention<VarlenTrain, true>(tmQKV, tmO, key_mask, seq, H, grid, stream, lse, *drop);
-    return launch_attention<VarlenTrain>(tmQKV, tmO, key_mask, seq, H, grid, stream, lse);
-  }
-  return launch_attention<Varlen>(tmQKV, tmO, key_mask, Varlen{cu_seqlens, m}, H, grid, stream);
+  return D == 64 ? attention_varlen_fwd_d<64>(qkv, cu_seqlens, key_mask, out, maps, T, B, max_len, H, stream, lse, drop)
+                 : attention_varlen_fwd_d<32>(qkv, cu_seqlens, key_mask, out, maps, T, B, max_len, H, stream, lse, drop);
 }
 
 }  // namespace edl

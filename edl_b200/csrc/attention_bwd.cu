@@ -1,5 +1,5 @@
-// Masked multi-head attention backward for sm_90a (padded layout, head dim 64, L <= 512): the training path of the
-// Transformer student.  With S = Q K^T / 8 and P = softmax over the valid keys,
+// Masked multi-head attention backward for sm_90a (padded layout, head dim 64 or 32, L <= 512): the training path of
+// the Transformer student.  With S = Q K^T / 8 and P = softmax over the valid keys (head dim 64; 32 below),
 //
 //   dV = P^T dO,   dP = dO V^T,   dS = P o (dP - D) with D = rowsum(dO o O),   dQ = dS K / 8,   dK = dS^T Q / 8.
 //
@@ -32,6 +32,13 @@
 // attn_bwd_delta 40, no spills; packed: attn_bwd_dkdv 173 registers (220 with dropout), attn_bwd_dq 136 (175), no
 // spills;
 // static shared memory 36.5 KB (dkdv: Q, Q^T, dO, dO^T tiles + lse / D) and 27.1 KB (dq: K, K^T, V tiles + key flags).
+//
+// Head dim 32 (template parameter D; the D = 64 instantiations compile to the SASS they had before it existed): the
+// tiles are 64 x D (row pitch 72 kept, so fragment loads still hit 32 distinct banks) and their transposes D x 64; S and
+// dP take K = D (two k16 steps), dQ / dK / dV are D / 8 accumulator tiles wide, dQ and dK are scaled by 1 / sqrt(32),
+// and the delta pass leaves lanes 16..31 idle.  Budgets, no spills: attn_bwd_dkdv 131 registers (149 with dropout),
+// attn_bwd_dq 101 (180), attn_bwd_delta 32; packed: attn_bwd_dkdv 132 (145), attn_bwd_dq 101 (160); static shared
+// memory 27.5 KB (dkdv) and 22.6 KB (dq).
 #include "common.cuh"
 #include "kernels.h"
 #include "philox.cuh"
@@ -41,7 +48,11 @@ namespace {
 
 constexpr int kT = 64;        // tile rows (keys or queries)
 constexpr int kP = 72;        // shared-memory row pitch in bf16
-constexpr float kScaleLog2 = 0.125f * 1.4426950408889634f;
+// 1 / sqrt(D) and 1 / sqrt(D) * log2(e) of head dim D (64 or 32), as the forward (attention.cu) forms them
+template <int D>
+constexpr float kInvSqrtD = D == 64 ? 0.125f : (float)(1.0 / 5.656854249492381);
+template <int D>
+constexpr float kScaleLog2 = D == 64 ? 0.125f * 1.4426950408889634f : (float)(1.4426950408889634 / 5.656854249492381);
 
 EDL_DEVICE uint32_t pack2(float a, float b) {
   const __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
@@ -58,12 +69,15 @@ EDL_DEVICE void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uin
 
 EDL_DEVICE uint32_t lds(const __nv_bfloat16* p) { return *reinterpret_cast<const uint32_t*>(p); }
 
-// 64 rows x 64 columns of one head from a [B * L, ld] bf16 buffer (rows at or past L read as 0) into a row-major tile
-// and, if t != nullptr, its transpose
+// 64 rows x W columns of one head from a [B * L, ld] bf16 buffer (rows at or past L read as 0) into a row-major tile
+// and, if t != nullptr, its transpose (W rows of 64)
+template <int W>
 EDL_DEVICE void load_tile(const __nv_bfloat16* __restrict__ src, int64_t ld, int r0, int L, __nv_bfloat16* s,
                           __nv_bfloat16* t) {
-  for (int v = threadIdx.x; v < kT * 8; v += 128) {
-    const int r = v >> 3, c = (v & 7) * 8;
+  static_assert(W == 64 || W == 32, "tile width 64 or 32");
+  constexpr int kShift = W == 64 ? 3 : 2;                       // log2 of the 8-column chunks per row
+  for (int v = threadIdx.x; v < kT * (W / 8); v += 128) {
+    const int r = v >> kShift, c = (v & (W / 8 - 1)) * 8;
     bf16x8 x;
     if (r0 + r < L) x = *reinterpret_cast<const bf16x8*>(src + (int64_t)(r0 + r) * ld + c);
     else x = bf16x8{};
@@ -76,10 +90,11 @@ EDL_DEVICE void load_tile(const __nv_bfloat16* __restrict__ src, int64_t ld, int
   }
 }
 
-// A fragments of rows r0 .. r0 + 15 of a row-major tile, the four 16-column k steps
-EDL_DEVICE void load_afrag(const __nv_bfloat16* s, int r0, int g, int t, uint32_t (&a)[4][4]) {
+// A fragments of rows r0 .. r0 + 15 of a row-major tile, the K / 16 16-column k steps
+template <int K>
+EDL_DEVICE void load_afrag(const __nv_bfloat16* s, int r0, int g, int t, uint32_t (&a)[K / 16][4]) {
 #pragma unroll
-  for (int k = 0; k < 4; ++k) {
+  for (int k = 0; k < K / 16; ++k) {
     a[k][0] = lds(s + (r0 + g) * kP + k * 16 + 2 * t);
     a[k][1] = lds(s + (r0 + g + 8) * kP + k * 16 + 2 * t);
     a[k][2] = lds(s + (r0 + g) * kP + k * 16 + 8 + 2 * t);
@@ -87,12 +102,13 @@ EDL_DEVICE void load_afrag(const __nv_bfloat16* s, int r0, int g, int t, uint32_
   }
 }
 
-// c[j] (16 x 8, j = 0..7) += A (16 x 64) * Y^T, Y a row-major tile whose rows are the 64 output columns
-EDL_DEVICE void mma_rows(float (&c)[8][4], const uint32_t (&a)[4][4], const __nv_bfloat16* y, int g, int t) {
+// c[j] (16 x 8, j = 0..7) += A (16 x K) * Y^T, Y a row-major tile whose rows are the 64 output columns
+template <int K>
+EDL_DEVICE void mma_rows(float (&c)[8][4], const uint32_t (&a)[K / 16][4], const __nv_bfloat16* y, int g, int t) {
 #pragma unroll
   for (int j = 0; j < 8; ++j)
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
+    for (int k = 0; k < K / 16; ++k)
       mma16816(c[j], a[k], lds(y + (j * 8 + g) * kP + k * 16 + 2 * t), lds(y + (j * 8 + g) * kP + k * 16 + 8 + 2 * t));
 }
 
@@ -107,19 +123,22 @@ EDL_DEVICE void acc_to_afrag(const float (&c)[8][4], uint32_t (&a)[4][4]) {
   }
 }
 
-// rows r .. of a 16 x 64 accumulator (times `scale`) -> bf16 columns col0 .. of dqkv rows (rows at or past L skipped)
-EDL_DEVICE void store_rows(const float (&c)[8][4], __nv_bfloat16* __restrict__ dst, int64_t ld, int r, int L, int t,
+// rows r .. of a 16 x W accumulator (times `scale`) -> bf16 columns col0 .. of dqkv rows (rows at or past L skipped)
+template <int W>
+EDL_DEVICE void store_rows(const float (&c)[W / 8][4], __nv_bfloat16* __restrict__ dst, int64_t ld, int r, int L, int t,
                            float scale) {
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     if (r + 8 * h >= L) continue;
     __nv_bfloat16* row = dst + (int64_t)(r + 8 * h) * ld + 2 * t;
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
+    for (int j = 0; j < W / 8; ++j)
       *reinterpret_cast<uint32_t*>(row + j * 8) = pack2(c[j][2 * h] * scale, c[j][2 * h + 1] * scale);
   }
 }
 
+// one warp per row, lane l holds columns 2 l, 2 l + 1 (lanes past D / 2 add 0)
+template <int D = 64>
 __global__ void __launch_bounds__(256)
 attn_bwd_delta(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ dout, float* __restrict__ delta,
                int B, int L, int H) {
@@ -128,25 +147,29 @@ attn_bwd_delta(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __res
   if (r >= (int64_t)B * L) return;
   const int b = (int)(r / L), i = (int)(r % L);
   for (int h = 0; h < H; ++h) {
-    const int64_t o = r * H * 64 + h * 64 + 2 * lane;
-    const float2 x = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(out + o));
-    const float2 y = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(dout + o));
-    const float s = warp_sum(fmaf(x.x, y.x, x.y * y.y));
+    const int64_t o = r * H * D + h * D + 2 * lane;
+    float v = 0.f;
+    if (2 * lane < D) {
+      const float2 x = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(out + o));
+      const float2 y = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(dout + o));
+      v = fmaf(x.x, y.x, x.y * y.y);
+    }
+    const float s = warp_sum(v);
     if (lane == 0) delta[((int64_t)b * H + h) * L + i] = s;
   }
 }
 
-template <bool kDrop, bool kVarlen = false>
+template <bool kDrop, bool kVarlen = false, int D = 64>
 __global__ void __launch_bounds__(128)
 attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ mask,
               const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse, const float* __restrict__ delta,
               __nv_bfloat16* __restrict__ dqkv, int L, int H, const PhiloxArgs drop,
               const int* __restrict__ cu_seqlens = nullptr, int T = 0) {
-  __shared__ alignas(16) __nv_bfloat16 sQ[kT * kP], sQt[kT * kP], sO[kT * kP], sOt[kT * kP];
+  __shared__ alignas(16) __nv_bfloat16 sQ[kT * kP], sQt[D * kP], sO[kT * kP], sOt[D * kP];
   __shared__ float sL[kT], sD[kT];
   const int k0 = blockIdx.x * kT, h = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const int64_t ldq = (int64_t)3 * H * 64, ldo = (int64_t)H * 64;
+  const int64_t ldq = (int64_t)3 * H * D, ldo = (int64_t)H * D;
   int64_t r0 = (int64_t)b * L;                                  // the sequence's first row
   if constexpr (kVarlen) {
     r0 = cu_seqlens[b];
@@ -159,12 +182,12 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
   const int dl = kVarlen ? kAttnMaxLen : L;
   const uint64_t dsh = kVarlen ? ((uint64_t)b * H + h) * kAttnMaxLen : (uint64_t)sh;
   // this warp's 16 keys of K and V as A fragments (staged through the Q / dO tiles)
-  load_tile(base + (H + h) * 64, ldq, k0, L, sQ, nullptr);
-  load_tile(base + (2 * H + h) * 64, ldq, k0, L, sO, nullptr);
+  load_tile<D>(base + (H + h) * D, ldq, k0, L, sQ, nullptr);
+  load_tile<D>(base + (2 * H + h) * D, ldq, k0, L, sO, nullptr);
   __syncthreads();
-  uint32_t kf[4][4], vf[4][4];
-  load_afrag(sQ, warp * 16, g, t, kf);
-  load_afrag(sO, warp * 16, g, t, vf);
+  uint32_t kf[D / 16][4], vf[D / 16][4];
+  load_afrag<D>(sQ, warp * 16, g, t, kf);
+  load_afrag<D>(sO, warp * 16, g, t, vf);
   const int key0 = k0 + warp * 16 + g;
   bool kv[2];
 #pragma unroll
@@ -172,9 +195,9 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
     const int key = key0 + 8 * e;
     kv[e] = key < L && (mask == nullptr || mask[r0 + key] != 0);
   }
-  float dk[8][4], dv[8][4];
+  float dk[D / 8][4], dv[D / 8][4];
 #pragma unroll
-  for (int j = 0; j < 8; ++j)
+  for (int j = 0; j < D / 8; ++j)
 #pragma unroll
     for (int e = 0; e < 4; ++e) dk[j][e] = dv[j][e] = 0.f;
   [[maybe_unused]] PhiloxKey pk;
@@ -182,8 +205,8 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
 
   for (int q0 = 0; q0 < L; q0 += kT) {
     __syncthreads();                                        // the previous tiles (or the K / V staging) are consumed
-    load_tile(base + h * 64, ldq, q0, L, sQ, sQt);
-    load_tile(dout + r0 * ldo + h * 64, ldo, q0, L, sO, sOt);
+    load_tile<D>(base + h * D, ldq, q0, L, sQ, sQt);
+    load_tile<D>(dout + r0 * ldo + h * D, ldo, q0, L, sO, sOt);
     if (threadIdx.x < kT) {
       const int q = q0 + threadIdx.x;
       sL[threadIdx.x] = q < L ? lse[sh + q] : INFINITY;
@@ -207,14 +230,14 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
     for (int j = 0; j < 8; ++j)
 #pragma unroll
       for (int e = 0; e < 4; ++e) p[j][e] = dp[j][e] = 0.f;
-    mma_rows(p, kf, sQ, g, t);
-    mma_rows(dp, vf, sO, g, t);
+    mma_rows<D>(p, kf, sQ, g, t);
+    mma_rows<D>(dp, vf, sO, g, t);
 #pragma unroll
     for (int j = 0; j < 8; ++j)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int qc = j * 8 + 2 * t + (e & 1);
-        const float pe = kv[e >> 1] ? exp2f(p[j][e] * kScaleLog2 - sL[qc]) : 0.f;
+        const float pe = kv[e >> 1] ? exp2f(p[j][e] * kScaleLog2<D> - sL[qc]) : 0.f;
         if constexpr (kDrop) {
           const float z = (km >> (j * 4 + e)) & 1u ? pk.scale : 0.f;
           p[j][e] = pe * z;
@@ -229,7 +252,7 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
     acc_to_afrag(p, pa);
     acc_to_afrag(dp, sa);
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
+    for (int j = 0; j < D / 8; ++j)
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const __nv_bfloat16* ro = sOt + (j * 8 + g) * kP + k * 16 + 2 * t;
@@ -239,21 +262,21 @@ attn_bwd_dkdv(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__
       }
   }
   __nv_bfloat16* drow = dqkv + r0 * ldq;
-  store_rows(dk, drow + (H + h) * 64, ldq, key0, L, t, 0.125f);
-  store_rows(dv, drow + (2 * H + h) * 64, ldq, key0, L, t, 1.f);
+  store_rows<D>(dk, drow + (H + h) * D, ldq, key0, L, t, kInvSqrtD<D>);
+  store_rows<D>(dv, drow + (2 * H + h) * D, ldq, key0, L, t, 1.f);
 }
 
-template <bool kDrop, bool kVarlen = false>
+template <bool kDrop, bool kVarlen = false, int D = 64>
 __global__ void __launch_bounds__(128)
 attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ mask,
             const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse, const float* __restrict__ delta,
             __nv_bfloat16* __restrict__ dqkv, int L, int H, const PhiloxArgs drop,
             const int* __restrict__ cu_seqlens = nullptr, int T = 0) {
-  __shared__ alignas(16) __nv_bfloat16 sK[kT * kP], sKt[kT * kP], sV[kT * kP];
+  __shared__ alignas(16) __nv_bfloat16 sK[kT * kP], sKt[D * kP], sV[kT * kP];
   __shared__ uint8_t sM[kT];
   const int q0 = blockIdx.x * kT, h = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const int64_t ldq = (int64_t)3 * H * 64, ldo = (int64_t)H * 64;
+  const int64_t ldq = (int64_t)3 * H * D, ldo = (int64_t)H * D;
   int64_t r0 = (int64_t)b * L;                                  // the sequence's first row
   if constexpr (kVarlen) {
     r0 = cu_seqlens[b];
@@ -266,12 +289,12 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
   const int dl = kVarlen ? kAttnMaxLen : L;
   const uint64_t dsh = kVarlen ? ((uint64_t)b * H + h) * kAttnMaxLen : (uint64_t)sh;
   // this warp's 16 queries of Q and dO as A fragments (staged through the K / V tiles)
-  load_tile(base + h * 64, ldq, q0, L, sK, nullptr);
-  load_tile(dout + r0 * ldo + h * 64, ldo, q0, L, sV, nullptr);
+  load_tile<D>(base + h * D, ldq, q0, L, sK, nullptr);
+  load_tile<D>(dout + r0 * ldo + h * D, ldo, q0, L, sV, nullptr);
   __syncthreads();
-  uint32_t qf[4][4], of[4][4];
-  load_afrag(sK, warp * 16, g, t, qf);
-  load_afrag(sV, warp * 16, g, t, of);
+  uint32_t qf[D / 16][4], of[D / 16][4];
+  load_afrag<D>(sK, warp * 16, g, t, qf);
+  load_afrag<D>(sV, warp * 16, g, t, of);
   const int qr = q0 + warp * 16 + g;
   float rl[2], rd[2];
 #pragma unroll
@@ -280,9 +303,9 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
     rl[e] = q < L ? lse[sh + q] : INFINITY;
     rd[e] = q < L ? delta[sh + q] : 0.f;
   }
-  float dq[8][4];
+  float dq[D / 8][4];
 #pragma unroll
-  for (int j = 0; j < 8; ++j)
+  for (int j = 0; j < D / 8; ++j)
 #pragma unroll
     for (int e = 0; e < 4; ++e) dq[j][e] = 0.f;
   [[maybe_unused]] PhiloxKey pk;
@@ -290,8 +313,8 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
 
   for (int kb = 0; kb < L; kb += kT) {
     __syncthreads();
-    load_tile(base + (H + h) * 64, ldq, kb, L, sK, sKt);
-    load_tile(base + (2 * H + h) * 64, ldq, kb, L, sV, nullptr);
+    load_tile<D>(base + (H + h) * D, ldq, kb, L, sK, sKt);
+    load_tile<D>(base + (2 * H + h) * D, ldq, kb, L, sV, nullptr);
     if (threadIdx.x < kT) {
       const int key = kb + threadIdx.x;
       sM[threadIdx.x] = (key < L && (mask == nullptr || mask[r0 + key] != 0)) ? 1 : 0;
@@ -302,8 +325,8 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
     for (int j = 0; j < 8; ++j)
 #pragma unroll
       for (int e = 0; e < 4; ++e) s[j][e] = dp[j][e] = 0.f;
-    mma_rows(s, qf, sK, g, t);
-    mma_rows(dp, of, sV, g, t);
+    mma_rows<D>(s, qf, sK, g, t);
+    mma_rows<D>(dp, of, sV, g, t);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       [[maybe_unused]] uint32_t keep[2];
@@ -315,7 +338,7 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int kc = j * 8 + 2 * t + (e & 1);
-        const float pe = sM[kc] ? exp2f(s[j][e] * kScaleLog2 - rl[e >> 1]) : 0.f;
+        const float pe = sM[kc] ? exp2f(s[j][e] * kScaleLog2<D> - rl[e >> 1]) : 0.f;
         if constexpr (kDrop) {
           const float z = (keep[e >> 1] >> (e & 1)) & 1u ? pk.scale : 0.f;
           s[j][e] = pe * (dp[j][e] * z - rd[e >> 1]);
@@ -327,61 +350,81 @@ attn_bwd_dq(const __nv_bfloat16* __restrict__ qkv, const uint8_t* __restrict__ m
     uint32_t sa[4][4];
     acc_to_afrag(s, sa);
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
+    for (int j = 0; j < D / 8; ++j)
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const __nv_bfloat16* rk = sKt + (j * 8 + g) * kP + k * 16 + 2 * t;
         mma16816(dq[j], sa[k], lds(rk), lds(rk + 8));
       }
   }
-  store_rows(dq, dqkv + r0 * ldq + h * 64, ldq, qr, L, t, 0.125f);
+  store_rows<D>(dq, dqkv + r0 * ldq + h * D, ldq, qr, L, t, kInvSqrtD<D>);
 }
 
-}  // namespace
-
-const char* attention_bwd(const void* qkv, const uint8_t* mask, const void* out, const float* lse, const void* dout,
-                          void* dqkv, float* delta, int B, int L, int H, cudaStream_t stream, const PhiloxArgs* drop) {
-  if (!attention_supported(B, L, H, 64)) return "attention_bwd: unsupported shape (head dim 64, 1 <= L <= 512)";
+template <int D>
+const char* attention_bwd_d(const void* qkv, const uint8_t* mask, const void* out, const float* lse, const void* dout,
+                            void* dqkv, float* delta, int B, int L, int H, cudaStream_t stream, const PhiloxArgs* drop) {
   const auto* q = reinterpret_cast<const __nv_bfloat16*>(qkv);
   const auto* o = reinterpret_cast<const __nv_bfloat16*>(out);
   const auto* d = reinterpret_cast<const __nv_bfloat16*>(dout);
   auto* dq = reinterpret_cast<__nv_bfloat16*>(dqkv);
   const int64_t rows = (int64_t)B * L;
-  attn_bwd_delta<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(o, d, delta, B, L, H);
+  attn_bwd_delta<D><<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(o, d, delta, B, L, H);
   const dim3 grid((L + kT - 1) / kT, H, B);
   if (drop != nullptr) {
-    attn_bwd_dkdv<true><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, *drop);
-    attn_bwd_dq<true><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, *drop);
+    attn_bwd_dkdv<true, false, D><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, *drop);
+    attn_bwd_dq<true, false, D><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, *drop);
   } else {
-    attn_bwd_dkdv<false><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, PhiloxArgs{});
-    attn_bwd_dq<false><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, PhiloxArgs{});
+    attn_bwd_dkdv<false, false, D><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, PhiloxArgs{});
+    attn_bwd_dq<false, false, D><<<grid, 128, 0, stream>>>(q, mask, d, lse, delta, dq, L, H, PhiloxArgs{});
   }
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
-const char* attention_varlen_bwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, const void* out,
-                                 const float* lse, const void* dout, void* dqkv, float* delta, int T, int B, int max_len,
-                                 int H, cudaStream_t stream, const PhiloxArgs* drop) {
-  if (!attention_varlen_supported(T, B, max_len, H, 64))
-    return "attention_varlen_bwd: unsupported shape (head dim 64, T >= 1, 1 <= max_len <= 512)";
+template <int D>
+const char* attention_varlen_bwd_d(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, const void* out,
+                                   const float* lse, const void* dout, void* dqkv, float* delta, int T, int B,
+                                   int max_len, int H, cudaStream_t stream, const PhiloxArgs* drop) {
   const auto* q = reinterpret_cast<const __nv_bfloat16*>(qkv);
   const auto* o = reinterpret_cast<const __nv_bfloat16*>(out);
   const auto* d = reinterpret_cast<const __nv_bfloat16*>(dout);
   auto* dq = reinterpret_cast<__nv_bfloat16*>(dqkv);
-  attn_bwd_delta<<<(unsigned)(((int64_t)T + 7) / 8), 256, 0, stream>>>(o, d, delta, 1, T, H);   // D [H, T]
+  attn_bwd_delta<D><<<(unsigned)(((int64_t)T + 7) / 8), 256, 0, stream>>>(o, d, delta, 1, T, H);   // D [H, T]
   const dim3 grid((max_len + kT - 1) / kT, H, B);
   if (drop != nullptr) {
-    attn_bwd_dkdv<true, true><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, *drop, cu_seqlens, T);
-    attn_bwd_dq<true, true><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, *drop, cu_seqlens, T);
+    attn_bwd_dkdv<true, true, D><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, *drop,
+                                                            cu_seqlens, T);
+    attn_bwd_dq<true, true, D><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, *drop,
+                                                          cu_seqlens, T);
   } else {
-    attn_bwd_dkdv<false, true><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, PhiloxArgs{},
-                                                         cu_seqlens, T);
-    attn_bwd_dq<false, true><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, PhiloxArgs{},
-                                                       cu_seqlens, T);
+    attn_bwd_dkdv<false, true, D><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, PhiloxArgs{},
+                                                             cu_seqlens, T);
+    attn_bwd_dq<false, true, D><<<grid, 128, 0, stream>>>(q, key_mask, d, lse, delta, dq, max_len, H, PhiloxArgs{},
+                                                           cu_seqlens, T);
   }
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
+}  // namespace
+
+const char* attention_bwd(const void* qkv, const uint8_t* mask, const void* out, const float* lse, const void* dout,
+                          void* dqkv, float* delta, int B, int L, int H, int D, cudaStream_t stream,
+                          const PhiloxArgs* drop) {
+  if (!attention_supported(B, L, H, D)) return "attention_bwd: unsupported shape (head dim 32 or 64, 1 <= L <= 512)";
+  return D == 64 ? attention_bwd_d<64>(qkv, mask, out, lse, dout, dqkv, delta, B, L, H, stream, drop)
+                 : attention_bwd_d<32>(qkv, mask, out, lse, dout, dqkv, delta, B, L, H, stream, drop);
+}
+
+const char* attention_varlen_bwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, const void* out,
+                                 const float* lse, const void* dout, void* dqkv, float* delta, int T, int B, int max_len,
+                                 int H, int D, cudaStream_t stream, const PhiloxArgs* drop) {
+  if (!attention_varlen_supported(T, B, max_len, H, D))
+    return "attention_varlen_bwd: unsupported shape (head dim 32 or 64, T >= 1, 1 <= max_len <= 512)";
+  return D == 64 ? attention_varlen_bwd_d<64>(qkv, cu_seqlens, key_mask, out, lse, dout, dqkv, delta, T, B, max_len, H,
+                                              stream, drop)
+                 : attention_varlen_bwd_d<32>(qkv, cu_seqlens, key_mask, out, lse, dout, dqkv, delta, T, B, max_len, H,
+                                              stream, drop);
 }
 
 }  // namespace edl

@@ -344,7 +344,7 @@ const char* encode_tmap(void* out, const void* ptr, int rank, const uint64_t* di
 // its input without an im2col or a subsampling pass.
 const char* encode_tmap_strided(void* out, const void* ptr, int rank, const uint64_t* dims,
                                 const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides,
-                                int elem_bytes, bool swizzle) {
+                                int elem_bytes, int swizzle_bytes) {
   EncodeTiledFn fn = get_encode_fn();
   if (fn == nullptr) return "cuTensorMapEncodeTiled entry point not found";
   cuuint64_t d[5], st[4];
@@ -354,7 +354,10 @@ const char* encode_tmap_strided(void* out, const void* ptr, int rank, const uint
   CUresult r = fn(reinterpret_cast<CUtensorMap*>(out),
                   elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank,
                   const_cast<void*>(ptr), d, st, b, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  swizzle_bytes == 128  ? CU_TENSOR_MAP_SWIZZLE_128B
+                  : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                        : CU_TENSOR_MAP_SWIZZLE_NONE,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     snprintf(g_tmap_err, sizeof(g_tmap_err),

@@ -172,7 +172,7 @@ const char* encode_tmap(void* out, const void* ptr, int rank, const uint64_t* di
                         const uint64_t* strides_bytes, const uint32_t* box, int elem_bytes);
 const char* encode_tmap_strided(void* out, const void* ptr, int rank, const uint64_t* dims,
                                 const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides,
-                                int elem_bytes, bool swizzle = true);
+                                int elem_bytes, int swizzle_bytes = 128);   // 128, 64 or 0 (none)
 
 // FP8 (e4m3) inference GEMM (gemm_fp8.cu): D[M,N] bf16 = relu?((A[M,K] * B[N,K]^T) * col_scale[n] + col_shift[n])
 // A, B e4m3 bytes, K-major; col_scale carries act_scale * weight_scale[n] (* folded BN scale).

@@ -1053,7 +1053,7 @@ const char* gemm_bf16_persistent(const GemmArgs& g, cudaStream_t stream) {
       const uint64_t dims[2] = {(uint64_t)g.N / 8, (uint64_t)g.M};
       const uint64_t st[1] = {(uint64_t)g.N / 8};
       const uint32_t box[2] = {16, kBlockM};
-      if (const char* e = encode_tmap_strided(&tmBy, g.bn.mask, 2, dims, st, box, nullptr, 1, false)) return e;
+      if (const char* e = encode_tmap_strided(&tmBy, g.bn.mask, 2, dims, st, box, nullptr, 1, 0)) return e;
     }
     fill_bn(p, g.bn);
     const CUtensorMap* pby = (has_y || has_mask) ? &tmBy : nullptr;

@@ -224,36 +224,37 @@ void wait_flag_async(const void* flag, const void* seq_ptr, uint32_t seq_imm, do
 
 // ---- attention.cu / layernorm.cu: the Transformer encoder of the NLP teacher (inference) ----
 constexpr int kAttnMaxLen = 512;
+// head_dim (D below): 64 or 32
 bool attention_supported(int B, int L, int H, int head_dim);
-// qkv bf16 [B * L, 3 * H * 64] (Q | K | V column blocks, 16-byte aligned), mask uint8 [B, L] (1 = attend; nullptr: all),
-// out bf16 [B * L, H * 64].  lse: nullptr, or fp32 [B, H, L] that receives what the backward needs to recompute the
+// qkv bf16 [B * L, 3 * H * D] (Q | K | V column blocks, 16-byte aligned), mask uint8 [B, L] (1 = attend; nullptr: all),
+// out bf16 [B * L, H * D].  lse: nullptr, or fp32 [B, H, L] that receives what the backward needs to recompute the
 // probabilities (attention.cu).  drop (training, with lse): dropout on the probabilities, element (b, h, i, j) at flat
 // index ((b H + h) L + i) L + j of the mask.  Returns nullptr or an error string.
-const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, cudaStream_t stream,
-                          float* lse = nullptr, const PhiloxArgs* drop = nullptr);
+const char* attention_fwd(const void* qkv, const uint8_t* mask, void* out, int B, int L, int H, int D,
+                          cudaStream_t stream, float* lse = nullptr, const PhiloxArgs* drop = nullptr);
 // Backward of attention_fwd (attention_bwd.cu): from qkv, the forward's out and lse and the output gradient dout
-// (bf16 [B * L, H * 64]) writes dqkv bf16 [B * L, 3 * H * 64] (dQ | dK | dV in the layout of qkv).  delta: fp32 [B, H, L]
+// (bf16 [B * L, H * D]) writes dqkv bf16 [B * L, 3 * H * D] (dQ | dK | dV in the layout of qkv).  delta: fp32 [B, H, L]
 // workspace.  drop: the forward's dropout (the same mask is regenerated).  Deterministic, no atomics.
 const char* attention_bwd(const void* qkv, const uint8_t* mask, const void* out, const float* lse, const void* dout,
-                          void* dqkv, float* delta, int B, int L, int H, cudaStream_t stream,
+                          void* dqkv, float* delta, int B, int L, int H, int D, cudaStream_t stream,
                           const PhiloxArgs* drop = nullptr);
 bool attention_varlen_supported(int T, int B, int max_len, int H, int head_dim);
-// Packed sequences: qkv bf16 [T, 3 * H * 64], sequence b in rows [cu_seqlens[b], cu_seqlens[b + 1]) (int32 device
-// offsets, 1 <= length <= max_len <= 512), key_mask uint8 [T] (1 = attend; nullptr: all), out bf16 [T, H * 64];
+// Packed sequences: qkv bf16 [T, 3 * H * D], sequence b in rows [cu_seqlens[b], cu_seqlens[b + 1]) (int32 device
+// offsets, 1 <= length <= max_len <= 512), key_mask uint8 [T] (1 = attend; nullptr: all), out bf16 [T, H * D];
 // maps: device workspace of 2 * B CUtensorMaps (64-byte aligned).  A sequence's output depends on its own rows only.
 // lse (training): nullptr, or fp32 [H, T] that receives lse at h * T + packed row (a separate kernel instantiation; the
 // inference one is unchanged).  drop (training, with lse): dropout on the probabilities, element (b, h, i, j) at flat
 // index ((b H + h) 512 + i) 512 + j of the mask: the fixed stride kAttnMaxLen keeps the sequences' ranges disjoint.
 const char* attention_varlen_fwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, void* out, void* maps,
-                                 int T, int B, int max_len, int H, cudaStream_t stream, float* lse = nullptr,
+                                 int T, int B, int max_len, int H, int D, cudaStream_t stream, float* lse = nullptr,
                                  const PhiloxArgs* drop = nullptr);
 // Backward of the packed training forward (attention_bwd.cu): from qkv, out and lse [H, T] of attention_varlen_fwd and
-// dout bf16 [T, H * 64], writes the rows of every sequence of dqkv bf16 [T, 3 * H * 64] (rows outside all sequences are
+// dout bf16 [T, H * D], writes the rows of every sequence of dqkv bf16 [T, 3 * H * D] (rows outside all sequences are
 // not written).  delta: fp32 [H, T] workspace.  drop: the forward's dropout.  A sequence's gradients depend on its own
 // rows only.  Deterministic, no atomics, no host synchronisation.
 const char* attention_varlen_bwd(const void* qkv, const int* cu_seqlens, const uint8_t* key_mask, const void* out,
                                  const float* lse, const void* dout, void* dqkv, float* delta, int T, int B, int max_len,
-                                 int H, cudaStream_t stream, const PhiloxArgs* drop = nullptr);
+                                 int H, int D, cudaStream_t stream, const PhiloxArgs* drop = nullptr);
 constexpr int kLnMaxC = 1024;
 bool layernorm_supported(int C);
 // y[r] = (x[r] - mean) * rsqrt(var + eps) * gamma + beta over the C columns of each row; x, y bf16 [rows, C] (row pitch

@@ -118,12 +118,16 @@ EDL_DEVICE void fence_proxy_async_smem() {
 //   K-major : rows of 128 B (64 bf16), 8-row groups 1024 B apart -> SBO = 1024, LBO unused (1)
 //   MN-major: [k rows][64 mn elems = 128 B]; 8-k-row groups 1024 B apart -> SBO = 1024,
 //             64-element MN chunks LBO bytes apart
+// kSwizzleBytes = 64: SWIZZLE_64B (layout type 2), the same with rows of 64 B (32 bf16) and 8-row groups 512 B apart
+// (SBO = 512); the matching tensor map is CU_TENSOR_MAP_SWIZZLE_64B.
+template <int kSwizzleBytes = 128>
 EDL_DEVICE uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  static_assert(kSwizzleBytes == 128 || kSwizzleBytes == 64, "128B or 64B swizzle");
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
+  d |= (uint64_t)(kSwizzleBytes == 128 ? 1 : 2) << 62;
   return d;
 }
 

@@ -52,13 +52,24 @@ void check_bf16_2d(const Tensor& t, const char* name) {
               " must be a contiguous 2-D bf16 CUDA tensor");
 }
 
-// qkv [B * L, 3 * H * 64], mask uint8 [B, L] or None, out [B * L, H * 64]
+// The head dim D of a qkv [rows, 3 * H * D]: 64 or 32, the widths the attention kernels take
+int64_t head_dim(const Tensor& qkv, int64_t H) {
+  TORCH_CHECK(H >= 1, "attention: H >= 1 heads");
+  const int64_t D = qkv.size(1) / (3 * H);
+  TORCH_CHECK(qkv.size(1) == 3 * H * D && (D == 64 || D == 32),
+              "attention: qkv must be [rows, 3 * H * D] with head dim D = 64 or 32, got width ", qkv.size(1),
+              " for H = ", H);
+  return D;
+}
+
+// qkv [B * L, 3 * H * D], mask uint8 [B, L] or None, out [B * L, H * D]; D = 64 or 32
 void attention_fwd(const Tensor& qkv, const c10::optional<Tensor>& mask, Tensor& out, int64_t B, int64_t L, int64_t H,
                    const c10::optional<Tensor>& lse, const edl::PhiloxArgs* drop) {
   check_bf16_2d(qkv, "qkv");
   check_bf16_2d(out, "out");
-  TORCH_CHECK(qkv.size(0) == B * L && qkv.size(1) == 3 * H * 64, "qkv must be [B * L, 3 * H * 64]");
-  TORCH_CHECK(out.size(0) == B * L && out.size(1) == H * 64, "out must be [B * L, H * 64]");
+  const int64_t D = head_dim(qkv, H);
+  TORCH_CHECK(qkv.size(0) == B * L, "qkv must be [B * L, 3 * H * D]");
+  TORCH_CHECK(out.size(0) == B * L && out.size(1) == H * D, "out must be [B * L, H * D]");
   TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0);
   const uint8_t* mp = nullptr;
   if (mask.has_value() && mask->defined()) {
@@ -73,19 +84,19 @@ void attention_fwd(const Tensor& qkv, const c10::optional<Tensor>& mask, Tensor&
     lp = lse->data_ptr<float>();
   }
   c10::cuda::CUDAGuard guard(qkv.device());
-  const char* err = edl::attention_fwd(qkv.data_ptr(), mp, out.data_ptr(), (int)B, (int)L, (int)H,
+  const char* err = edl::attention_fwd(qkv.data_ptr(), mp, out.data_ptr(), (int)B, (int)L, (int)H, (int)D,
                                        at::cuda::getCurrentCUDAStream().stream(), lp, drop);
   TORCH_CHECK(err == nullptr, "edl attention_fwd failed: ", err);
 }
 
-// dqkv [B * L, 3 * H * 64] from qkv, the forward's out and lse [B, H, L], dout [B * L, H * 64]; delta fp32 [B, H, L]
+// dqkv [B * L, 3 * H * D] from qkv, the forward's out and lse [B, H, L], dout [B * L, H * D]; delta fp32 [B, H, L]
 void attention_bwd(const Tensor& qkv, const c10::optional<Tensor>& mask, const Tensor& out, const Tensor& lse,
                    const Tensor& dout, Tensor& dqkv, Tensor& delta, int64_t B, int64_t L, int64_t H,
                    const edl::PhiloxArgs* drop) {
   for (const Tensor* t : {&qkv, &out, &dout, static_cast<const Tensor*>(&dqkv)}) check_bf16_2d(*t, "attention_bwd operand");
-  TORCH_CHECK(qkv.size(0) == B * L && qkv.size(1) == 3 * H * 64 && dqkv.sizes() == qkv.sizes(),
-              "qkv / dqkv must be [B * L, 3 * H * 64]");
-  TORCH_CHECK(out.size(0) == B * L && out.size(1) == H * 64 && dout.sizes() == out.sizes(), "out / dout: [B * L, H * 64]");
+  const int64_t D = head_dim(qkv, H);
+  TORCH_CHECK(qkv.size(0) == B * L && dqkv.sizes() == qkv.sizes(), "qkv / dqkv must be [B * L, 3 * H * D]");
+  TORCH_CHECK(out.size(0) == B * L && out.size(1) == H * D && dout.sizes() == out.sizes(), "out / dout: [B * L, H * D]");
   for (const Tensor* t : {&lse, static_cast<const Tensor*>(&delta)})
     TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() == B * H * L,
                 "lse / delta must be contiguous fp32 [B, H, L] CUDA tensors");
@@ -99,7 +110,7 @@ void attention_bwd(const Tensor& qkv, const c10::optional<Tensor>& mask, const T
   }
   c10::cuda::CUDAGuard guard(qkv.device());
   const char* err = edl::attention_bwd(qkv.data_ptr(), mp, out.data_ptr(), lse.data_ptr<float>(), dout.data_ptr(),
-                                       dqkv.data_ptr(), delta.data_ptr<float>(), (int)B, (int)L, (int)H,
+                                       dqkv.data_ptr(), delta.data_ptr<float>(), (int)B, (int)L, (int)H, (int)D,
                                        at::cuda::getCurrentCUDAStream().stream(), drop);
   TORCH_CHECK(err == nullptr, "edl attention_bwd failed: ", err);
 }
@@ -119,7 +130,7 @@ int64_t check_varlen(const Tensor& cu_seqlens, const c10::optional<Tensor>& key_
   return B;
 }
 
-// qkv [T, 3 * H * 64], cu_seqlens int32 [B + 1], key_mask uint8 [T] or None, out [T, H * 64], maps uint8 [B * 256];
+// qkv [T, 3 * H * D], cu_seqlens int32 [B + 1], key_mask uint8 [T] or None, out [T, H * D], maps uint8 [B * 256];
 // training: lse fp32 [H, T] (and drop, with lse) or None
 void attention_varlen_fwd(const Tensor& qkv, const Tensor& cu_seqlens, const c10::optional<Tensor>& key_mask,
                           Tensor& out, Tensor& maps, int64_t max_len, int64_t H, const c10::optional<Tensor>& lse,
@@ -127,8 +138,8 @@ void attention_varlen_fwd(const Tensor& qkv, const Tensor& cu_seqlens, const c10
   check_bf16_2d(qkv, "qkv");
   check_bf16_2d(out, "out");
   const int64_t T = qkv.size(0);
-  TORCH_CHECK(qkv.size(1) == 3 * H * 64, "qkv must be [T, 3 * H * 64]");
-  TORCH_CHECK(out.size(0) == T && out.size(1) == H * 64, "out must be [T, H * 64]");
+  const int64_t D = head_dim(qkv, H);
+  TORCH_CHECK(out.size(0) == T && out.size(1) == H * D, "out must be [T, H * D]");
   TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0);
   const uint8_t* mp;
   const int64_t B = check_varlen(cu_seqlens, key_mask, T, &mp);
@@ -142,12 +153,12 @@ void attention_varlen_fwd(const Tensor& qkv, const Tensor& cu_seqlens, const c10
   }
   c10::cuda::CUDAGuard guard(qkv.device());
   const char* err = edl::attention_varlen_fwd(qkv.data_ptr(), cu_seqlens.data_ptr<int>(), mp, out.data_ptr(),
-                                              maps.data_ptr(), (int)T, (int)B, (int)max_len, (int)H,
+                                              maps.data_ptr(), (int)T, (int)B, (int)max_len, (int)H, (int)D,
                                               at::cuda::getCurrentCUDAStream().stream(), lp, drop);
   TORCH_CHECK(err == nullptr, "edl attention_varlen_fwd failed: ", err);
 }
 
-// dqkv [T, 3 * H * 64] (the rows of every sequence) from qkv, the packed forward's out and lse [H, T], dout [T, H * 64];
+// dqkv [T, 3 * H * D] (the rows of every sequence) from qkv, the packed forward's out and lse [H, T], dout [T, H * D];
 // delta fp32 [H, T]
 void attention_varlen_bwd(const Tensor& qkv, const Tensor& cu_seqlens, const c10::optional<Tensor>& key_mask,
                           const Tensor& out, const Tensor& lse, const Tensor& dout, Tensor& dqkv, Tensor& delta,
@@ -155,8 +166,9 @@ void attention_varlen_bwd(const Tensor& qkv, const Tensor& cu_seqlens, const c10
   for (const Tensor* t : {&qkv, &out, &dout, static_cast<const Tensor*>(&dqkv)})
     check_bf16_2d(*t, "attention_varlen_bwd operand");
   const int64_t T = qkv.size(0);
-  TORCH_CHECK(qkv.size(1) == 3 * H * 64 && dqkv.sizes() == qkv.sizes(), "qkv / dqkv must be [T, 3 * H * 64]");
-  TORCH_CHECK(out.size(0) == T && out.size(1) == H * 64 && dout.sizes() == out.sizes(), "out / dout: [T, H * 64]");
+  const int64_t D = head_dim(qkv, H);
+  TORCH_CHECK(dqkv.sizes() == qkv.sizes(), "qkv / dqkv must be [T, 3 * H * D]");
+  TORCH_CHECK(out.size(0) == T && out.size(1) == H * D && dout.sizes() == out.sizes(), "out / dout: [T, H * D]");
   for (const Tensor* t : {&lse, static_cast<const Tensor*>(&delta)})
     TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() == H * T &&
                 t->device() == qkv.device(), "lse / delta must be contiguous fp32 [H, T] CUDA tensors");
@@ -167,7 +179,7 @@ void attention_varlen_bwd(const Tensor& qkv, const Tensor& cu_seqlens, const c10
   c10::cuda::CUDAGuard guard(qkv.device());
   const char* err = edl::attention_varlen_bwd(qkv.data_ptr(), cu_seqlens.data_ptr<int>(), mp, out.data_ptr(),
                                               lse.data_ptr<float>(), dout.data_ptr(), dqkv.data_ptr(),
-                                              delta.data_ptr<float>(), (int)T, (int)B, (int)max_len, (int)H,
+                                              delta.data_ptr<float>(), (int)T, (int)B, (int)max_len, (int)H, (int)D,
                                               at::cuda::getCurrentCUDAStream().stream(), drop);
   TORCH_CHECK(err == nullptr, "edl attention_varlen_bwd failed: ", err);
 }

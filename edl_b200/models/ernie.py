@@ -439,10 +439,19 @@ def ernie_base(num_labels=2):
     return ErnieEncoder(18000, 768, 12, 12, 3072, 513, 2, num_labels)
 
 
-def ernie_student(num_labels=2, dropout=0.0):
-    """The Transformer student: the teacher's vocabulary (18000) and feeds, hidden 384, 4 layers, 6 heads, FFN 1536;
-    ``dropout`` sets both its hidden and attention dropout (BERT trains with 0.1)."""
-    return ErnieStudent(18000, 384, 4, 6, 1536, 513, 2, num_labels, hidden_dropout=dropout, attention_dropout=dropout)
+def ernie_student(num_labels=2, dropout=0.0, heads=6):
+    """The Transformer student: the teacher's vocabulary (18000) and feeds, hidden 384, 4 layers, FFN 1536;
+    ``dropout`` sets both its hidden and attention dropout (BERT trains with 0.1).  ``heads``: 6 heads of 64, or 12 of
+    32 (the MiniLM-L12-H384 shape); the attention kernels take head dims 32 and 64.  The parameters do not depend on
+    it."""
+    return ErnieStudent(18000, 384, 4, heads, 1536, 513, 2, num_labels, hidden_dropout=dropout,
+                        attention_dropout=dropout)
+
+
+def minilm_l12_h384(num_labels=2):
+    """A MiniLM-L12-H384-shaped BERT encoder: vocabulary 30522, hidden 384, 12 layers, 12 heads of 32, FFN 1536, 512
+    positions, 2 segment types.  ``load_bert_state_dict`` / ``load_weights`` take such a checkpoint."""
+    return ErnieEncoder(30522, 384, 12, 12, 1536, 512, 2, num_labels)
 
 
 def ernie_tiny(num_labels=2):

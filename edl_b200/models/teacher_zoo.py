@@ -1,9 +1,10 @@
 """Named teacher models for ``python -m paddle_edl.distill.teacher_server --model NAME``.
 ``build(name) -> (module, feed_names, fetch_names, feed_shapes)``; the fetch name of the image
 teachers is ``score`` (softmax probabilities), matching the reference's serving model
-(example/distill/resnet/train_with_fleet.py:446).  The sequence teachers (``ernie_base``, ``ernie_tiny``) take the
-reference's four ERNIE feeds as its ``ernie_reader`` batches them -- ``input_ids``, ``position_ids``, ``segment_ids``
-int64 [L, 1] and ``input_mask`` float [L, 1] per sample -- and fetch ``logits``, fp32 [B, num_labels]."""
+(example/distill/resnet/train_with_fleet.py:446).  The sequence teachers (``ernie_base``, ``minilm_l12_h384``,
+``ernie_tiny``) take the reference's four ERNIE feeds as its ``ernie_reader`` batches them -- ``input_ids``,
+``position_ids``, ``segment_ids`` int64 [L, 1] and ``input_mask`` float [L, 1] per sample -- and fetch ``logits``, fp32
+[B, num_labels]."""
 import torch
 import torch.nn as nn
 
@@ -36,9 +37,10 @@ def build(name):
     if name == "mnist_cnn":
         from .small import MnistTeacher
         return _Probs(MnistTeacher(), channels_last=False), ["img"], ["fc_0.tmp_2"], {"img": [1, 28, 28]}
-    if name in ("ernie_base", "ernie_tiny"):
+    if name in ("ernie_base", "minilm_l12_h384", "ernie_tiny"):
         from . import ernie
-        net = ernie.ernie_base() if name == "ernie_base" else ernie.ernie_tiny()
+        net = {"ernie_base": ernie.ernie_base, "minilm_l12_h384": ernie.minilm_l12_h384,
+               "ernie_tiny": ernie.ernie_tiny}[name]()
         feeds = ["input_ids", "position_ids", "segment_ids", "input_mask"]
         return net, feeds, ["logits"], {f: [ERNIE_MAX_SEQ_LEN, 1] for f in feeds}
     raise ValueError("unknown teacher model %r" % name)

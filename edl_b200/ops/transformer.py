@@ -2,7 +2,8 @@
 the inference path of the ERNIE / BERT sequence teacher (models/ernie.py).
 
 Dispatch rule of the package: CPU tensors run the small float32 reference implementations below; on CUDA a shape a
-kernel cannot take (head dim other than 64, sequences longer than 512, a hidden size above 1024 or not a multiple of 8)
+kernel cannot take (head dim other than 32 or 64, sequences longer than 512, a hidden size above 1024 or not a
+multiple of 8)
 runs the same reference math on the library through ``count_fallback``.
 
 ``layer_norm_e4m3`` and ``embedding_layernorm_e4m3`` also return the block-scaled e4m3 copy of their bf16 output
@@ -248,10 +249,11 @@ def attention_varlen_supported(qkv, cu_seqlens, max_len, heads) -> bool:
 
 
 def attention_varlen(qkv, cu_seqlens, max_len, heads, key_mask=None, out=None):
-    """Masked multi-head self-attention over sequences packed back to back (inference).  ``qkv`` [T, 3 * H * 64] is the
-    QKV projection's output on the packed tokens; sequence b is rows [cu_seqlens[b], cu_seqlens[b + 1]) (int32 [B + 1],
-    offset 0, non-decreasing, lengths 1..512); ``max_len`` (host int) is at least the longest length; ``key_mask``
-    [T] (nonzero = attend) or None.  Returns O [T, H * 64].  Per sequence this is ``attention`` with L = its length,
+    """Masked multi-head self-attention over sequences packed back to back (inference).  ``qkv`` [T, 3 * H * D] is the
+    QKV projection's output on the packed tokens (head dim D = qkv.shape[1] / 3H; the kernels take 32 and 64);
+    sequence b is rows [cu_seqlens[b], cu_seqlens[b + 1]) (int32 [B + 1], offset 0, non-decreasing, lengths 1..512);
+    ``max_len`` (host int) is at least the longest length; ``key_mask`` [T] (nonzero = attend) or None.  Returns
+    O [T, H * D].  Per sequence this is ``attention`` with L = its length,
     and its output depends on its own rows only.
 
     ``cu_seqlens`` is not read back to the host, so the call can be captured in a CUDA graph; ``pack_sequences``
@@ -471,12 +473,13 @@ def attention_train_supported(x, batch, seq_len, heads, head_dim=64) -> bool:
 
 
 def attention_forward_saved(qkv, mask, batch, seq_len, heads, drop=None):
-    """The kernel forward with the statistics the backward needs: (out bf16 [B * L, H * 64], lse fp32 [B, H, L]).
+    """The kernel forward with the statistics the backward needs: (out bf16 [B * L, H * D], lse fp32 [B, H, L]), D the
+    head dim of qkv [B * L, 3 * H * D] (32 or 64).
     ``drop``: a drawn dropout site (``_draw``) for the probabilities, element (b, h, i, j) at ((b H + h) L + i) L + j;
     lse is that of the undropped softmax."""
     from . import native, count_launch
 
-    out = torch.empty((batch * seq_len, heads * 64), device=qkv.device, dtype=torch.bfloat16)
+    out = torch.empty((batch * seq_len, qkv.shape[1] // 3), device=qkv.device, dtype=torch.bfloat16)
     lse = torch.empty((batch, heads, seq_len), device=qkv.device, dtype=torch.float32)
     native().attention_fwd(qkv, mask, out, batch, seq_len, heads, lse, drop)
     count_launch()
@@ -484,7 +487,7 @@ def attention_forward_saved(qkv, mask, batch, seq_len, heads, drop=None):
 
 
 def attention_backward(qkv, mask, out, lse, dout, batch, seq_len, heads, drop=None):
-    """dqkv bf16 [B * L, 3 * H * 64] (dQ | dK | dV in qkv's layout) of ``attention``, from the forward's ``out`` and
+    """dqkv bf16 [B * L, 3 * H * D] (dQ | dK | dV in qkv's layout) of ``attention``, from the forward's ``out`` and
     ``lse`` (``attention_forward_saved``, with the same ``drop``) and the output gradient ``dout``."""
     from . import native, count_launch
 
@@ -496,14 +499,14 @@ def attention_backward(qkv, mask, out, lse, dout, batch, seq_len, heads, drop=No
 
 
 def attention_varlen_forward_saved(qkv, cu_seqlens, max_len, heads, key_mask=None, drop=None):
-    """The packed kernel forward with the statistics the backward needs: (out bf16 [T, H * 64], lse fp32 [H, T], lse
+    """The packed kernel forward with the statistics the backward needs: (out bf16 [T, H * D], lse fp32 [H, T], lse
     of head h and packed row r at [h, r]).  ``drop``: a drawn dropout site for the probabilities, element (b, h, i, j) at
     ((b H + h) 512 + i) 512 + j; lse is that of the undropped softmax.  ``cu_seqlens`` int32 and ``key_mask`` uint8 (or
     None), contiguous, on qkv's device."""
     from . import native, count_launch
 
     t = qkv.shape[0]
-    out = torch.empty((t, heads * 64), device=qkv.device, dtype=torch.bfloat16)
+    out = torch.empty((t, qkv.shape[1] // 3), device=qkv.device, dtype=torch.bfloat16)
     lse = torch.empty((heads, t), device=qkv.device, dtype=torch.float32)
     maps = torch.empty((cu_seqlens.numel() - 1) * 256, device=qkv.device, dtype=torch.uint8)
     native().attention_varlen_fwd(qkv, cu_seqlens, key_mask, out, maps, int(max_len), heads, lse, drop)
@@ -512,7 +515,7 @@ def attention_varlen_forward_saved(qkv, cu_seqlens, max_len, heads, key_mask=Non
 
 
 def attention_varlen_backward(qkv, cu_seqlens, max_len, heads, key_mask, out, lse, dout, drop=None):
-    """dqkv bf16 [T, 3 * H * 64] of ``attention_varlen`` from the forward's ``out`` and ``lse``
+    """dqkv bf16 [T, 3 * H * D] of ``attention_varlen`` from the forward's ``out`` and ``lse``
     (``attention_varlen_forward_saved``, with the same ``drop``) and the output gradient ``dout``.  Every row must
     belong to a sequence (cu_seqlens[-1] == T, as ``pack_sequences`` makes it): rows outside all sequences are not
     written."""
@@ -595,13 +598,12 @@ class _AttentionVarlenFn(torch.autograd.Function):
 
 def attention_varlen_trainable(qkv, cu_seqlens, max_len, heads, key_mask=None, dropout_p=0.0):
     """``attention_varlen`` with a gradient, the packed sibling of ``attention_trainable``: the kernel path saves lse
-    [H, T] and runs the packed backward of attention_bwd.cu.  ``qkv`` [T, 3 * H * 64] with every row inside a sequence
+    [H, T] and runs the packed backward of attention_bwd.cu.  ``qkv`` [T, 3 * H * D] with every row inside a sequence
     (cu_seqlens[-1] == T).  ``dropout_p``: dropout on the attention probabilities (one site, index
     ((b H + h) 512 + i) 512 + j).  On CPU, and for a shape the kernels do not take, ``attention_varlen_reference`` runs
     under autograd (counted through ``count_fallback`` on CUDA)."""
     p = _check_p(dropout_p)
-    if qkv.is_cuda and attention_varlen_supported(_bf16(qkv).contiguous(), cu_seqlens, max_len, heads) \
-            and qkv.shape[1] == 3 * heads * 64:
+    if qkv.is_cuda and attention_varlen_supported(_bf16(qkv).contiguous(), cu_seqlens, max_len, heads):
         layout = _Packed(_cu_i32(cu_seqlens), max_len, _mask_u8(key_mask, qkv.device))
         return _AttentionVarlenFn.apply(qkv, layout, heads, _draw(qkv.device, p) if p > 0.0 else None)
     if qkv.is_cuda:
@@ -704,12 +706,12 @@ def attention_block(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, 
     CUDA), the weights in any float dtype (cast to bf16 here), ``mask`` [B, L] (nonzero = attend) or None.  Returns
     bf16 on the kernel path (the input of the following LayerNorm); differentiable in x and the four parameters.
     ``attn_dropout`` drops attention probabilities, then ``hidden_dropout`` the output branch before the residual add
-    (two sites, in that order; branch index row * C + col)."""
+    (two sites, in that order; branch index row * C + col).  The kernels take head dim C / heads = 32 or 64."""
     from .gemm import _grad_sink
 
     pa, ph = _check_p(attn_dropout), _check_p(hidden_dropout)
     c = x.shape[-1]
-    if x.is_cuda and c % 8 == 0 and c == heads * 64 and attention_train_supported(x, batch, seq_len, heads):
+    if x.is_cuda and c % 8 == 0 and c % heads == 0 and attention_train_supported(x, batch, seq_len, heads, c // heads):
         sinks = tuple(_grad_sink(p) for p in (qkv_w, qkv_b, out_w, out_b))
         drops = tuple(_draw(x.device, p) if p > 0.0 else None for p in (pa, ph))
         return _AttentionBlockFn.apply(x, qkv_w, qkv_b, out_w, out_b,
@@ -734,11 +736,11 @@ def attention_block_varlen(x, qkv_w, qkv_b, out_w, out_b, cu_seqlens, max_len, h
 
     pa, ph = _check_p(attn_dropout), _check_p(hidden_dropout)
     c = x.shape[-1]
-    if (x.is_cuda and x.dim() == 2 and c % 8 == 0 and c == heads * 64 and cu_seqlens.is_cuda
+    if (x.is_cuda and x.dim() == 2 and c % 8 == 0 and c % heads == 0 and cu_seqlens.is_cuda
             and cu_seqlens.dim() == 1 and cu_seqlens.numel() >= 2):
         from . import native
 
-        ok = native().attention_varlen_supported(x.shape[0], cu_seqlens.numel() - 1, int(max_len), heads, 64)
+        ok = native().attention_varlen_supported(x.shape[0], cu_seqlens.numel() - 1, int(max_len), heads, c // heads)
     else:
         ok = False
     if ok:

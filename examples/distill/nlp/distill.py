@@ -40,6 +40,8 @@ def main():
     ap.add_argument("--packed", action="store_true",
                     help="--model ernie: the student trains on each batch packed to its real tokens (the teacher still "
                          "receives the padded feeds)")
+    ap.add_argument("--heads", type=int, default=6,
+                    help="--model ernie: attention heads of the hidden-384 student (12: the MiniLM-shaped head dim 32)")
     args = ap.parse_args()
     if args.packed and args.model != "ernie":
         ap.error("--packed needs --model ernie")
@@ -52,7 +54,8 @@ def main():
     if args.model in ("lstm", "ernie"):  # these students run on the GPU when there is one
         dev = torch.device("cuda" if torch.cuda.is_available() else "cpu")
         # the Transformer student builds its four feeds from the ids (positions 0.., segment 0, mask ids != 0)
-        student = (BiLSTM(args.vocab) if args.model == "lstm" else ernie_student(dropout=args.dropout)).to(dev)
+        student = (BiLSTM(args.vocab) if args.model == "lstm" else ernie_student(dropout=args.dropout,
+                                                                                      heads=args.heads)).to(dev)
     else:
         student = BOW(args.vocab) if args.model == "bow" else TextCNN(args.vocab)
     opt = torch.optim.AdamW(student.parameters(), 1e-4 if args.model == "ernie" else 1e-3)   # a Transformer wants less

@@ -15,13 +15,14 @@ from paddle_edl.models.small import BOW, BiLSTM, TextCNN  # noqa: E402
 from paddle_edl.models.ernie import ernie_student, pack_sequences  # noqa: E402
 
 
-def build_model(name, vocab, dropout=0.0):
+def build_model(name, vocab, dropout=0.0, heads=6):
     """(model, device): the LSTM and Transformer students run on the GPU when there is one (csrc/lstm.cu, the encoder
     kernels), the others on the CPU.  The Transformer student has the teacher's 18000-id vocabulary and builds its four
-    feeds from the ids (positions 0.., segment 0, mask ids != 0); ``dropout`` is its hidden and attention dropout."""
+    feeds from the ids (positions 0.., segment 0, mask ids != 0); ``dropout`` is its hidden and attention dropout,
+    ``heads`` its attention heads (6 of 64 or 12 of 32 at hidden 384)."""
     if name in ("lstm", "ernie"):
         dev = torch.device("cuda" if torch.cuda.is_available() else "cpu")
-        return (BiLSTM(vocab) if name == "lstm" else ernie_student(dropout=dropout)).to(dev), dev
+        return (BiLSTM(vocab) if name == "lstm" else ernie_student(dropout=dropout, heads=heads)).to(dev), dev
     return (BOW(vocab) if name == "bow" else TextCNN(vocab)), torch.device("cpu")
 
 
@@ -62,6 +63,8 @@ def main():
     ap.add_argument("--dropout", type=float, default=0.0, help="hidden and attention dropout of --model ernie")
     ap.add_argument("--packed", action="store_true",
                     help="--model ernie: train on each batch packed to its real tokens (forward_packed)")
+    ap.add_argument("--heads", type=int, default=6,
+                    help="--model ernie: attention heads of the hidden-384 student (12: the MiniLM-shaped head dim 32)")
     args = ap.parse_args()
     if args.packed and args.model != "ernie":
         ap.error("--packed needs --model ernie")
@@ -75,7 +78,7 @@ def main():
         vocab = args.vocab
         train_iter = lambda ep: batches(synthetic_corpus(args.samples, vocab, args.seq_len, ep), 16)   # noqa: E731
         dev_data = list(batches(synthetic_corpus(256, vocab, args.seq_len, 10_000), 16))
-    model, dev = build_model(args.model, vocab, args.dropout)
+    model, dev = build_model(args.model, vocab, args.dropout, args.heads)
     opt = torch.optim.AdamW(model.parameters(), 1e-4 if args.model == "ernie" else 1e-3)   # a Transformer wants less
     for ep in range(args.epochs):
         for ids, label in train_iter(ep):

@@ -8,7 +8,10 @@ p, ours at 0, and the bf16 torch model with F.dropout at the same sites and SDPA
 MIN_LEN`` the sample lengths are drawn uniformly from [MIN_LEN, seq] (fixed seed) and it times three steps on that
 batch and the same weights: ours padded (``forward``), ours packed (``forward_packed`` on ``pack_sequences`` of the
 batch) and torch padded; it also reports the real-token fraction and the host time of ``pack_sequences`` per batch.
-All GPU times come from CUDA events.  Prints the GPU name and power limit with the numbers."""
+With ``--heads H`` the student has H heads (6 of 64 by default, 12 of 32 for the MiniLM shape) in every arm, and the
+output also reports ``heads`` and the attention forward alone against SDPA's (without ``--heads`` the output is that of
+the 6-head student, as before).  All GPU times come from CUDA events.  Prints the GPU name and power limit with the
+numbers."""
 import argparse
 import json
 import os
@@ -99,6 +102,8 @@ def main():
     ap.add_argument("--dropout", type=float, default=None, help="time training steps with this dropout instead")
     ap.add_argument("--packed", type=int, default=None, metavar="MIN_LEN",
                     help="lengths uniform in [MIN_LEN, seq]: time the padded step, the packed step and torch")
+    ap.add_argument("--heads", type=int, default=None,
+                    help="attention heads of the student (default 6); also time the attention forward alone")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_ernie_student: needs a GPU")
@@ -116,9 +121,10 @@ def main():
     label = torch.randint(0, 2, (b,), device=dev)
     keep = ids != 0
 
-    ours = ernie_student().to(dev)
+    h = 6 if args.heads is None else args.heads
+    ours = ernie_student(heads=h).to(dev)
     opt = torch.optim.AdamW(ours.parameters(), 1e-4, capturable=True)
-    ref = ernie_student().to(dev).to(torch.bfloat16)
+    ref = ernie_student(heads=h).to(dev).to(torch.bfloat16)
     ref.load_state_dict({k: v.to(torch.bfloat16) for k, v in ours.state_dict().items()})
     ropt = torch.optim.AdamW(ref.parameters(), 1e-4, capturable=True)
 
@@ -141,24 +147,36 @@ def main():
     fallbacks = ops.fallbacks()
     t_torch = graph_time(step_torch, args.warmup, args.iters)
 
-    # attention backward alone: one layer's shapes
-    h = 6
-    qkv = torch.randn(b * l, 3 * h * 64, device=dev).to(torch.bfloat16)
+    # attention backward (and forward) alone: one layer's shapes
+    hd = ours.head_dim
+    qkv = torch.randn(b * l, 3 * h * hd, device=dev).to(torch.bfloat16)
     mask = keep.to(torch.uint8).contiguous()
-    do = torch.randn(b * l, h * 64, device=dev).to(torch.bfloat16)
+    do = torch.randn(b * l, h * hd, device=dev).to(torch.bfloat16)
     out, lse = ops.transformer.attention_forward_saved(qkv, mask, b, l, h)
     t_abwd = event_time(lambda: ops.transformer.attention_backward(qkv, mask, out, lse, do, b, l, h),
                         args.warmup, args.iters * 4)
-    q, k, v = (qkv.view(b, l, 3, h, 64)[:, :, i].transpose(1, 2).detach().requires_grad_(True) for i in range(3))
+    q, k, v = (qkv.view(b, l, 3, h, hd)[:, :, i].transpose(1, 2).detach().requires_grad_(True) for i in range(3))
     o = F.scaled_dot_product_attention(q, k, v, attn_mask=keep.view(b, 1, 1, l))
-    g_o = do.view(b, l, h, 64).transpose(1, 2)
+    g_o = do.view(b, l, h, hd).transpose(1, 2)
     t_sdpa = event_time(lambda: torch.autograd.grad(o, (q, k, v), g_o, retain_graph=True), args.warmup,
                         args.iters * 4)
-    name, limit = gpu_info()
-    print(json.dumps({"gpu": name, "power_limit": limit, "batch": b, "seq": l,
-                      "train_step_ms": {"ours": round(t_ours, 3), "torch_bf16": round(t_torch, 3)},
-                      "attention_bwd_us": {"ours": round(t_abwd * 1e3, 1), "sdpa": round(t_sdpa * 1e3, 1)},
-                      "fallbacks": fallbacks}))
+    res = {"gpu": None, "power_limit": None, "batch": b, "seq": l,
+           "train_step_ms": {"ours": round(t_ours, 3), "torch_bf16": round(t_torch, 3)},
+           "attention_bwd_us": {"ours": round(t_abwd * 1e3, 1), "sdpa": round(t_sdpa * 1e3, 1)},
+           "fallbacks": fallbacks}
+    if args.heads is not None:
+        ops.reset_fallbacks()
+        t_afwd = event_time(lambda: ops.transformer.attention_forward_saved(qkv, mask, b, l, h), args.warmup,
+                            args.iters * 4)
+        fallbacks.update(ops.fallbacks())
+        with torch.no_grad():
+            qd, kd, vd = (t.detach() for t in (q, k, v))
+            t_sfwd = event_time(lambda: F.scaled_dot_product_attention(qd, kd, vd, attn_mask=keep.view(b, 1, 1, l)),
+                                args.warmup, args.iters * 4)
+        res["heads"] = h
+        res["attention_fwd_us"] = {"ours": round(t_afwd * 1e3, 1), "sdpa": round(t_sfwd * 1e3, 1)}
+    res["gpu"], res["power_limit"] = gpu_info()
+    print(json.dumps(res))
 
 
 def bench_dropout(args, ours, opt, ref, ropt, ids, label, keep):
