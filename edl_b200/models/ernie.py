@@ -318,7 +318,7 @@ class ErnieStudent(ErnieEncoder):
     fp32 master copies; on CUDA each forward casts the matrices to bf16 and runs the training kernels of
     ops/transformer.py (attention and its backward, LayerNorm and embedding-LayerNorm with their backward, FFN1 with
     the GELU training epilogue and FFN2's gelu'-epilogue dgrad, residual gradients fused into the dgrad GEMMs).  On CPU
-    the forward is the encoder's float32 reference under torch autograd.
+    the same ops run their float32 references under torch autograd.
 
     Dropout (keyword-only ``hidden_dropout`` / ``attention_dropout``, default 0; only while ``self.training``) sits
     where BERT puts it.  Each site draws one (seed, offset) pair of 4 offset units from the default CUDA generator of
@@ -363,31 +363,12 @@ class ErnieStudent(ErnieEncoder):
                else position_ids.reshape(b, l).long())
         seg = torch.zeros_like(ids) if segment_ids is None else segment_ids.reshape(b, l).long()
         keep = (ids != 0) if input_mask is None else (input_mask.reshape(b, l) != 0)
-        c = self.hidden
-        hd, ad = (self.hidden_dropout, self.attention_dropout) if self.training else (0.0, 0.0)
-        if not self.word_emb.is_cuda:
-            if hd > 0.0 or ad > 0.0:
-                return self._forward_dropout_cpu(ids, pos, seg, keep, hd, ad)
-            return self._forward_reference(ids, pos, seg, lambda qkv: ops.attention(qkv, keep, b, l, self.heads,
-                                                                                    self.head_dim),
-                                           lambda x: x.view(b, l, c)[:, 0])
         mask = keep.to(torch.uint8).contiguous()
-        x = ops.embedding_layernorm_trainable(ids, pos, seg, self.word_emb, self.pos_emb, self.seg_emb, self.emb_ln_g,
-                                              self.emb_ln_b, self.eps, dropout_p=hd)
-        for lyr in self.layers:
-            h = ops.attention_block(x, lyr.qkv_w, lyr.qkv_b, lyr.out_w, lyr.out_b, mask, b, l, self.heads,
-                                    attn_dropout=ad, hidden_dropout=hd)
-            x = ops.layer_norm_trainable(h, lyr.ln1_g, lyr.ln1_b, self.eps)
-            h = ops.gelu_ffn(x, lyr.ffn1_w, lyr.ffn1_b, lyr.ffn2_w, lyr.ffn2_b, dropout_p=hd)
-            x = ops.layer_norm_trainable(h, lyr.ln2_g, lyr.ln2_b, self.eps)
-        bf = torch.bfloat16
-        pooled = torch.tanh(ops.linear_bf16(x.view(b, l, c)[:, 0], self.pool_w.to(bf), self.pool_b))
-        pooled = ops.dropout(pooled, hd)
-        n = self.num_labels
-        pad = max(CLS_PAD, -(-n // CLS_PAD) * CLS_PAD) - n          # TMA-describable classifier rows, as the encoder
-        logits = ops.linear_bf16(pooled, F.pad(self.cls_w, (0, 0, 0, pad)).to(bf), F.pad(self.cls_b, (0, pad)))
-        return logits[:, :n].float()
-
+        return self._train_forward(
+            ids, pos, seg,
+            lambda x, lyr, ad, hd: ops.attention_block(x, lyr.qkv_w, lyr.qkv_b, lyr.out_w, lyr.out_b, mask, b, l,
+                                                       self.heads, attn_dropout=ad, hidden_dropout=hd),
+            lambda x: x.view(b, l, self.hidden)[:, 0])                               # [B, C], row pitch L * C
 
     def forward_packed(self, ids, pos, seg, cu_seqlens, max_len, key_mask=None):
         """The training forward over packed sequences, with the arguments ``pack_sequences`` returns: ids / pos / seg
@@ -399,39 +380,34 @@ class ErnieStudent(ErnieEncoder):
         dev = self.word_emb.device
         ids, pos, seg, cu_seqlens = (t.to(dev) for t in (ids, pos, seg, cu_seqlens))
         key_mask = None if key_mask is None else key_mask.to(dev)
+        return self._train_forward(
+            ids, pos, seg,
+            lambda x, lyr, ad, hd: ops.attention_block_varlen(x, lyr.qkv_w, lyr.qkv_b, lyr.out_w, lyr.out_b,
+                                                              cu_seqlens, max_len, self.heads, key_mask,
+                                                              attn_dropout=ad, hidden_dropout=hd),
+            lambda x: x.index_select(0, cu_seqlens[:-1].long()))
+
+    def _train_forward(self, ids, pos, seg, attention_block, cls_rows):
+        """The layers of ``forward`` and ``forward_packed``: ``attention_block(x, layer, attention_dropout,
+        hidden_dropout)`` is one layer's attention sub-layer in the batch's layout, ``cls_rows(x)`` the [CLS] rows."""
         hd, ad = (self.hidden_dropout, self.attention_dropout) if self.training else (0.0, 0.0)
         x = ops.embedding_layernorm_trainable(ids, pos, seg, self.word_emb, self.pos_emb, self.seg_emb, self.emb_ln_g,
                                               self.emb_ln_b, self.eps, dropout_p=hd)
         for lyr in self.layers:
-            h = ops.attention_block_varlen(x, lyr.qkv_w, lyr.qkv_b, lyr.out_w, lyr.out_b, cu_seqlens, max_len,
-                                           self.heads, key_mask, attn_dropout=ad, hidden_dropout=hd)
+            h = attention_block(x, lyr, ad, hd)
             x = ops.layer_norm_trainable(h, lyr.ln1_g, lyr.ln1_b, self.eps)
             h = ops.gelu_ffn(x, lyr.ffn1_w, lyr.ffn1_b, lyr.ffn2_w, lyr.ffn2_b, dropout_p=hd)
             x = ops.layer_norm_trainable(h, lyr.ln2_g, lyr.ln2_b, self.eps)
-        cls = x.index_select(0, cu_seqlens[:-1].long())
+        cls = cls_rows(x)
         if not self.word_emb.is_cuda:
             pooled = ops.dropout(torch.tanh(F.linear(cls, self.pool_w, self.pool_b)), hd)
             return F.linear(pooled, self.cls_w, self.cls_b)
         bf = torch.bfloat16
         pooled = ops.dropout(torch.tanh(ops.linear_bf16(cls, self.pool_w.to(bf), self.pool_b)), hd)
         n = self.num_labels
-        pad = max(CLS_PAD, -(-n // CLS_PAD) * CLS_PAD) - n
+        pad = max(CLS_PAD, -(-n // CLS_PAD) * CLS_PAD) - n          # TMA-describable classifier rows, as the encoder
         logits = ops.linear_bf16(pooled, F.pad(self.cls_w, (0, 0, 0, pad)).to(bf), F.pad(self.cls_b, (0, pad)))
         return logits[:, :n].float()
-
-    def _forward_dropout_cpu(self, ids, pos, seg, keep, hd, ad):
-        """The float32 training forward on CPU with dropout at the documented sites (F.dropout masks)."""
-        b, l = ids.shape
-        x = ops.embedding_layernorm_trainable(ids, pos, seg, self.word_emb, self.pos_emb, self.seg_emb, self.emb_ln_g,
-                                              self.emb_ln_b, self.eps, dropout_p=hd)
-        for lyr in self.layers:
-            h = ops.attention_block(x, lyr.qkv_w, lyr.qkv_b, lyr.out_w, lyr.out_b, keep, b, l, self.heads,
-                                    attn_dropout=ad, hidden_dropout=hd)
-            x = ops.layer_norm_trainable(h, lyr.ln1_g, lyr.ln1_b, self.eps)
-            h = ops.gelu_ffn(x, lyr.ffn1_w, lyr.ffn1_b, lyr.ffn2_w, lyr.ffn2_b, dropout_p=hd)
-            x = ops.layer_norm_trainable(h, lyr.ln2_g, lyr.ln2_b, self.eps)
-        pooled = ops.dropout(torch.tanh(F.linear(x.view(b, l, self.hidden)[:, 0], self.pool_w, self.pool_b)), hd)
-        return F.linear(pooled, self.cls_w, self.cls_b)
 
 
 def ernie_base(num_labels=2):

@@ -90,50 +90,26 @@ def _draw(device, p):
     return native().dropout_draw(device.index if device.index is not None else torch.cuda.current_device(), p)
 
 
-def _fallback_z(drop, shape, device):
-    """Z = keep * scale (float32, ``shape``) of a drawn site over the flat indices of ``shape``: the kernels' mask for
-    the float32 fallback.  Needs the host values of the draw, so it cannot run under CUDA-graph capture."""
+def _fallback_z(drop, shape, device, strides=None):
+    """Z = keep * scale (float32, ``shape``) of a drawn site, element (k_0, k_1, ...) at the flat index
+    sum_d k_d strides_d (by default the strides of a contiguous ``shape``): the kernels' mask for the float32 fallback.
+    Needs the host values of the draw, so it cannot run under CUDA-graph capture."""
     if drop.captured:
         raise RuntimeError("dropout: the float32 fallback cannot be captured in a CUDA graph")
-    n = 1
-    for d in shape:
-        n *= d
-    keep = _keep(drop.seed, drop.offset, torch.arange(n, device=device), drop.threshold)
-    return (keep.float() * drop.scale).view(shape)
+    index = torch.zeros((), dtype=torch.int64, device=device)
+    for n, s in zip(shape, strides or torch.empty(shape, device="meta").stride()):
+        index = index.unsqueeze(-1) + torch.arange(n, device=device) * s
+    return _keep(drop.seed, drop.offset, index, drop.threshold).float() * drop.scale
 
 
-def _site_z(t, p, shape):
+def _site_z(t, p, shape, strides=None):
     """Z of a dropout site on the float32 reference path: None at p = 0, F.dropout's mask on CPU, the kernels' mask
-    (one generator draw) on CUDA."""
+    (one generator draw, flat indices as in ``_fallback_z``) on CUDA."""
     if p == 0.0:
         return None
     if not t.is_cuda:
         return torch.nn.functional.dropout(torch.ones(shape, dtype=torch.float32), p, True)
-    return _fallback_z(_draw(t.device, p), shape, t.device)
-
-
-def _varlen_site_z(t, p, cu_seqlens, max_len, heads):
-    """Z of the attention-probability site of a packed batch on the float32 reference path, as a list of per-sequence
-    [1, H, len_b, len_b] tensors: None at p = 0; on CUDA the kernels' mask (one generator draw), element (b, h, i, j)
-    at ((b H + h) 512 + i) 512 + j; on CPU the blocks [b, :, :len_b, :len_b] of one F.dropout mask of
-    [B, H, max_len, max_len]."""
-    if p == 0.0:
-        return None
-    cu = [int(v) for v in cu_seqlens.tolist()]
-    lens = [e - s for s, e in zip(cu[:-1], cu[1:])]
-    if not t.is_cuda:
-        z = torch.nn.functional.dropout(torch.ones((len(lens), heads, max_len, max_len)), p, True)
-        return [z[b:b + 1, :, :n, :n] for b, n in enumerate(lens)]
-    drop = _draw(t.device, p)
-    if drop.captured:
-        raise RuntimeError("dropout: the float32 fallback cannot be captured in a CUDA graph")
-    out = []
-    for b, n in enumerate(lens):
-        i = torch.arange(n, device=t.device, dtype=torch.int64)
-        h = torch.arange(heads, device=t.device, dtype=torch.int64)
-        idx = (((b * heads + h).view(-1, 1, 1) * _ATTN_MAX_LEN + i.view(1, -1, 1)) * _ATTN_MAX_LEN + i.view(1, 1, -1))
-        out.append((_keep(drop.seed, drop.offset, idx, drop.threshold).float() * drop.scale).unsqueeze(0))
-    return out
+    return _fallback_z(_draw(t.device, p), shape, t.device, strides)
 
 
 def _dropout_apply(x, drop):
@@ -214,12 +190,20 @@ def attention(qkv, mask, batch, seq_len, heads, head_dim=64, out=None):
         return attention_reference(qkv, mask, batch, seq_len, heads, head_dim)
     if out is None:
         out = torch.empty((batch * seq_len, heads * head_dim), device=qkv.device, dtype=torch.bfloat16)
-    m = None
-    if mask is not None:
-        m = mask if (mask.dtype == torch.uint8 and mask.is_contiguous()) else (mask != 0).to(torch.uint8).contiguous()
-    native().attention_fwd(qkv, m, out, batch, seq_len, heads, None, None)
+    native().attention_fwd(qkv, _mask_u8(mask), out, batch, seq_len, heads, None, None)
     count_launch()
     return out
+
+
+def _mask_u8(mask):
+    if mask is None:
+        return None
+    return mask if (mask.dtype == torch.uint8 and mask.is_contiguous()) else (mask != 0).to(torch.uint8).contiguous()
+
+
+def _cu_i32(cu_seqlens):
+    return cu_seqlens if (cu_seqlens.dtype == torch.int32 and cu_seqlens.is_contiguous()) else \
+        cu_seqlens.to(torch.int32).contiguous()
 
 
 # ----------------------------------------------------------------------------------------- variable-length attention
@@ -269,14 +253,9 @@ def attention_varlen(qkv, cu_seqlens, max_len, heads, key_mask=None, out=None):
     b = cu_seqlens.numel() - 1
     if out is None:
         out = torch.empty((qkv.shape[0], qkv.shape[1] // 3), device=qkv.device, dtype=torch.bfloat16)
-    cu = cu_seqlens if (cu_seqlens.dtype == torch.int32 and cu_seqlens.is_contiguous()) else \
-        cu_seqlens.to(torch.int32).contiguous()
-    km = None
-    if key_mask is not None:
-        km = key_mask if (key_mask.dtype == torch.uint8 and key_mask.is_contiguous()) else \
-            (key_mask != 0).to(torch.uint8).contiguous()
     maps = torch.empty(b * 256, device=qkv.device, dtype=torch.uint8)        # two 128-byte tensor maps per sequence
-    native().attention_varlen_fwd(qkv, cu, km, out, maps, int(max_len), heads, None, None)
+    native().attention_varlen_fwd(qkv, _cu_i32(cu_seqlens), _mask_u8(key_mask), out, maps, int(max_len), heads, None,
+                                  None)
     count_launch(2)
     return out
 
@@ -313,15 +292,16 @@ def layer_norm(x, gamma, beta, eps=1e-12, out=None):
 
 
 # ------------------------------------------------------------------------------------------- embedding + LayerNorm
-def _check_ids(ids, n, what):
-    if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= n):
-        raise IndexError("embedding_layernorm: %s out of range [0, %d): min %d, max %d"
-                         % (what, n, int(ids.min()), int(ids.max())))
+def _check_ids(ids, pos_ids, seg_ids, word, pos, seg):
+    for t, tab, what in ((ids, word, "input id"), (pos_ids, pos, "position id"), (seg_ids, seg, "segment id")):
+        n = tab.shape[0]
+        if t.numel() and (int(t.min()) < 0 or int(t.max()) >= n):
+            raise IndexError("embedding_layernorm: %s out of range [0, %d): min %d, max %d"
+                             % (what, n, int(t.min()), int(t.max())))
 
 
 def embedding_layernorm_reference(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps):
-    for t, tab, what in ((ids, word, "input id"), (pos_ids, pos, "position id"), (seg_ids, seg, "segment id")):
-        _check_ids(t, tab.shape[0], what)
+    _check_ids(ids, pos_ids, seg_ids, word, pos, seg)
     x = word.float()[ids.reshape(-1)] + pos.float()[pos_ids.reshape(-1)] + seg.float()[seg_ids.reshape(-1)]
     return layer_norm_reference(x, gamma, beta, eps).to(word.dtype)
 
@@ -349,20 +329,28 @@ def embedding_layernorm(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps=
     return _embedding_layernorm_kernel(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps, out, None)
 
 
-def _embedding_layernorm_kernel(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps, out, drop):
-    from . import native, count_launch
+def _embedding_launch(launch, ids, pos_ids, seg_ids, word, pos, seg):
+    """``launch(ids, pos_ids, seg_ids, err)``, an embedding-LayerNorm kernel, on the ids flattened to int64 on word's
+    device.  The kernel never reads outside a table; it raises the device flag ``err``, checked after the launch except
+    while a CUDA graph is being captured."""
+    from . import count_launch
 
-    rows = ids.numel()
-    if out is None:
-        out = torch.empty((rows, word.shape[1]), device=word.device, dtype=torch.bfloat16)
     err = torch.zeros(1, dtype=torch.int32, device=word.device)
     ids, pos_ids, seg_ids = (t.reshape(-1).to(word.device, torch.int64).contiguous() for t in (ids, pos_ids, seg_ids))
-    native().embedding_layernorm_fwd(ids, pos_ids, seg_ids, word, pos, seg, gamma.float().contiguous(),
-                                     beta.float().contiguous(), out, float(eps), err, drop)
+    launch(ids, pos_ids, seg_ids, err)
     count_launch()
     if not torch.cuda.is_current_stream_capturing() and int(err.item()) != 0:
-        for t, tab, what in ((ids, word, "input id"), (pos_ids, pos, "position id"), (seg_ids, seg, "segment id")):
-            _check_ids(t, tab.shape[0], what)
+        _check_ids(ids, pos_ids, seg_ids, word, pos, seg)
+
+
+def _embedding_layernorm_kernel(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta, eps, out, drop):
+    from . import native
+
+    if out is None:
+        out = torch.empty((ids.numel(), word.shape[1]), device=word.device, dtype=torch.bfloat16)
+    _embedding_launch(lambda i, p, s, err: native().embedding_layernorm_fwd(
+        i, p, s, word, pos, seg, gamma.float().contiguous(), beta.float().contiguous(), out, float(eps), err, drop),
+        ids, pos_ids, seg_ids, word, pos, seg)
     return out
 
 
@@ -406,21 +394,15 @@ def embedding_layernorm_e4m3(ids, pos_ids, seg_ids, word, pos, seg, gamma, beta,
     """``embedding_layernorm`` that also returns the block-scaled e4m3 copy of its output: (y, q, sa) as in
     ``layer_norm_e4m3``.  Out-of-range ids are handled as in ``embedding_layernorm`` (checked after the launch except
     under CUDA-graph capture)."""
-    from . import native, count_launch
+    from . import native
     from .fp8 import quantize_e4m3_blocks_reference
 
     if word.is_cuda and embedding_layernorm_e4m3_supported(word, pos, seg):
-        rows = ids.numel()
-        y = torch.empty((rows, word.shape[1]), device=word.device, dtype=torch.bfloat16)
+        y = torch.empty((ids.numel(), word.shape[1]), device=word.device, dtype=torch.bfloat16)
         q, sa = _quant_out(y)
-        err = torch.zeros(1, dtype=torch.int32, device=word.device)
-        ids, pos_ids, seg_ids = (t.reshape(-1).to(word.device, torch.int64).contiguous() for t in (ids, pos_ids, seg_ids))
-        native().embedding_layernorm_e4m3_fwd(ids, pos_ids, seg_ids, word, pos, seg, gamma.float().contiguous(),
-                                              beta.float().contiguous(), y, q, sa, float(eps), err)
-        count_launch()
-        if not torch.cuda.is_current_stream_capturing() and int(err.item()) != 0:
-            for t, tab, what in ((ids, word, "input id"), (pos_ids, pos, "position id"), (seg_ids, seg, "segment id")):
-                _check_ids(t, tab.shape[0], what)
+        _embedding_launch(lambda i, p, s, err: native().embedding_layernorm_e4m3_fwd(
+            i, p, s, word, pos, seg, gamma.float().contiguous(), beta.float().contiguous(), y, q, sa, float(eps), err),
+            ids, pos_ids, seg_ids, word, pos, seg)
         return y, q, sa
     if word.is_cuda:
         _count("embedding_layernorm_e4m3: no kernel for width %d %s: float32 math on the library"
@@ -465,11 +447,19 @@ def _wgrad_to(dy, x, w, sink):
     return None if g is None else g.to(w.dtype)
 
 
-def attention_train_supported(x, batch, seq_len, heads, head_dim=64) -> bool:
-    from . import native
+def _weight_bias_grads(needs, sinks, *layers):
+    """The gradients (weight, bias, weight, bias, ...) of linear layers y = x W^T + b given as (dy, x, W, b), each
+    delivered by ``_wgrad_to`` / ``_bias_grad`` through its sink in ``sinks`` when its flag in ``needs`` is set."""
+    g = []
+    for i, (dy, x, w, b) in enumerate(layers):
+        g.append(_wgrad_to(dy, x, w, sinks[2 * i]) if needs[2 * i] else None)
+        g.append(_bias_grad(dy.float().sum(0), b, sinks[2 * i + 1]) if needs[2 * i + 1] else None)
+    return g
 
-    return (x.is_cuda and x.dim() == 2 and x.shape[0] == batch * seq_len and x.shape[1] % 8 == 0
-            and native().attention_supported(batch, seq_len, heads, head_dim))
+
+def attention_train_supported(x, batch, seq_len, heads, head_dim=64) -> bool:
+    return (x.is_cuda and x.dim() == 2 and x.shape[1] % 8 == 0
+            and _Padded(None, batch, seq_len).supported(x.shape[0], heads, head_dim))
 
 
 def attention_forward_saved(qkv, mask, batch, seq_len, heads, drop=None):
@@ -529,22 +519,20 @@ def attention_varlen_backward(qkv, cu_seqlens, max_len, heads, key_mask, out, ls
     return dqkv
 
 
-def _mask_u8(mask, device):
-    if mask is None:
-        return None
-    return mask if (mask.dtype == torch.uint8 and mask.is_contiguous()) else (mask != 0).to(torch.uint8).contiguous()
-
-
-def _cu_i32(cu_seqlens):
-    return cu_seqlens if (cu_seqlens.dtype == torch.int32 and cu_seqlens.is_contiguous()) else \
-        cu_seqlens.to(torch.int32).contiguous()
-
-
+# A layout is everything the training attention knows about how sequences sit in the rows: the kernels' shape check,
+# the kernel forward / backward pair, the float32 reference, the fallback mask of the probability-dropout site and the
+# shape in a fallback message.  The other dropout sites are row-wise and do not depend on it.
 class _Padded:
-    """The padded layout of the attention kernels: ``mask`` uint8 [B, L] or None, rows b * L + i."""
+    """The padded layout [B, L]: rows b * L + i, ``mask`` [B, L] (nonzero = attend) or None."""
 
     def __init__(self, mask, batch, seq_len):
-        self.mask, self.batch, self.seq_len = mask, batch, seq_len
+        self.mask, self.batch, self.seq_len = _mask_u8(mask), batch, seq_len
+
+    def supported(self, rows, heads, head_dim):
+        from . import native
+
+        return rows == self.batch * self.seq_len and native().attention_supported(self.batch, self.seq_len, heads,
+                                                                                  head_dim)
 
     def forward(self, qkv, heads, drop):
         return attention_forward_saved(qkv, self.mask, self.batch, self.seq_len, heads, drop)
@@ -552,12 +540,30 @@ class _Padded:
     def backward(self, qkv, out, lse, dout, heads, drop):
         return attention_backward(qkv, self.mask, out, lse, dout, self.batch, self.seq_len, heads, drop)
 
+    def reference(self, qkv, heads, head_dim, drop_z):
+        return attention_reference(qkv, self.mask, self.batch, self.seq_len, heads, head_dim, drop_z)
+
+    def dropout_z(self, t, p, heads):
+        """Probability (b, h, i, j) at ((b H + h) L + i) L + j."""
+        return _site_z(t, p, (self.batch, heads, self.seq_len, self.seq_len))
+
+    def describe(self, rows, heads, width):
+        return "B %d, L %d, H %d, width %d" % (self.batch, self.seq_len, heads, width)
+
 
 class _Packed:
-    """Sequences packed back to back: ``cu_seqlens`` int32 [B + 1], host ``max_len``, ``key_mask`` uint8 [T] or None."""
+    """Sequences packed back to back: ``cu_seqlens`` [B + 1], host ``max_len``, ``key_mask`` [T] (nonzero = attend) or
+    None."""
 
     def __init__(self, cu_seqlens, max_len, key_mask):
-        self.cu_seqlens, self.max_len, self.key_mask = cu_seqlens, int(max_len), key_mask
+        self.cu_seqlens, self.max_len, self.key_mask = _cu_i32(cu_seqlens), int(max_len), _mask_u8(key_mask)
+
+    def supported(self, rows, heads, head_dim):
+        from . import native
+
+        cu = self.cu_seqlens
+        return (cu.is_cuda and cu.dim() == 1 and cu.numel() >= 2
+                and native().attention_varlen_supported(rows, cu.numel() - 1, self.max_len, heads, head_dim))
 
     def forward(self, qkv, heads, drop):
         return attention_varlen_forward_saved(qkv, self.cu_seqlens, self.max_len, heads, self.key_mask, drop)
@@ -565,26 +571,27 @@ class _Packed:
     def backward(self, qkv, out, lse, dout, heads, drop):
         return attention_varlen_backward(qkv, self.cu_seqlens, self.max_len, heads, self.key_mask, out, lse, dout, drop)
 
+    def reference(self, qkv, heads, head_dim, drop_z):
+        return attention_varlen_reference(qkv, self.cu_seqlens, self.max_len, heads, self.key_mask, drop_z)
+
+    def dropout_z(self, t, p, heads):
+        """Per sequence b a [1, H, len_b, len_b] block, probability (b, h, i, j) at ((b H + h) 512 + i) 512 + j; on
+        CPU the blocks of one F.dropout mask of [B, H, max_len, max_len]."""
+        m, k = self.max_len, _ATTN_MAX_LEN
+        z = _site_z(t, p, (self.cu_seqlens.numel() - 1, heads, m, m), (heads * k * k, k * k, k, 1))
+        if z is None:
+            return None
+        cu = self.cu_seqlens.tolist()
+        return [z[b:b + 1, :, :e - s, :e - s] for b, (s, e) in enumerate(zip(cu[:-1], cu[1:]))]
+
+    def describe(self, rows, heads, width):
+        return "T %d, B %d, max_len %d, H %d, width %d" % (rows, self.cu_seqlens.numel() - 1, self.max_len, heads,
+                                                           width)
+
 
 class _AttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, mask, batch, seq_len, heads, drop):
-        qkv = _bf16(qkv).contiguous()
-        out, lse = attention_forward_saved(qkv, mask, batch, seq_len, heads, drop)
-        ctx.save_for_backward(qkv, mask, out, lse)
-        ctx.shape, ctx.drop = (batch, seq_len, heads), drop
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        qkv, mask, out, lse = ctx.saved_tensors
-        return attention_backward(qkv, mask, out, lse, dout, *ctx.shape, ctx.drop), None, None, None, None, None
-
-
-class _AttentionVarlenFn(torch.autograd.Function):
-    @staticmethod
     def forward(ctx, qkv, layout, heads, drop):
-        qkv = _bf16(qkv).contiguous()
         out, lse = layout.forward(qkv, heads, drop)
         ctx.save_for_backward(qkv, out, lse)
         ctx.layout, ctx.heads, ctx.drop = layout, heads, drop
@@ -596,35 +603,33 @@ class _AttentionVarlenFn(torch.autograd.Function):
         return ctx.layout.backward(qkv, out, lse, dout, ctx.heads, ctx.drop), None, None, None
 
 
+def _attention_trainable(name, qkv, layout, heads, head_dim, dropout_p):
+    """``attention_trainable`` / ``attention_varlen_trainable`` over ``layout``; ``name`` heads the fallback message."""
+    p = _check_p(dropout_p)
+    if qkv.is_cuda and qkv.dim() == 2 and qkv.shape[1] == 3 * heads * head_dim:
+        q = _bf16(qkv).contiguous()
+        if q.data_ptr() % 16 == 0 and layout.supported(q.shape[0], heads, head_dim):
+            return _AttentionFn.apply(q, layout, heads, _draw(q.device, p) if p > 0.0 else None)
+    if qkv.is_cuda:
+        _count("%s: no training kernel for %s: float32 math on the library"
+               % (name, layout.describe(qkv.shape[0], heads, qkv.shape[-1])))
+    return layout.reference(qkv.float(), heads, head_dim, layout.dropout_z(qkv, p, heads))
+
+
 def attention_varlen_trainable(qkv, cu_seqlens, max_len, heads, key_mask=None, dropout_p=0.0):
     """``attention_varlen`` with a gradient, the packed sibling of ``attention_trainable``: the kernel path saves lse
     [H, T] and runs the packed backward of attention_bwd.cu.  ``qkv`` [T, 3 * H * D] with every row inside a sequence
     (cu_seqlens[-1] == T).  ``dropout_p``: dropout on the attention probabilities (one site, index
     ((b H + h) 512 + i) 512 + j).  On CPU, and for a shape the kernels do not take, ``attention_varlen_reference`` runs
     under autograd (counted through ``count_fallback`` on CUDA)."""
-    p = _check_p(dropout_p)
-    if qkv.is_cuda and attention_varlen_supported(_bf16(qkv).contiguous(), cu_seqlens, max_len, heads):
-        layout = _Packed(_cu_i32(cu_seqlens), max_len, _mask_u8(key_mask, qkv.device))
-        return _AttentionVarlenFn.apply(qkv, layout, heads, _draw(qkv.device, p) if p > 0.0 else None)
-    if qkv.is_cuda:
-        _count("attention_varlen: no training kernel for T %d, B %d, max_len %d, H %d, width %d: float32 math on the "
-               "library" % (qkv.shape[0], cu_seqlens.numel() - 1, max_len, heads, qkv.shape[-1]))
-    z = _varlen_site_z(qkv, p, cu_seqlens, max_len, heads)
-    return attention_varlen_reference(qkv.float(), cu_seqlens, max_len, heads, key_mask, z)
+    return _attention_trainable("attention_varlen", qkv, _Packed(cu_seqlens, max_len, key_mask), heads,
+                                qkv.shape[-1] // (3 * heads), dropout_p)
 
 
 def attention_trainable(qkv, mask, batch, seq_len, heads, head_dim=64, dropout_p=0.0):
     """``attention`` with a gradient: the kernel path saves lse and runs attention_bwd.cu in the backward.
     ``dropout_p``: dropout on the attention probabilities (one site, index ((b H + h) L + i) L + j)."""
-    p = _check_p(dropout_p)
-    if qkv.is_cuda and attention_supported(_bf16(qkv).contiguous(), batch, seq_len, heads, head_dim):
-        return _AttentionFn.apply(qkv, _mask_u8(mask, qkv.device), batch, seq_len, heads,
-                                  _draw(qkv.device, p) if p > 0.0 else None)
-    if qkv.is_cuda:
-        _count("attention: no training kernel for B %d, L %d, H %d, head dim %d: float32 math on the library"
-               % (batch, seq_len, heads, head_dim))
-    z = _site_z(qkv, p, (batch, heads, seq_len, seq_len))
-    return attention_reference(qkv.float(), mask, batch, seq_len, heads, head_dim, z)
+    return _attention_trainable("attention", qkv, _Padded(mask, batch, seq_len), heads, head_dim, dropout_p)
 
 
 class _AttentionBlockFn(torch.autograd.Function):
@@ -663,42 +668,30 @@ class _AttentionBlockFn(torch.autograd.Function):
         dctx = gemm_bf16(dhb, wo, b_mn_major=True)
         dqkv = ctx.layout.backward(qkv, o, lse, dctx, ctx.heads, ctx.drops[0])
         dx = gemm_bf16(dqkv, wq, b_mn_major=True, add=dh) if ctx.needs_input_grad[0] else None
-        s = ctx.sinks
-        g = [None] * 4
-        if ctx.needs_input_grad[1]:
-            g[0] = _wgrad_to(dqkv, x, qkv_w, s[0])
-        if ctx.needs_input_grad[2]:
-            g[1] = _bias_grad(dqkv.float().sum(0), qkv_b, s[1])
-        if ctx.needs_input_grad[3]:
-            g[2] = _wgrad_to(dhb, o, out_w, s[2])
-        if ctx.needs_input_grad[4]:
-            g[3] = _bias_grad(dhb.float().sum(0), out_b, s[3])
+        g = _weight_bias_grads(ctx.needs_input_grad[1:5], ctx.sinks, (dqkv, x, qkv_w, qkv_b), (dhb, o, out_w, out_b))
         return (dx, *g, None, None, None, None)
 
 
-def _block_reference(x, qkv_w, qkv_b, out_w, out_b, attend, hidden_z):
+def _attention_block(name, x, qkv_w, qkv_b, out_w, out_b, layout, heads, attn_dropout, hidden_dropout):
+    """``attention_block`` / ``attention_block_varlen`` over ``layout``; ``name`` heads the fallback message."""
+    from .gemm import _grad_sink
+
+    pa, ph = _check_p(attn_dropout), _check_p(hidden_dropout)
+    c = x.shape[-1]
+    if x.is_cuda and x.dim() == 2 and c % 8 == 0 and c % heads == 0 and layout.supported(x.shape[0], heads, c // heads):
+        sinks = tuple(_grad_sink(p) for p in (qkv_w, qkv_b, out_w, out_b))
+        drops = tuple(_draw(x.device, p) if p > 0.0 else None for p in (pa, ph))
+        return _AttentionBlockFn.apply(x, qkv_w, qkv_b, out_w, out_b, layout, heads, sinks, drops)
+    if x.is_cuda:
+        _count("%s: no kernel for %s: float32 math on the library" % (name, layout.describe(x.shape[0], heads, c)))
+    za = layout.dropout_z(x, pa, heads)
+    zh = _site_z(x, ph, (x.shape[0], c))
     f = torch.float32
     xf = x.float()
     qkv = torch.nn.functional.linear(xf, qkv_w.to(f), qkv_b.to(f))
-    h = torch.nn.functional.linear(attend(qkv), out_w.to(f), out_b.to(f))
-    return (h if hidden_z is None else hidden_z * h) + xf
-
-
-def attention_block_reference(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, attn_z=None, hidden_z=None):
-    """Float32 math of ``attention_block``; ``attn_z`` [B, H, L, L] / ``hidden_z`` [B * L, C]: dropout (keep * scale)
-    on the probabilities and on the output branch."""
-    d = qkv_w.shape[0] // (3 * heads)
-    return _block_reference(x, qkv_w, qkv_b, out_w, out_b,
-                            lambda qkv: attention_reference(qkv, mask, batch, seq_len, heads, d, attn_z), hidden_z)
-
-
-def attention_block_varlen_reference(x, qkv_w, qkv_b, out_w, out_b, cu_seqlens, max_len, heads, key_mask=None,
-                                     attn_z=None, hidden_z=None):
-    """Float32 math of ``attention_block_varlen``; ``attn_z``: per-sequence probability dropout as in
-    ``attention_varlen_reference``, ``hidden_z`` [T, C]: the output-branch dropout."""
-    return _block_reference(x, qkv_w, qkv_b, out_w, out_b,
-                            lambda qkv: attention_varlen_reference(qkv, cu_seqlens, max_len, heads, key_mask, attn_z),
-                            hidden_z)
+    h = torch.nn.functional.linear(layout.reference(qkv, heads, qkv.shape[1] // (3 * heads), za), out_w.to(f),
+                                   out_b.to(f))
+    return (h if zh is None else zh * h) + xf
 
 
 def attention_block(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, attn_dropout=0.0, hidden_dropout=0.0):
@@ -707,21 +700,8 @@ def attention_block(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, 
     bf16 on the kernel path (the input of the following LayerNorm); differentiable in x and the four parameters.
     ``attn_dropout`` drops attention probabilities, then ``hidden_dropout`` the output branch before the residual add
     (two sites, in that order; branch index row * C + col).  The kernels take head dim C / heads = 32 or 64."""
-    from .gemm import _grad_sink
-
-    pa, ph = _check_p(attn_dropout), _check_p(hidden_dropout)
-    c = x.shape[-1]
-    if x.is_cuda and c % 8 == 0 and c % heads == 0 and attention_train_supported(x, batch, seq_len, heads, c // heads):
-        sinks = tuple(_grad_sink(p) for p in (qkv_w, qkv_b, out_w, out_b))
-        drops = tuple(_draw(x.device, p) if p > 0.0 else None for p in (pa, ph))
-        return _AttentionBlockFn.apply(x, qkv_w, qkv_b, out_w, out_b,
-                                       _Padded(_mask_u8(mask, x.device), batch, seq_len), heads, sinks, drops)
-    if x.is_cuda:
-        _count("attention_block: no kernel for B %d, L %d, H %d, width %d: float32 math on the library"
-               % (batch, seq_len, heads, c))
-    za = _site_z(x, pa, (batch, heads, seq_len, seq_len))
-    zh = _site_z(x, ph, (x.shape[0], c))
-    return attention_block_reference(x, qkv_w, qkv_b, out_w, out_b, mask, batch, seq_len, heads, za, zh)
+    return _attention_block("attention_block", x, qkv_w, qkv_b, out_w, out_b, _Padded(mask, batch, seq_len), heads,
+                            attn_dropout, hidden_dropout)
 
 
 def attention_block_varlen(x, qkv_w, qkv_b, out_w, out_b, cu_seqlens, max_len, heads, key_mask=None,
@@ -732,29 +712,8 @@ def attention_block_varlen(x, qkv_w, qkv_b, out_w, out_b, cu_seqlens, max_len, h
     gradient and weight-gradient hand-off as the padded form; attention runs the packed kernels.  Dropout sites as in
     ``attention_block``: the probabilities at ((b H + h) 512 + i) 512 + j, then the output branch at row * C + col.
     Nothing reads back to the host on the kernel path."""
-    from .gemm import _grad_sink
-
-    pa, ph = _check_p(attn_dropout), _check_p(hidden_dropout)
-    c = x.shape[-1]
-    if (x.is_cuda and x.dim() == 2 and c % 8 == 0 and c % heads == 0 and cu_seqlens.is_cuda
-            and cu_seqlens.dim() == 1 and cu_seqlens.numel() >= 2):
-        from . import native
-
-        ok = native().attention_varlen_supported(x.shape[0], cu_seqlens.numel() - 1, int(max_len), heads, c // heads)
-    else:
-        ok = False
-    if ok:
-        sinks = tuple(_grad_sink(p) for p in (qkv_w, qkv_b, out_w, out_b))
-        drops = tuple(_draw(x.device, p) if p > 0.0 else None for p in (pa, ph))
-        layout = _Packed(_cu_i32(cu_seqlens), max_len, _mask_u8(key_mask, x.device))
-        return _AttentionBlockFn.apply(x, qkv_w, qkv_b, out_w, out_b, layout, heads, sinks, drops)
-    if x.is_cuda:
-        _count("attention_block_varlen: no kernel for T %d, B %d, max_len %d, H %d, width %d: float32 math on the "
-               "library" % (x.shape[0], cu_seqlens.numel() - 1, max_len, heads, c))
-    za = _varlen_site_z(x, pa, cu_seqlens, max_len, heads)
-    zh = _site_z(x, ph, (x.shape[0], c))
-    return attention_block_varlen_reference(x, qkv_w, qkv_b, out_w, out_b, cu_seqlens, max_len, heads, key_mask, za,
-                                            zh)
+    return _attention_block("attention_block_varlen", x, qkv_w, qkv_b, out_w, out_b,
+                            _Packed(cu_seqlens, max_len, key_mask), heads, attn_dropout, hidden_dropout)
 
 
 class _GeluFfnFn(torch.autograd.Function):
@@ -788,16 +747,7 @@ class _GeluFfnFn(torch.autograd.Function):
         dhb = dh if ctx.drop is None else _dropout_apply(dh, ctx.drop)
         du = gemm_bf16_gelu_grad(dhb, w2h, u)
         dx = gemm_bf16(du, w1h, b_mn_major=True, add=dh) if ctx.needs_input_grad[0] else None
-        s = ctx.sinks
-        g = [None] * 4
-        if ctx.needs_input_grad[1]:
-            g[0] = _wgrad_to(du, x, w1, s[0])
-        if ctx.needs_input_grad[2]:
-            g[1] = _bias_grad(du.float().sum(0), b1, s[1])
-        if ctx.needs_input_grad[3]:
-            g[2] = _wgrad_to(dhb, y, w2, s[2])
-        if ctx.needs_input_grad[4]:
-            g[3] = _bias_grad(dhb.float().sum(0), b2, s[3])
+        g = _weight_bias_grads(ctx.needs_input_grad[1:5], ctx.sinks, (du, x, w1, b1), (dhb, y, w2, b2))
         return (dx, *g, None, None)
 
 
@@ -839,12 +789,8 @@ def _ln_part(rows, c, device):
 class _LayerNormFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gamma, beta, eps):
-        from . import native, count_launch
-
         x = _bf16(x).contiguous()
-        y = torch.empty_like(x)
-        native().layernorm_fwd(x, gamma.float().contiguous(), beta.float().contiguous(), y, float(eps))
-        count_launch()
+        y = layer_norm(x, gamma, beta, eps)
         ctx.save_for_backward(x, gamma, beta)
         ctx.eps = eps
         return y
