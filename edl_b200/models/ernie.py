@@ -8,7 +8,8 @@ Inference only.
 On CUDA every layer runs on the package's own kernels: the wgmma GEMM (bias in the epilogue, the residual as its fused
 addend, GELU as a compile-time epilogue variant), the attention kernel reading Q / K / V in place from the QKV output,
 the LayerNorm and the embedding-sum + LayerNorm kernels.  The weight matrices are cast to bf16 once, at the first CUDA
-forward after a load or a move; biases and LayerNorm parameters stay fp32.  On CPU the same forward runs in float32
+forward after a move or any change of a parameter (``load_state_dict``, ``load_bert_state_dict``, an in-place update
+under ``no_grad``); biases and LayerNorm parameters stay fp32.  On CPU the same forward runs in float32
 PyTorch math (the reference the GPU path is tested against).
 
 ``forward_packed`` runs the same layers on a batch packed to its real tokens (``pack_sequences``) with the
@@ -99,6 +100,7 @@ class ErnieEncoder(nn.Module):
         self.cls_w, self.cls_b = mat(num_labels, hidden), vec(num_labels)
         self.requires_grad_(False)
         self._dev = None          # CUDA copies of the weights (bf16 matrices, fp32 vectors), built at first use
+        self._dev_key = None      # the _weights_key they were built from
         self._fp8 = False         # enable_fp8: the encoder's linear layers run block-scaled e4m3
 
     def enable_fp8(self, scaling="block"):
@@ -117,8 +119,19 @@ class ErnieEncoder(nn.Module):
         return super()._apply(fn, *args, **kwargs)
 
     # ------------------------------------------------------------------------------------------------- weights
+    def _weights_key(self):
+        """What the device copies are built from: the mode, the device and each parameter's storage and version.  An
+        in-place update (``load_state_dict``, or ``copy_`` / ``mul_`` under ``no_grad``) bumps the version.  The
+        parameters are read from the encoder's and its layers' own tables, which hold all of them: a quarter of the host
+        time of walking ``parameters()`` on every forward."""
+        return (self._fp8, self.word_emb.device) + tuple(
+            (p.data_ptr(), p._version) for mod in (self, *self.layers) for p in mod._parameters.values())
+
     def _device_weights(self):
-        if self._dev is None:
+        """The weights the forward reads (bf16 or e4m3 matrices, fp32 vectors), rebuilt whenever ``_weights_key``
+        changes, so a forward always serves the module's current parameters."""
+        key = self._weights_key()
+        if self._dev is None or self._dev_key != key:
             def m(t):
                 return t.detach().to(torch.bfloat16).contiguous()
 
@@ -144,6 +157,7 @@ class ErnieEncoder(nn.Module):
                     for lyr in self.layers],
                 "head": (m(self.pool_w), v(self.pool_b), m(cls_w), v(cls_b)),
             }
+            self._dev_key = key
         return self._dev
 
     def load_bert_state_dict(self, sd, strict=True):

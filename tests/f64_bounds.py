@@ -702,6 +702,46 @@ def fp8_tensor_tau(k):
     return math.ceil(k / 32) * 2.0 ** -12 + 3 * EPS32
 
 
+def check_gelu_e4m3(q, sa, pre, mag, k, what=""):
+    """The GELU -> e4m3 epilogue of the block-scaled GEMM (``fp8.gemm_fp8_gelu_e4m3``): e4m3 bytes ``q`` [M, N] and block
+    scales ``sa`` [ceil(N / 128), M] against float64 ``pre``, the dequantised product plus bias, and its magnitude ``mag``.
+
+    g = gelu(pre) in float64.  The kernel's g is within e_g = 1.13 fp8_tau(K) mag of it (GELU is 1.13-Lipschitz), plus
+    half a bf16 ulp (it quantises the bf16 g).  Each dequantised element q s is then within
+    e_g + 2^-4 (|g| + e_g) + 2^-10 s + 2^-22 (|g| + e_g) of g: half an e4m3 ulp (3 mantissa bits), half the subnormal
+    step 2^-9 s, and the fp32 division by s.  Each block's scale is exactly 1 when its g are all 0, and otherwise
+    448 s = its max|g| within the block's largest element bound.  Returns the worst element error / bound."""
+    n = q.shape[1]
+    e_g = 1.13 * fp8_tau(k) * mag
+    g64 = 0.5 * pre * (1 + torch.erf(pre / math.sqrt(2)))
+    e_g = e_g + 0.5 * ulp(g64.abs() + e_g, 8)
+    s = sa.t().repeat_interleave(128, 1)[:, :n].double()         # [M, N]: each element's block scale
+    deq = q.view(torch.float8_e4m3fn).double() * s
+    bound = e_g + 2.0 ** -4 * (g64.abs() + e_g) + 2.0 ** -10 * s + 2.0 ** -22 * (g64.abs() + e_g)
+    err = (deq - g64).abs()
+    ratio = float((err / bound).nan_to_num(float("inf")).max()) if err.numel() else 0.0
+    _log(what, ratio, None)
+    bad = ~(err <= bound)
+    if bad.any():
+        raise AssertionError("%s: %d elements out of bounds, first %s: q*s %r, g %r, bound %r, worst ratio %.3g" % (
+            what, int(bad.sum()), bad.nonzero()[0].tolist(), float(deq[bad][0]), float(g64[bad][0]),
+            float(bound[bad][0]), ratio))
+    nb = sa.shape[0]
+    pad = nb * 128 - n
+    gmax = F.pad(g64.abs(), (0, pad)).view(-1, nb, 128).amax(2)
+    emax = F.pad(bound, (0, pad)).view(-1, nb, 128).amax(2)
+    s_blk = sa.t().double()
+    zero = gmax == 0
+    if not torch.equal(s_blk[zero], torch.ones_like(s_blk[zero])):
+        raise AssertionError("%s: an all-zero block's scale is not 1" % what)
+    off = ~((448 * s_blk - gmax).abs() <= emax) & ~zero
+    if off.any():
+        r, b = off.nonzero()[0].tolist()
+        raise AssertionError("%s: %d block scales off, first row %d block %d: 448 s %r, max|g| %r" % (
+            what, int(off.sum()), r, b, float(448 * s_blk[r, b]), float(gmax[r, b])))
+    return ratio
+
+
 def dequant_a(q, sa):
     """float64 [M, K] = e4m3(q) * sa[k // 128, m]"""
     k = q.shape[1]

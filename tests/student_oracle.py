@@ -71,26 +71,28 @@ LOG2E = math.log2(math.e)
 
 
 # --------------------------------------------------------------------------------------------- float64 references
-def attention_ref(qkv, mask, b, l, h):
-    """(ref, slack) of the attention kernel's output [B * L, H * 64] in float64 (see tests/test_ernie_gpu.py's
-    docstring for the bound)."""
-    x = qkv.double().view(b, l, 3, h, 64)
-    q, k, v = (x[:, :, i].transpose(1, 2) for i in range(3))                       # [B, H, L, 64]
+def attention_ref(qkv, mask, b, l, h, d=64):
+    """(ref, slack) of the attention kernel's output [B * L, H * d] in float64 (see tests/test_ernie_gpu.py's docstring
+    for the bound, written there for d = 64: the scores take d / 16 + 1 fp32 roundings and the exponent scale is
+    c = log2(e) / sqrt(d), as in tests/test_attention_hd32_gpu.py)."""
+    x = qkv.double().view(b, l, 3, h, d)
+    q, k, v = (x[:, :, i].transpose(1, 2) for i in range(3))                       # [B, H, L, d]
     s = q @ k.transpose(-1, -2)
     smag = q.abs() @ k.abs().transpose(-1, -2)
     keep = (torch.ones(b, l, dtype=torch.bool, device=qkv.device) if mask is None else mask != 0).view(b, 1, 1, l)
-    c = LOG2E / 8
+    rd = math.sqrt(d)
+    c = LOG2E / rd
     cs = (s * c).masked_fill(~keep, float("-inf"))
     m = cs.amax(-1, keepdim=True)
-    w = torch.softmax((s / 8).masked_fill(~keep, float("-inf")), -1).nan_to_num(0.0)    # 2^(c s) = e^(s / 8)
+    w = torch.softmax((s / rd).masked_fill(~keep, float("-inf")), -1).nan_to_num(0.0)   # 2^(c s) = e^(s / sqrt d)
     ref = w @ v
     wv = w @ v.abs()
-    delta = c * 5 * EPS32 * smag + EPS32 * (cs.abs() + (cs - m).abs())
+    delta = c * (d / 16 + 1) * EPS32 * smag + EPS32 * (cs.abs() + (cs - m).abs())
     eps_j = 2.0 ** -8 + 2.0 ** -21 + 1.01 * math.log(2) * delta
     eps = eps_j.masked_fill(~keep, 0.0).amax(-1, keepdim=True)
     n_tiles = -(-l // 64)
     slack = (2 * eps / (1 - eps) + (8 * n_tiles + 32) * EPS32) * wv
-    flat = lambda t: t.transpose(1, 2).reshape(b * l, h * 64)                     # noqa: E731
+    flat = lambda t: t.transpose(1, 2).reshape(b * l, h * d)                      # noqa: E731
     return flat(ref), flat(slack)
 
 

@@ -16,7 +16,6 @@ k-block's four 32-deep MMAs (2^-12 each) on top of the fp32 roundings of the pro
 End to end: ernie_base in FP8 against its bf16 path and against the CPU emulation, packed against padded, a graph replay,
 and a CUDA teacher server."""
 import copy
-import math
 import threading
 
 import numpy as np
@@ -32,7 +31,7 @@ if not torch.cuda.is_available():
 from edl_b200 import ops  # noqa: E402
 from edl_b200.models import ernie, teacher_zoo  # noqa: E402
 from edl_b200.ops import fp8  # noqa: E402
-from f64_bounds import Guarded, check_bf16, dequant_a, dequant_w, fp8_tau, guarded, ulp  # noqa: E402
+from f64_bounds import Guarded, check_bf16, check_gelu_e4m3, dequant_a, dequant_w, fp8_tau, guarded  # noqa: E402
 from test_ernie_gpu import _inputs  # noqa: E402
 
 DEV = torch.device("cuda", 0)
@@ -164,28 +163,10 @@ def test_gelu_e4m3_epilogue_vs_float64(m, n, k):
 
     a64, w64 = dequant_a(qa, sa), dequant_w(qw, sw)
     pre = a64 @ w64.t() + bias.double()
-    bnd = fp8_tau(k) * (a64.abs() @ w64.abs().t() + bias.double().abs())
-    g64 = 0.5 * pre * (1 + torch.erf(pre / math.sqrt(2)))
-    e_g = 1.13 * bnd                                          # GELU is 1.13-Lipschitz
-    e_g = e_g + 0.5 * ulp(g64.abs() + e_g, 8)                 # the bf16 rounding of g
-    s = sa_out.t().repeat_interleave(128, 1)[:, :n].double()  # [M, N]: each element's block scale
-    deq = q.t.view(torch.float8_e4m3fn).double() * s
-    bound = e_g + 2.0 ** -4 * (g64.abs() + e_g) + 2.0 ** -10 * s + 2.0 ** -22 * (g64.abs() + e_g)
-    err = (deq - g64).abs()
-    bad = ~(err <= bound)
-    print("gelu e4m3 epilogue %d x %d x %d: worst |q s - g| / bound %.3f" % (m, n, k, float((err / bound).max())))
-    assert not bad.any(), "%d elements out of bounds, first %s: q*s %r, g %r, bound %r, worst ratio %.3g" % (
-        int(bad.sum()), bad.nonzero()[0].tolist(), float(deq[bad][0]), float(g64[bad][0]), float(bound[bad][0]),
-        float((err / bound).max()))
-    # each block: 448 s = its bf16 max|g| (1 for an all-zero block)
-    pad = nb * 128 - n
-    gmax = F.pad(g64.abs(), (0, pad)).view(m, nb, 128).amax(2)
-    emax = F.pad(bound, (0, pad)).view(m, nb, 128).amax(2)
-    s_blk = sa_out.t().double()
-    zero_blk = gmax == 0
-    assert torch.equal(s_blk[zero_blk], torch.ones_like(s_blk[zero_blk]))
-    assert bool(zero_blk[zero, 0])
-    assert ((448 * s_blk - gmax).abs() <= emax)[~zero_blk].all()
+    mag = a64.abs() @ w64.abs().t() + bias.double().abs()
+    assert not pre[zero, :128].any()                          # the all-zero block whose scale must be exactly 1
+    ratio = check_gelu_e4m3(q.t, sa_out, pre, mag, k, what="gelu e4m3 epilogue %d x %d x %d" % (m, n, k))
+    print("gelu e4m3 epilogue %d x %d x %d: worst |q s - g| / bound %.3f" % (m, n, k, ratio))
     # the op front end returns the same bytes and scales
     q2, s2 = fp8.gemm_fp8_gelu_e4m3(qa, sa, qw, sw, bias=bias)
     assert torch.equal(q2, q.t) and torch.equal(_bits(s2), _bits(sa_out))
